@@ -19,8 +19,8 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 FULL = (160, 192, 224)
-# first-step loss vs the fp32 CPU oracle, per convolution engine (measured on B200 at 160x192x224: bf16 1.8e-7, bf16x3 2.7e-7;
-# the moved image is within 1e-4 in every mode, the flow field is what bf16 operands cost: 6e-3 vs 1.4e-5 for bf16x3)
+# first-step loss vs the fp32 CPU oracle, per convolution engine (relative error; the flow field is what bf16 operands cost,
+# see tests/test_gpu_bf16_engine.py)
 PARITY_TOL = {"bf16": 1e-5, "bf16x3": 1e-5, "f32": 1e-5}
 METRIC = "vol-pairs/sec (3D 160x192x224 VxmDense int_steps=7 train step, NCC+Grad, Adam)"
 UNIT = "vol-pairs/s"
@@ -42,6 +42,9 @@ def parse():
     ap.add_argument("--no-parity", action="store_true", help="skip the first-step loss check against the CPU oracle and the bf16x3 parity-mode leg")
     ap.add_argument("--no-gpu-eager", action="store_true", help="skip the reference-torch-on-GPU (eager ATen / cuDNN) baseline leg")
     ap.add_argument("--no-c4", action="store_true", help="skip the BASELINE config 4 sweep (256^3 warp / VecInt GB/s)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed to DIR/<name>.npy (float32, at "
+                         "most 64 MB): loss, updated parameters, and every volume output at a fixed seeded sample of voxels")
     return ap.parse_args()
 
 
@@ -51,7 +54,7 @@ def load_peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sus=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sus=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sus=989.0, source="H100 SXM data sheet (700 W; dense bf16), not measured")
 
 
 # ------------------------------------------------------------------------------------------------
@@ -212,48 +215,8 @@ def reference_arm(args):
 
 
 # ------------------------------------------------------------------------------------------------
-# helper legs of the B200 arm
+# helper legs of the GPU arm
 # ------------------------------------------------------------------------------------------------
-CONV_SOURCES = ("conv3d_tc_s.cu", "conv3d_tc_s2.cu", "conv3d_tc_wgrad2.cu", "tc_common.cuh")
-
-
-def _strip_comments(text):
-    """C / CUDA source without comments and blank lines (string literals respected): the hash below identifies the CODE the
-    committed ncu pass measured — rewording a comment must not invalidate it, changing a statement must."""
-    out, i, n, in_str = [], 0, len(text), False
-    while i < n:
-        c = text[i]
-        if in_str:
-            out.append(c)
-            if c == "\\" and i + 1 < n:
-                out.append(text[i + 1]); i += 1
-            elif c == '"':
-                in_str = False
-        elif c == '"':
-            in_str = True; out.append(c)
-        elif text.startswith("//", i):
-            while i < n and text[i] != "\n":
-                i += 1
-            continue
-        elif text.startswith("/*", i):
-            j = text.find("*/", i + 2)
-            i = n if j < 0 else j + 2
-            continue
-        else:
-            out.append(c)
-        i += 1
-    return "\n".join(l.strip() for l in "".join(out).splitlines() if l.strip())
-
-
-def conv_source_hash():
-    import hashlib
-    h = hashlib.sha256()
-    for f in CONV_SOURCES:
-        with open(os.path.join(ROOT, "voxelmorph_b200", "csrc", f), "r") as fh:
-            h.update(_strip_comments(fh.read()).encode())
-    return h.hexdigest()[:16]
-
-
 def default_cfg(shape):
     return dict(inshape=tuple(shape), nb_unet_features=None, nb_unet_levels=None, unet_feat_mult=1, nb_unet_conv_per_level=1,
                 int_steps=7, int_downsize=2, bidir=False, use_probs=False, src_feats=1, trg_feats=1, unet_half_res=False)
@@ -337,7 +300,7 @@ def engine_leg(vxm, dev, shape, pairs_dev, engine, steps=10, warmup=3):
 
 
 # ------------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ------------------------------------------------------------------------------------------------
 def b200_arm(args):
     import numpy as np
@@ -346,7 +309,7 @@ def b200_arm(args):
     from voxelmorph_b200 import dist as vdist
 
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device (the B200 path has no CPU fallback; use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device (the GPU path has no CPU fallback; use --impl reference for the CPU arm)")
     os.environ["VXM_B200_TRANSPARENT_DP"] = "0"     # bench drives its one allreduce per step itself (inside the CUDA graph)
     world, rank, local = vdist.init_from_env()
     if world != args.gpus:
@@ -407,11 +370,24 @@ def b200_arm(args):
     pairs_dev = [tuple(x.to(dev) for x in smp) for smp in pairs_host]
     dice = vxm.losses.Dice().loss
 
+    # --dump-outputs: every step copies its outputs into persistent buffers (allocated by the first, eager step; the copies
+    # are part of the captured graph).  Holding the step's own output tensors instead would keep its autograd graph alive.
+    last = {}
+
+    def keep(**outs):
+        if args.dump_outputs:
+            for k, v in outs.items():
+                if k not in last:
+                    last[k] = torch.empty_like(v, requires_grad=False)
+                last[k].copy_(v.detach())
+
     def forward_loss(*inp):
         if semi:
             y, pre, yseg = model(inp[0], inp[1], inp[2])
+            keep(moved=y, flow=pre, moved_seg=yseg)
             return ncc(inp[1], y) + 0.01 * grad(None, pre) + 0.01 * dice(inp[3], yseg)
         y, flow = model(inp[0], inp[1])
+        keep(moved=y, flow=flow)
         return ncc(inp[1], y) + 0.01 * grad(None, flow)
     loss_host = torch.empty((), dtype=torch.float32).pin_memory()
 
@@ -477,11 +453,14 @@ def b200_arm(args):
     barrier()
     t_host0 = time.time()
     e0.record()
+    loss = None
     for i in range(K):
-        step(*pairs_dev[i % NPAIR])
+        loss = step(*pairs_dev[i % NPAIR])
     e1.record()
     barrier()
     t_host1 = time.time()
+    if args.dump_outputs and rank == 0 and K > 0:
+        dump_outputs(args.dump_outputs, loss, last, opt.fp.flat)
     ms = e0.elapsed_time(e1)
     launches = (launches_per_step * K) if graphed else (vxm._lib.launch_count() - n0)
     ms = vdist.max_over_ranks(ms, dev)
@@ -590,20 +569,8 @@ def b200_arm(args):
     _, flops_step = conv_flops_per_step(shape)
     ach = flops_step / (conv_total_ms * 1e-3) / 1e12
     engine = ops.conv_engine()
-    # DRAM traffic of the conv family per step: taken from the committed ncu pass over this same command
-    # (profiles/r1_traffic.json; ncu cannot run inside a timed bench), valid for the full-size bf16 workload only.
-    traffic, traffic_src = None, None
-    tj = os.path.join(ROOT, "profiles", "r2_traffic.json")
-    if engine == "bf16" and tuple(shape) == (160, 192, 224) and os.path.exists(tj):
-        with open(tj) as f:
-            tinfo = json.load(f)
-        if tinfo.get("conv_source_sha") == conv_source_hash():
-            traffic, traffic_src = tinfo["conv_dram_mbytes_per_step"] * 1e6, tinfo["source"]
-        else:
-            traffic_src = ("stale: profiles/r2_traffic.json was captured for conv sources %s, the library was built from %s"
-                           % (tinfo.get("conv_source_sha"), conv_source_hash()))
-    roofline = dict(bound="tensor", kernel="conv3d k3 fwd+dgrad+wgrad, all 12 layers (%s)" % ("tcgen05 bf16 implicit GEMM" if engine == "bf16" else "fp32 FFMA engine"),
-                    achieved=ach, peak=peaks["tf_burst"], unit="TFLOP/s", frac=ach / peaks["tf_burst"], traffic=traffic, traffic_unit="bytes per step (all conv launches)", traffic_source=traffic_src,
+    roofline = dict(bound="tensor", kernel="conv3d k3 fwd+dgrad+wgrad, all 12 layers (%s)" % ("wgmma bf16 implicit GEMM" if engine == "bf16" else "fp32 FFMA engine"),
+                    achieved=ach, peak=peaks["tf_burst"], unit="TFLOP/s", frac=ach / peaks["tf_burst"],
                     peak_source=peaks["source"] + ", burst bf16 (the conv launches are replayed in isolation behind a sleep, not inside the long step)",
                     frac_of_sustained=ach / peaks["tf_sus"], ms_per_step=conv_total_ms, conv_launches=n_conv_launches,
                     share_of_step=conv_total_ms / (ms / K), flops_per_step=flops_step)
@@ -613,7 +580,7 @@ def b200_arm(args):
     if not args.no_parity and engine == "bf16" and world == 1 and not semi:
         try:
             parity_mode = engine_leg(vxm, dev, shape, pairs_dev, "bf16x3")
-            parity_mode["note"] = ("same step with the split-precision tensor-core forward (3 tcgen05 passes per layer, flow / moved image "
+            parity_mode["note"] = ("same step with the split-precision tensor-core forward (3 wgmma passes per layer, flow / moved image "
                                    "within 1e-4 of the fp32 reference: tests/test_gpu_bf16_engine.py); backward on bf16 operands")
         except Exception as e:  # noqa: BLE001
             parity_mode = dict(error=str(e)[:300])
@@ -647,7 +614,7 @@ def b200_arm(args):
                             global_batch=world, parallelism="dp%d (one flat-gradient allreduce per step)" % world,
                             conv_engine=engine, cuda_graph=graphed,
                             l2="inputs rotate over %d resident pairs; per-step working set ~%.1f GB of full-resolution "
-                               "activations >> 126 MB L2, so no explicit flush" % (NPAIR, act_gb)),
+                               "activations >> 50 MB L2, so no explicit flush" % (NPAIR, act_gb)),
                 clocks=clk, e2e=e2e, gpu_launches=int(launches), launches_per_step=launches / K,
                 roofline=roofline, kernels=kernels, cpu_baseline=cpu, parity_check=parity, parity_mode=parity_mode,
                 gpu_eager_baseline=gpu_eager, c4_sweep=c4)
@@ -655,10 +622,39 @@ def b200_arm(args):
     _leave(world, rank)
 
 
+DUMP_BYTES = 64 << 20      # --dump-outputs writes at most this much in all
+DUMP_SAMPLE = 1 << 20      # and at most this many voxels of a volume output (fixed seed: the same voxels every run)
+
+
+def dump_outputs(out_dir, loss, last, params):
+    """Write the last timed step's results as float32 .npy files: the loss, the updated parameters (all of them), and, of
+    every volume output, all channels at a fixed seeded sample of voxels.  The volume outputs share what DUMP_BYTES leaves
+    after the loss and the parameters equally; an output with C rows (batch x channels) gets at most share / (4 C) voxels."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = dict(loss=loss.detach().float().reshape(1), params=params.detach().float())
+    fixed = sum(4 * t.numel() for t in arrays.values())
+    share = (DUMP_BYTES - fixed) // max(1, len(last))
+    for name, t in last.items():
+        t = t.detach().float()
+        flat = t.reshape(t.shape[0] * t.shape[1], -1)                  # (batch * channels, voxels)
+        rows, nvox = flat.shape
+        nkeep = min(nvox, DUMP_SAMPLE, share // (4 * rows))
+        if nkeep < nvox:
+            idx = np.sort(np.random.RandomState(0).choice(nvox, nkeep, replace=False))
+            flat = flat[:, torch.from_numpy(idx).to(flat.device)]
+        arrays[name] = flat
+    total = sum(4 * t.numel() for t in arrays.values())
+    assert total <= DUMP_BYTES, "dump of %d bytes exceeds %d" % (total, DUMP_BYTES)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.cpu().numpy().astype(np.float32))
+
+
 def _leave(world, rank=None):
     """End of a rank's work.  Under torchrun every rank leaves with os._exit(0), rank 0 last: the captured CUDA graph
     still holds NCCL kernels, and tearing the process group down with it alive (destroy_process_group / interpreter
-    shutdown) blocked both ranks after the JSON line had been printed (2 x B200, round 1).  The ranks meet on the
+    shutdown) blocked both ranks after the JSON line had been printed.  The ranks meet on the
     rendezvous store (no collective): rank 0 posts `bench_done`, the others acknowledge, then everybody exits."""
     sys.stdout.flush()
     sys.stderr.flush()

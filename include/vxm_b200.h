@@ -1,5 +1,5 @@
 /*
- * vxm_b200 — C ABI of the B200-native VxmDense registration path.
+ * vxm_b200 — C ABI of the H100-native (sm_90a) VxmDense registration path.
  *
  * Drop-in boundary.  The reference (voxelmorph/voxelmorph, torch backend) has no FFI
  * layer of its own: its hot path bottoms out in PyTorch operators (F.grid_sample,
@@ -48,7 +48,7 @@ extern "C" {
 #define VXM_ARITH_FAST 2
 
 const char* vxm_last_error(void);
-/* library / build identification ("vxm_b200 <version> sm_100a") */
+/* library / build identification ("vxm_b200 <version> sm_90a") */
 const char* vxm_version(void);
 /* number of kernel launches issued through this library by the calling process so far */
 uint64_t vxm_launch_count(void);
@@ -152,9 +152,9 @@ int vxm_conv3d_bwd_f32(const float* grad_y, const float* y, const float* x, cons
                        int B, int Cin, int Cout, int D, int H, int W, int kd,
                        float leaky_slope, void* stream);
 
-/* ---- Conv3d k=3 on tcgen05 tensor cores (bf16 operands, fp32 TMEM accumulation), channels-last ----
+/* ---- Conv3d k=3 on the tensor cores (wgmma, bf16 operands, fp32 register accumulation), channels-last ----
  * The throughput engine for reference networks.py:299-304 / :211,257; forward and dgrad share one kernel.
- * Activations are bf16 NDHWC (B,D,H,W,C).  Weights are pre-packed by vxm_conv3d_tc_pack into the UMMA
+ * Activations are bf16 NDHWC (B,D,H,W,C).  Weights are pre-packed by vxm_conv3d_tc_pack into the wgmma
  * canonical K-major layout [tap][K/16][2][N][8] (bf16); `transposed` = 1 packs the dgrad operator
  * (channel roles swapped, taps flipped).  np = MMA N (16 or 32) >= number of output channels. */
 size_t vxm_conv3d_tc_packed_bytes(int cin_eff, int np, int kd);
@@ -201,11 +201,11 @@ int vxm_conv3d_tcs_pack_multi(const void* descs_dev, int ndesc, int total, void*
 int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                        int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
                        float slope, void* out2, int csplit, void* stream);
-/* variant of the above with two alternating MMA-issuing warps (8-row tiles only: Ca + Cb in {8,16,32,48}, padded
- * Cout in {16,32}); same arguments, weights packed by vxm_conv3d_tcs_pack.  Selected with VXM_B200_TCS2=1. */
+/* same as vxm_conv3d_tcs_fwd (kept for callers of the former two-issuer variant; the kernel behind vxm_conv3d_tcs_fwd
+ * already runs two MMA warpgroups) */
 int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
-                       int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                       float slope, void* out2, int csplit, void* stream);
+                        int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
+                        float slope, void* out2, int csplit, void* stream);
 /* Split-precision ("bf16x3") passes of the same kernel — the in-tolerance tensor-core mode (reference layer:
  * voxelmorph/torch/networks.py:290-305 in fp32).  Every operand is a bf16 pair hi + lo (16 mantissa bits); a layer is
  * three launches that accumulate  x_lo*w_hi + x_hi*w_lo + x_hi*w_hi  in fp32:
@@ -227,7 +227,7 @@ int vxm_conv3d_tc_wgrad(const void* xa, const void* xb, const float* const* xf, 
                         int nplanar_x, const void* gz, const float* const* gf, const long long* gf_bstride,
                         int nplanar_g, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
                         int Ca, int Cb, int up, int Cin_real, int Cg, int Cout_real, int kd, int accumulate, void* stream);
-/* Deferred reduction of the weight gradient (channels-last bf16 sources only): `_partial` launches the tcgen05 kernel(s) of
+/* Deferred reduction of the weight gradient (channels-last bf16 sources only): `_partial` launches the wgmma kernel(s) of
  * one layer into caller-provided workspace (`work_used` bytes of it are then owned by this layer until the flush) and
  * appends the pending reductions to a HOST array of descriptors (vxm_conv3d_tc_wgrad2_desc_bytes() each, at most
  * vxm_conv3d_tc_wgrad2_max_pending()); `_flush` reduces every pending layer in ONE launch, in a fixed order

@@ -2,7 +2,7 @@
 
 TEST INFRASTRUCTURE ONLY.  Everything is generated with numpy's PCG64 streams and exact
 float32 arithmetic (adds / multiplies only, no transcendental functions), so the same
-arrays are reproduced bit for bit on the GPU box.
+arrays are reproduced bit for bit on any machine.
 """
 import numpy as np
 

@@ -1,10 +1,9 @@
-"""Freeze outputs of the UNMODIFIED reference (voxelmorph @ /root/reference, torch CPU fp32)
+"""Freeze outputs of the UNMODIFIED reference (voxelmorph at $VXM_REFERENCE_ROOT, torch CPU fp32)
 into tests/golden/*.npz.
 
-TEST INFRASTRUCTURE ONLY.  Run in the build container (the reference tree does not exist on
-the GPU box):
+TEST INFRASTRUCTURE ONLY (needs the reference tree, see oracle/ref_import.py):
 
-    python -m oracle.make_golden
+    VXM_REFERENCE_ROOT=<reference checkout> python -m oracle.make_golden
 
 Inputs come from oracle/cases.py (seeded, exact arithmetic) and are stored beside the
 outputs.  The fixtures pin (i) the restatements in oracle/spec_np.py and oracle/ref_torch.py
@@ -29,6 +28,15 @@ SMALL_FEATS = [[4, 8, 8, 8], [8, 8, 8, 8, 8, 4, 4]]
 
 def t(x):
     return torch.from_numpy(np.ascontiguousarray(x))
+
+
+def save_split(name, out, parts=2):
+    """tests/golden/<name>.npz and <name>.part2.npz ...: the arrays dealt round-robin over `parts` files, each well under
+    1 MB (tests/conftest.py's `golden` fixture merges them)."""
+    keys = list(out)
+    for p in range(parts):
+        fn = name + (".npz" if p == 0 else ".part%d.npz" % (p + 1))
+        np.savez_compressed(os.path.join(GOLD, fn), **{k: out[k] for k in keys[p::parts]})
 
 
 def sha(a):
@@ -86,7 +94,7 @@ def main():
                resize_up_odd=vxm.layers.ResizeTransform(0.5, 3)(t(odd)).numpy(),
                resize2_down=vxm.layers.ResizeTransform(2, 2)(t(flow2)).numpy(),
                resize2_up=vxm.layers.ResizeTransform(0.5, 2)(t(flow2)).numpy())
-    np.savez_compressed(os.path.join(GOLD, "layers.npz"), **out)
+    save_split("layers", out)
 
     # ---- losses (values and autograd gradients w.r.t. y_pred) ----------------------------
     out = {}
@@ -168,7 +176,7 @@ def main():
         opt.step()
         for k in ("flow.weight", "unet_model.encoder.0.0.main.weight"):
             out["%s/after/%s" % (name, k)] = dict(model.named_parameters())[k].detach().numpy().copy()
-    np.savez_compressed(os.path.join(GOLD, "vxmdense.npz"), **out)
+    save_split("vxmdense", out)
 
     # ---- full-size nearest-neighbour label warp: digest only (inputs regenerate exactly) ---
     full = (160, 192, 224)
@@ -181,7 +189,7 @@ def main():
                    linear_full_sum=float(lin.astype(np.float64).sum()),
                    linear_full_abs_sum=float(np.abs(lin).astype(np.float64).sum()))
     # a crop of the real scan / segmentation shipped with the reference (data, not code)
-    d = "/root/reference/data"
+    d = os.path.join(ref_import.REFERENCE_ROOT, "data")
     if os.path.isfile(os.path.join(d, "test_scan.npz")):
         seg = np.load(os.path.join(d, "test_scan.npz"))["seg"].astype(np.float32)
         crop = seg[48:80, 64:112, 80:120][None, None]

@@ -1,7 +1,7 @@
 """Freeze the behaviour of the reference generators (voxelmorph/generators.py) for tests/test_generators.py.
 
-TEST INFRASTRUCTURE ONLY; runs in the build container where /root/reference exists:
-    python -m oracle.make_golden_generators
+TEST INFRASTRUCTURE ONLY (needs the reference tree, see oracle/ref_import.py):
+    VXM_REFERENCE_ROOT=<reference checkout> python -m oracle.make_golden_generators
 writes tests/golden/generators.json: for every case of tests/test_generators.CASES the shapes and sums of six consecutive
 yields of the UNMODIFIED reference generator on the synthetic dataset of `make_dataset` (np.random seeded)."""
 import json

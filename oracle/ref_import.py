@@ -1,10 +1,8 @@
-"""Import the *unmodified* reference (voxelmorph @ /root/reference) on CPU.
+"""Import the *unmodified* reference (voxelmorph, checked out at $VXM_REFERENCE_ROOT) on CPU.
 
-TEST INFRASTRUCTURE ONLY, and only usable in the build container: `/root/reference`
-does not exist on the GPU box.  It is used by `oracle/make_golden.py` to freeze the
-reference's outputs into `tests/golden/` and by `tests/test_oracle_vs_reference.py`
-(skipped when the reference tree is absent) to pin the restatements in
-`oracle/spec_np.py` / `oracle/ref_torch.py`.
+TEST INFRASTRUCTURE ONLY: used by `oracle/make_golden*.py` to freeze the reference's outputs into
+`tests/golden/`, against which the tests pin the restatements in `oracle/spec_np.py` / `oracle/ref_torch.py`.
+Nothing in the test suite imports the reference itself.
 
 The reference hard-imports three packages that are absent from this image and
 irrelevant to the torch hot path (`neurite`, `skimage.measure`, `pystrum`):
@@ -17,17 +15,17 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get("VXM_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("VXM_REFERENCE_ROOT", "")
 
 
 def available() -> bool:
-    return os.path.isdir(os.path.join(REFERENCE_ROOT, "voxelmorph", "torch"))
+    return bool(REFERENCE_ROOT) and os.path.isdir(os.path.join(REFERENCE_ROOT, "voxelmorph", "torch"))
 
 
 def import_reference():
     """Return the reference `voxelmorph` module (torch backend)."""
     if not available():
-        raise RuntimeError("reference tree not present at %s" % REFERENCE_ROOT)
+        raise RuntimeError("reference tree not found: set VXM_REFERENCE_ROOT to a checkout of the reference (now %r)" % REFERENCE_ROOT)
     os.environ["VXM_BACKEND"] = "pytorch"
     os.environ["NEURITE_BACKEND"] = "pytorch"
     if "voxelmorph" in sys.modules and getattr(sys.modules["voxelmorph"], "__file__", "").startswith(REFERENCE_ROOT):

@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
 
 
 @pytest.fixture(scope="session")
@@ -23,8 +23,13 @@ def golden():
             self._c = {}
 
         def __call__(self, name):
+            # a fixture may be stored in several files (name.npz, name.part2.npz, ...) to keep every file small
             if name not in self._c:
-                self._c[name] = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+                d = {}
+                for f in sorted(os.listdir(GOLDEN)):
+                    if f == name + ".npz" or (f.startswith(name + ".part") and f.endswith(".npz")):
+                        d.update(np.load(os.path.join(GOLDEN, f)))
+                self._c[name] = d
             return self._c[name]
     return G()
 

@@ -1,7 +1,7 @@
 """CPU tests of the host-side data feed (voxelmorph_b200/generators.py, "next" row N1) against the reference generators:
-same yield structure, shapes, values and the same sequence of np.random draws.  The live comparison imports the unmodified
-reference (build container only; skipped where /root/reference is absent); the frozen expectations in
-tests/golden/generators.json (written by oracle/make_golden_generators.py from the reference) travel everywhere."""
+same yield structure, shapes, values and the same sequence of np.random draws, checked against outputs of the unmodified
+reference frozen into tests/golden/ (generators.json by oracle/make_golden_generators.py, reference_live.npz by
+oracle/make_golden_live.py)."""
 import json
 import os
 
@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 
 from conftest import ROOT
-from oracle import ref_import
 
 GOLDEN = os.path.join(ROOT, "tests", "golden", "generators.json")
 
@@ -68,6 +67,14 @@ def run_case(mod, files, case, steps=6, seed=7):
     return [next(gen) for _ in range(steps)]
 
 
+def flatten(item, out):
+    """Nested lists / tuples of arrays -> arrays appended to `out` in order; returns the nesting as a string."""
+    if isinstance(item, (list, tuple)):
+        return "[" + ",".join(flatten(x, out) for x in item) + "]"
+    out.append(np.asarray(item))
+    return "a"
+
+
 def assert_same(a, b):
     if isinstance(a, (list, tuple)):
         assert isinstance(b, (list, tuple)) and len(a) == len(b)
@@ -88,15 +95,17 @@ def test_matches_frozen_reference_behaviour(tmp_path, name):
     assert got == gold[name]
 
 
-@pytest.mark.skipif(not ref_import.available(), reason="reference tree not present")
 @pytest.mark.parametrize("name", sorted(CASES))
-def test_matches_live_reference(tmp_path, name):
+def test_matches_live_reference(tmp_path, golden, name):
+    """Every yielded array against the reference generators' own output on the same files and seed (frozen by
+    oracle/make_golden_live.py)."""
     from voxelmorph_b200 import generators
-    vxm_ref = ref_import.import_reference()
+    ref = golden("reference_live")
     files = make_dataset(tmp_path)
-    ours = run_case(generators, files, CASES[name])
-    ref = run_case(vxm_ref.generators, files, CASES[name])
-    assert_same(ours, ref)
+    arrs = []
+    structure = flatten(run_case(generators, files, CASES[name]), arrs)
+    assert structure == json.loads(str(ref["generators/structure"]))[name]
+    assert_same(arrs, [ref["generators/%s/%d" % (name, i)] for i in range(len(arrs))])
 
 
 def test_decode_once_float32_and_views(tmp_path):

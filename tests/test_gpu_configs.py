@@ -78,7 +78,7 @@ def test_config5_semisupervised_composition(vxm, cuda):
     warped_c = ref_torch.spatial_transform(t(seg_m).double(), seg_flow_c)
     loss_c = ref_torch.dice_loss(t(seg_f).double(), warped_c)
     loss_c.backward()
-    # --- B200 path
+    # --- GPU path
     fg = t(pos_flow).to(cuda).requires_grad_(True)
     seg_flow_g = vxm.layers.ResizeTransform(2, 3)(fg)
     warped_g = vxm.layers.SpatialTransformer(half)(t(seg_m).to(cuda), seg_flow_g)

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 (bf16 operands, fp32 TMEM accumulation) convolution engine against the CPU
+"""GPU parity tests of the wgmma (bf16 operands, fp32 accumulation) convolution engine against the CPU
 oracle evaluated on the SAME bf16-rounded operands (fp64 accumulation).  Tolerances: bf16-output paths 1e-2 of
 max|ref| (output rounding is 2^-9 relative), fp32-output paths 1e-4."""
 import numpy as np
@@ -265,10 +265,10 @@ def test_tct_cin64(tc, cuda, variant):
     assert rel_err(tc.from_ndhwc(out).cpu(), ref) <= 1e-2
 
 
-# ---- round 2: TMA tile staging and the specialised epilogues are pure re-implementations: results must not change ----
+# ---- TMA tile staging and the specialised epilogues are pure re-implementations: results must not change ----
 
 @pytest.mark.parametrize("shape,Ca,Cb,up,Cout,mode", [
-    ((12, 24, 70), 16, 0, False, 16, "fwd"),      # one channel group, tensor copy only (conv_tcs2, forward epilogue)
+    ((12, 24, 70), 16, 0, False, 16, "fwd"),      # one channel group, tensor copy only (forward epilogue)
     ((12, 24, 70), 32, 16, True, 32, "fwd"),      # upsampled group on cp.async + skip group by tensor copy (conv_tcs)
     ((10, 20, 40), 16, 0, False, 32, "dgrad"),    # dgrad epilogue (mask)
     ((10, 20, 40), 32, 0, False, 48, "split"),    # raw + channel split epilogue
@@ -308,7 +308,7 @@ def test_tma_and_lean_epilogue_match_reference_paths(tc, cuda, monkeypatch, shap
         assert torch.equal(v, ref), k      # same MMAs in the same order, same fp32 epilogue arithmetic: bit-identical
 
 
-# ---- round 2: kd folded into the channels (first convolution / flow head) ----
+# ---- kd folded into the channels (first convolution / flow head) ----
 
 def _khm_wgrad(tc, x, gz, cin_real, cout_real, cuda):
     batch = tc.WgradBatch.get(cuda)

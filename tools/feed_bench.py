@@ -1,6 +1,6 @@
 """Host-side feed rate of the scan-to-scan generator (row N1): batches/s a training loop can draw, including the
 train.py:200-201 host conversion (`torch.from_numpy(d).float().permute(0, 4, 1, 2, 3)`), for
-  reference  : the unmodified voxelmorph.generators.scan_to_scan (build container only: needs /root/reference)
+  reference  : the unmodified voxelmorph.generators.scan_to_scan (needs the reference tree: VXM_REFERENCE_ROOT, see oracle/ref_import.py)
   b200       : voxelmorph_b200.generators.scan_to_scan (decode-once cache, float32, zero-copy batch of one)
   b200+prefetch : the same behind generators.Prefetcher
 on N synthetic compressed .npz volumes of the BASELINE shape.  CPU only; prints one JSON line.

@@ -1,5 +1,5 @@
 """Summarise an `ncu --set full` report (.ncu-rep) into a markdown table: per kernel the duration, DRAM traffic, tensor-pipe /
-shared-memory-operand utilisation and the top warp-stall sites.  Usage: python tools/ncu_summary.py report.ncu-rep [...] > profiles/x.md
+shared-memory-operand utilisation and the top warp-stall sites.  Usage: python tools/ncu_summary.py report.ncu-rep [...] > summary.md
 (runs `ncu -i` locally; no GPU needed)."""
 import csv, io, subprocess, sys, collections
 
@@ -13,9 +13,8 @@ KEYS = [
     ("launch__registers_per_thread", "regs/thread"),
     ("launch__shared_mem_per_block_dynamic", "dyn smem/block"),
     ("sm__pipe_tc_cycles_active.avg.pct_of_peak_sustained_elapsed", "tensor pipe (tc) cycles active"),
-    ("sm__ops_path_tensor_op_utchmma_src_bf16_dst_fp32_sparsity_off.avg.pct_of_peak_sustained_elapsed", "UTCHMMA bf16 math rate vs peak"),
+    ("sm__pipe_tensor_op_gmma_cycles_active.avg.pct_of_peak_sustained_elapsed", "wgmma pipe cycles active"),
     ("l1tex__data_pipe_tc_wavefronts_mem_shared.sum.pct_of_peak_sustained_elapsed", "tensor-core smem operand wavefronts vs peak"),
-    ("smsp__mem_tensor_reads_op_utcmma_matrix_c.sum.pct_of_peak_sustained_elapsed", "TMEM accumulator reads by MMA vs peak"),
     ("sm__inst_executed.avg.pct_of_peak_sustained_elapsed", "instruction issue vs peak"),
     ("lts__t_sector_hit_rate.pct", "L2 hit rate"),
     ("lts__throughput.avg.pct_of_peak_sustained_elapsed", "L2 throughput vs peak"),

@@ -1,4 +1,4 @@
-"""Round-2 measurement aid for the memory-bound kernels: every kernel is called straight through the C ABI (no autograd
+"""Measurement aid for the memory-bound kernels: every kernel is called straight through the C ABI (no autograd
 around it) at the benchmark shapes.
 
   python tools/r2_memprof.py time     -> CUDA-event timings (L2 flushed between launches), JSON on stdout
@@ -15,6 +15,7 @@ import torch
 import voxelmorph_b200 as vxm
 from voxelmorph_b200 import _lib
 
+HBM_GBS = 3350.0   # H100 SXM data-sheet HBM3 bandwidth (700 W); frac is relative to it
 mode = sys.argv[1] if len(sys.argv) > 1 else "time"
 dev = torch.device("cuda:0")
 lib = _lib.load()
@@ -93,6 +94,6 @@ for name, (fn, nbytes) in K.items():
         torch.cuda.synchronize()
         ts.append(a.elapsed_time(b) * 1e3)
     t = statistics.median(ts)
-    res[name] = dict(us=round(t, 1), gbs=round(nbytes / t / 1e3, 1) if nbytes else None, frac=round(nbytes / t / 1e3 / 6572.9, 3) if nbytes else None)
-    print("%-30s %8.1f us  %s" % (name, t, "" if not nbytes else "%7.1f GB/s  %.3f" % (nbytes / t / 1e3, nbytes / t / 1e3 / 6572.9)), file=sys.stderr)
+    res[name] = dict(us=round(t, 1), gbs=round(nbytes / t / 1e3, 1) if nbytes else None, frac=round(nbytes / t / 1e3 / HBM_GBS, 3) if nbytes else None)
+    print("%-30s %8.1f us  %s" % (name, t, "" if not nbytes else "%7.1f GB/s  %.3f" % (nbytes / t / 1e3, nbytes / t / 1e3 / HBM_GBS)), file=sys.stderr)
 print(json.dumps(res))

@@ -1,4 +1,4 @@
-"""Run one tcgen05 conv layer a few times (for ncu)."""
+"""Run one tensor-core conv layer a few times (for a profiler)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

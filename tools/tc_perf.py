@@ -1,4 +1,4 @@
-"""Per-layer timing of the tcgen05 convolution kernels at the benchmark shapes (CUDA events, isolated launches)."""
+"""Per-layer timing of the tensor-core convolution kernels at the benchmark shapes (CUDA events, isolated launches)."""
 import sys, os, statistics, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,6 +1,6 @@
 """`import voxelmorph as vxm` for the unmodified reference scripts (scripts/torch/train.py, register.py):
 the import surface of the reference package (voxelmorph/__init__.py:20-44) re-exported from `voxelmorph_b200`,
-whose operators are hand-written sm_100a kernels behind the C ABI of include/vxm_b200.h.
+whose operators are hand-written sm_90a kernels behind the C ABI of include/vxm_b200.h.
 
     os.environ['VXM_BACKEND'] = 'pytorch'; import voxelmorph as vxm
     vxm.networks.VxmDense, vxm.layers.{SpatialTransformer,VecInt,ResizeTransform}, vxm.losses.{NCC,MSE,Dice,Grad},
@@ -21,7 +21,7 @@ from .py.utils import default_unet_features   # noqa: E402,F401
 
 backend = py.utils.get_backend()
 if backend != 'pytorch':
-    raise ImportError("this voxelmorph build (voxelmorph_b200, B200 / sm_100a) provides the pytorch backend only: "
+    raise ImportError("this voxelmorph build (voxelmorph_b200, H100 / sm_90a) provides the pytorch backend only: "
                       "set the VXM_BACKEND environment variable to 'pytorch' before importing voxelmorph")
 os.environ['NEURITE_BACKEND'] = 'pytorch'
 

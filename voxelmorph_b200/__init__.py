@@ -1,4 +1,4 @@
-"""voxelmorph_b200 — B200-native (sm_100a) VxmDense registration path.
+"""voxelmorph_b200 — H100-native (sm_90a) VxmDense registration path.
 
 Mirrors the torch backend of voxelmorph (`voxelmorph.torch.{layers,networks,losses,modelio}`)
 class for class; every operator runs in a hand-written CUDA kernel reached through the

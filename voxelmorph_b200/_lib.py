@@ -146,7 +146,7 @@ def require_cuda(*tensors, what="voxelmorph_b200"):
         if t is None:
             continue
         if not t.is_cuda:
-            raise VxmError("%s: CUDA tensors are required (the B200 path has no CPU fallback); got a %s tensor"
+            raise VxmError("%s: CUDA tensors are required (the GPU path has no CPU fallback); got a %s tensor"
                            % (what, t.device))
         if t.dtype != torch.float32:
             raise VxmError("%s: float32 tensors are required at the module boundary; got %s" % (what, t.dtype))

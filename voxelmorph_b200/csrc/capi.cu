@@ -32,10 +32,10 @@ int check_launch(const char* what) {
 int sm_count() {
   static thread_local int cached_dev = -1, cached = 0;
   int dev = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;   // H100 SXM
   if (dev != cached_dev) {
     int n = 0;
-    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;
+    if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;
     cached = n;
     cached_dev = dev;
   }
@@ -84,5 +84,5 @@ int make_act_tmap(CUtensorMap* out, const void* base, int B, int D, int H, int W
 }  // namespace vxm
 
 extern "C" const char* vxm_last_error(void) { return vxm::g_err; }
-extern "C" const char* vxm_version(void) { return "vxm_b200 0.1 sm_100a"; }
+extern "C" const char* vxm_version(void) { return "vxm_b200 0.1 sm_90a"; }
 extern "C" uint64_t vxm_launch_count(void) { return vxm::g_launches.load(std::memory_order_relaxed); }

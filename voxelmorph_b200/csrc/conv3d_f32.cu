@@ -3,7 +3,7 @@
 //
 // This is the fp32 "parity" engine (CUDA-core FFMA, NCDHW planar): it reproduces the reference's
 // fp32 convolution to ~1e-6 relative so that the 1e-4 flow / moved-image tolerance holds through
-// the 12-layer U-Net.  The bf16 tcgen05/TMEM implicit-GEMM engine (conv3d_tc.cu) is the
+// the 12-layer U-Net.  The bf16 wgmma implicit-GEMM engine (conv3d_tc.cu) is the
 // throughput path.
 //
 // forward / dgrad share one kernel: dgrad is the same convolution with the roles of Cin / Cout

@@ -1,24 +1,23 @@
-// Conv3d k=3 s=1 p=1 as an implicit GEMM on the 5th-generation tensor cores (tcgen05.mma, accumulators in
-// TMEM) — the throughput engine behind reference voxelmorph/torch/networks.py:299-304 (ConvBlock) and
-// :211,257 (flow head).  Forward and dgrad share this kernel (dgrad = same convolution with swapped
-// channel roles and flipped taps, see vxm_conv3d_tc_pack).
+// Conv3d k=3 s=1 p=1 as an implicit GEMM on the Hopper tensor cores (wgmma.mma_async, accumulators in registers) —
+// the one-MMA-per-tap engine behind reference voxelmorph/torch/networks.py:299-304 (ConvBlock) and :211,257 (flow head),
+// kept as the tested baseline of the kw-stacked kernels (VXM_B200_TC_KERNEL=n).  Forward and dgrad share this kernel
+// (dgrad = same convolution with swapped channel roles and flipped taps, see vxm_conv3d_tc_pack).
 //
 // Formulation (per output d-slice of a 16 x 8 (h x w) tile):
 //     D[128 voxels x N=Cout] += A_tap[128 voxels x 16 ch] * W_tap[N x 16 ch]        27 taps x Cin/16 K-steps
 //   * activations are bf16, channels-last (NDHWC); a halo'd slab of each input slice, (16+2) x (8+2) voxels,
-//     is staged in shared memory as [Cin/8][180 rows][8 ch] = the UMMA "K-major, no swizzle" canonical
+//     is staged in shared memory as [Cin/8][180 rows][8 ch] = the wgmma "K-major, no swizzle" canonical
 //     layout (core matrix = 8 voxels x 16 B).  In that layout a tap shift (kh, kw) is just a start-address
 //     offset of (kh*10 + kw) * 16 bytes, so all 9 in-plane taps read the SAME staged slab, and the 3 kd taps
-//     read the 3 resident slabs of a 4-deep ring that slides along D: every input voxel is fetched from
-//     L2/HBM ~1.4x, not 27x.
+//     read the 3 resident slabs of a ring that slides along D: every input voxel is fetched from L2/HBM ~1.4x, not 27x.
 //   * weights: bf16, pre-packed per (tap, K-step) into the canonical K-major layout; the whole filter bank
 //     stays resident in shared memory, loaded once per CTA with bulk-TMA copies (cp.async.bulk + mbarrier tx).
-//   * warp-specialised persistent CTA: warps 5-8 stage slabs with zero-filling cp.async (padding, nearest-x2
+//   * warp-specialised persistent CTA: warps 4-7 stage slabs with zero-filling cp.async (padding, nearest-x2
 //     upsample and the channel concat with the skip tensor are all address arithmetic in the loader — the
-//     48/64-channel concat tensor of networks.py:138 is never materialised); one elected thread of warp 4
-//     issues tcgen05.mma and tcgen05.commit; warps 0-3 drain TMEM (tcgen05.ld: one voxel's Cout channels per
-//     thread), add bias, apply LeakyReLU (or the dgrad mask) and write 16-byte bf16 NDHWC vectors.
-//     Pipelines: slab ring full/empty mbarriers (loader <-> MMA), TMEM full/empty (MMA <-> epilogue).
+//     48/64-channel concat tensor of networks.py:138 is never materialised); warpgroup 0 issues the wgmma chain of a
+//     tile (two m64 halves), then drains its registers (one voxel's Cout channels per thread after a shared-memory
+//     transpose), adds bias, applies LeakyReLU (or the dgrad mask) and writes 16-byte bf16 NDHWC vectors.
+//     Pipeline: slab ring full/empty mbarriers (loader <-> MMA warpgroup).
 #include <stdlib.h>
 
 #include "tc_common.cuh"
@@ -30,8 +29,8 @@ constexpr int TH = 16, TW = 8;
 constexpr int SW = TW + 2, SH = TH + 2;
 constexpr int ROWS = SH * SW;     // 180 voxels per channel-chunk plane
 constexpr int PLANE = ROWS * 16;  // bytes
-constexpr int MAXSLOT = 8, NACC = 2, KMAX = 12;
-constexpr int NLOADER = 128, NTHREADS = 288;
+constexpr int MAXSLOT = 8, KMAX = 12;
+constexpr int NLOADER = 128, NTHREADS = 256;   // warps 0-3: MMA + epilogue warpgroup, warps 4-7: loader
 
 struct ConvTcArgs {
   const __nv_bfloat16* xa;    // bf16 NDHWC source A (B,Da,Ha,Wa,Ca); half resolution when up == 1
@@ -61,38 +60,28 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tc_kernel(const ConvTcArgs a
   // the second 16-byte K chunk of the single K step reads a shared all-zero plane
   const bool halfk = planar || (a.Ca + a.Cb == 8);
   const int Cin = NK16 * 16;
-  constexpr int nk16 = NK16;
   const int nc8 = halfk ? 1 : Cin / 8;
   const uint32_t slab_bytes = (uint32_t)nc8 * PLANE;
   uint8_t* s_w = smem;
   uint8_t* s_slab = smem + ((a.wbytes + 127u) & ~127u);
   const int NSLOT = a.nslot;
   uint8_t* s_zero = s_slab + NSLOT * slab_bytes;   // one all-zero plane (only used in planar mode)
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_zero + PLANE);
+  float* s_stage = reinterpret_cast<float*>(s_zero + PLANE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + ACC_STAGE_FLOATS);
   uint64_t* full = bars;
   uint64_t* empty = bars + MAXSLOT;
-  uint64_t* tfull = bars + 2 * MAXSLOT;
-  uint64_t* tempty = tfull + NACC;
-  uint64_t* wbar = tempty + NACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
+  uint64_t* wbar = empty + MAXSLOT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t tmem_cols = (NACC * NP <= 32) ? 32u : ((NACC * NP <= 64) ? 64u : 128u);
-  static_assert(NACC * NP <= 128, "accumulators exceed the TMEM allocation");
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], NLOADER); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < NACC; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 128); }
+    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], NLOADER); mbar_init(&empty[i], 4); }   // one arrival per MMA warp
     mbar_init(wbar, 1);
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < PLANE / 16; i += NTHREADS) reinterpret_cast<uint4*>(s_zero)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (threadIdx.x == 0) {  // weights: bulk TMA copies, one mbarrier transaction
     mbar_expect_tx(wbar, a.wbytes);
@@ -104,11 +93,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tc_kernel(const ConvTcArgs a
 
   const int HW_tiles = a.tiles_h * a.tiles_w;
 
-  if (warp >= 5) {
+  if (warp >= 4) {
     // ================================ LOADER (128 threads) ================================
     // Runs ahead of the tensor core by (nslot - 3) slabs.  cp.async completion is reported straight to the
     // slab's "full" mbarrier (cp.async.mbarrier.arrive.noinc), so issuing slab s+1 never waits for slab s.
-    const int lt = threadIdx.x - 5 * 32;
+    const int lt = threadIdx.x - 4 * 32;
     uint32_t cnt = 0;
     const int Da = a.upd ? a.D >> 1 : a.D, Ha = a.up ? a.H >> 1 : a.H, Wa = a.up ? a.W >> 1 : a.W;
     const int nca8 = a.Ca >> 3;
@@ -177,84 +166,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tc_kernel(const ConvTcArgs a
         ++cnt;
       }
     }
-  } else if (warp == 4) {
-    // ================================ MMA ISSUER (one thread) ================================
-    // The whole warp runs this loop (warp-uniform control flow keeps the descriptors in uniform registers);
-    // one elected lane issues the tcgen05 instructions.
-    {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-      const uint32_t slab_u32 = smem_u32(s_slab), w_u32 = smem_u32(s_w);
-      const uint32_t a_lbo = halfk ? (smem_u32(s_zero) - slab_u32) : (uint32_t)PLANE;
-      constexpr uint32_t b_tile16 = (uint32_t)NP * 32u / 16u;
-      mbar_wait(wbar, 0);
-      const uint64_t bdesc0 = make_desc_kmajor_noswz(w_u32, (uint32_t)NP * 16u, 128u);
-      uint32_t cnt_base = 0, acc_cnt = 0;
-      for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-        const int ch = (item / HW_tiles) % a.nchunks;
-        const int d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
-        const int nd = d1 - d0;
-        for (int j = 0; j < nd; ++j) {
-          if (KD == 3) {
-            if (j == 0) {
-              for (int q = 0; q < 2; ++q) { uint32_t c = cnt_base + q; mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1); }
-            }
-            uint32_t c = cnt_base + j + 2;
-            mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
-          } else {
-            uint32_t c = cnt_base + j;
-            mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
-          }
-          const uint32_t acc = acc_cnt % NACC;
-          mbar_wait(&tempty[acc], ((acc_cnt / NACC) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t tmem_d = tmem_base + acc * (uint32_t)NP;
-          uint64_t adesc_kd[KD];
-#pragma unroll
-          for (int kd = 0; kd < KD; ++kd) {
-            const uint32_t sl = (cnt_base + j + kd) % NSLOT;
-            // planar mode: the second K chunk (channels 8..15) reads the shared all-zero plane
-            adesc_kd[kd] = make_desc_kmajor_noswz(slab_u32 + sl * slab_bytes, halfk ? (a_lbo - sl * slab_bytes) : a_lbo, (uint32_t)SW * 16u);
-          }
-          if (elect_one()) {
-#pragma unroll
-            for (int kd = 0; kd < KD; ++kd) {
-#pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-#pragma unroll
-                for (int kw = 0; kw < 3; ++kw) {
-#pragma unroll
-                  for (int k = 0; k < NK16; ++k) {
-                    constexpr int dummy = 0; (void)dummy;
-                    const int tap = (kd * 3 + kh) * 3 + kw;
-                    // start-address field is in 16-byte units: tap shift (kh*SW + kw) rows, K step = 2 planes
-                    const uint64_t adesc = adesc_kd[kd] + (uint64_t)(kh * SW + kw + k * (2 * PLANE / 16));
-                    const uint64_t bdesc = bdesc0 + (uint64_t)((tap * NK16 + k) * b_tile16);
-                    umma_f16(tmem_d, adesc, bdesc, idesc, (kd | kh | kw | k) ? 1u : 0u);
-                  }
-                }
-              }
-            }
-            umma_commit(&tfull[acc]);
-            umma_commit(&empty[(cnt_base + j) % NSLOT]);   // oldest slab of the window is no longer needed
-          }
-          __syncwarp();
-          ++acc_cnt;
-        }
-        if (KD == 3) {
-          if (elect_one()) {
-            umma_commit(&empty[(cnt_base + nd) % NSLOT]);
-            umma_commit(&empty[(cnt_base + nd + 1) % NSLOT]);
-          }
-          __syncwarp();
-          cnt_base += nd + 2;
-        } else {
-          cnt_base += nd;
-        }
-      }
-    }
   } else {
-    // ================================ EPILOGUE (warps 0-3) ================================
-    uint32_t acc_cnt = 0;
+    // ================================ MMA + EPILOGUE (warpgroup 0) ================================
+    // The warpgroup issues the wgmma chain of a tile (two m64 halves: tile rows 0-63 / 64-127), releases the oldest
+    // slab of the window once the chain has completed, then drains its accumulators: one voxel's Cout channels per
+    // thread, bias, LeakyReLU (or the dgrad mask), 16-byte bf16 NDHWC vectors.
+    const uint32_t slab_u32 = smem_u32(s_slab), w_u32 = smem_u32(s_w);
+    const uint32_t a_lbo = halfk ? (smem_u32(s_zero) - slab_u32) : (uint32_t)PLANE;
+    constexpr uint32_t b_tile16 = (uint32_t)NP * 32u / 16u;
+    constexpr uint32_t half16 = 8u * SW;          // rows 64-127: 8 groups of 8 rows further, in 16-byte units
+    mbar_wait(wbar, 0);
+    const uint64_t bdesc0 = make_desc_kmajor_noswz(w_u32, (uint32_t)NP * 16u, 128u);
+    uint32_t cnt_base = 0;
     const int row = warp * 32 + lane;
     const int rh = row >> 3, rw = row & 7;
     const size_t HW = (size_t)a.H * a.W;
@@ -262,21 +185,56 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tc_kernel(const ConvTcArgs a
       const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
       const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
       const int h = ht * TH + rh, w = wt * TW + rw, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
+      const int nd = d1 - d0;
       const bool inside = h < a.H && w < a.W;
-      for (int d = d0; d < d1; ++d) {
-        const uint32_t acc = acc_cnt % NACC;
-        mbar_wait(&tfull[acc], (acc_cnt / NACC) & 1);
-        tc_fence_after();
+      for (int j = 0; j < nd; ++j) {
+        const int d = d0 + j;
+        if (KD == 3) {
+          if (j == 0) {
+            for (int q = 0; q < 2; ++q) { uint32_t c = cnt_base + q; mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1); }
+          }
+          uint32_t c = cnt_base + j + 2;
+          mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
+        } else {
+          uint32_t c = cnt_base + j;
+          mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
+        }
+        uint64_t adesc_kd[KD];
+#pragma unroll
+        for (int kd = 0; kd < KD; ++kd) {
+          const uint32_t sl = (cnt_base + j + kd) % NSLOT;
+          // planar mode: the second K chunk (channels 8..15) reads the shared all-zero plane
+          adesc_kd[kd] = make_desc_kmajor_noswz(slab_u32 + sl * slab_bytes, halfk ? (a_lbo - sl * slab_bytes) : a_lbo, (uint32_t)SW * 16u);
+        }
+        float acc0[NP / 2], acc1[NP / 2];
+        wg_fence();
+#pragma unroll
+        for (int kd = 0; kd < KD; ++kd) {
+#pragma unroll
+          for (int kh = 0; kh < 3; ++kh) {
+#pragma unroll
+            for (int kw = 0; kw < 3; ++kw) {
+#pragma unroll
+              for (int k = 0; k < NK16; ++k) {
+                const int tap = (kd * 3 + kh) * 3 + kw;
+                // start-address field is in 16-byte units: tap shift (kh*SW + kw) rows, K step = 2 planes
+                const uint64_t adesc = adesc_kd[kd] + (uint64_t)(kh * SW + kw + k * (2 * PLANE / 16));
+                const uint64_t bdesc = bdesc0 + (uint64_t)((tap * NK16 + k) * b_tile16);
+                const uint32_t accum = (kd | kh | kw | k) ? 1u : 0u;
+                Wgmma<NP, 0, 0>::mma(acc0, adesc, bdesc, accum);
+                Wgmma<NP, 0, 0>::mma(acc1, adesc + half16, bdesc, accum);
+              }
+            }
+          }
+        }
+        wg_commit();
+        wg_wait<0>();
+        if (lane == 0) mbar_arrive(&empty[(cnt_base + j) % NSLOT]);   // oldest slab of the window is no longer needed
         uint32_t r[NP];
-        const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + acc * (uint32_t)NP;
-        tmem_ld16(taddr, r);
-        if constexpr (NP > 16) tmem_ld16(taddr + 16, r + 16);
-        if constexpr (NP > 32) tmem_ld16(taddr + 32, r + 32);
-        if constexpr (NP > 48) tmem_ld16(taddr + 48, r + 48);
-        tmem_ld_wait();
-        tc_fence_before();
-        mbar_arrive(&tempty[acc]);
-        ++acc_cnt;
+        acc_row16(acc0, acc1, 0, s_stage, 1, r);
+        if constexpr (NP > 16) acc_row16(acc0, acc1, 16, s_stage, 1, r + 16);
+        if constexpr (NP > 32) acc_row16(acc0, acc1, 32, s_stage, 1, r + 32);
+        if constexpr (NP > 48) acc_row16(acc0, acc1, 48, s_stage, 1, r + 48);
         if (!inside) continue;
         const size_t vox = (((size_t)b * a.D + d) * a.H + h) * a.W + w;
         if (a.out_mode == 0) {
@@ -320,11 +278,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tc_kernel(const ConvTcArgs a
           }
         }
       }
+      if (KD == 3) {
+        if (lane == 0) {
+          mbar_arrive(&empty[(cnt_base + nd) % NSLOT]);
+          mbar_arrive(&empty[(cnt_base + nd + 1) % NSLOT]);
+        }
+        cnt_base += nd + 2;
+      } else {
+        cnt_base += nd;
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // Weight packing: fp32 (Cout, Cin, KD, 3, 3) -> bf16 [tap][k16][2][NP][8]  (canonical K-major, no swizzle).
@@ -407,7 +371,7 @@ extern "C" int vxm_conv3d_tc_fwd(const void* xa, const void* xb, const float* co
   a.wbytes = (uint32_t)vxm_conv3d_tc_packed_bytes(Cin, np, kd);   // Cin is rounded up to the K step (16)
   int nc8 = (nplanar > 0 || Ca + Cb == 8) ? 1 : Cin / 8;
   VXM_REQUIRE(nc8 * ROWS <= KMAX * NLOADER, "conv3d_tc_fwd: slab too large for the loader table");
-  size_t fixed = ((a.wbytes + 127u) & ~127u) + PLANE + 256;
+  size_t fixed = ((a.wbytes + 127u) & ~127u) + PLANE + ACC_STAGE_FLOATS * sizeof(float) + 256;
   int nslot = (int)((227 * 1024 - fixed) / ((size_t)nc8 * PLANE));
   if (nslot > MAXSLOT) nslot = MAXSLOT;
   VXM_REQUIRE(nslot >= 4, "conv3d_tc_fwd: not enough shared memory for the slab ring");

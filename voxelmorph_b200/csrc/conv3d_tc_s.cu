@@ -1,7 +1,7 @@
-// Conv3d k=3 on tcgen05, "kw-stacked" formulation with 128/64/32-byte SWIZZLED K-major operands.
+// Conv3d k=3 on the Hopper tensor cores (wgmma), "kw-stacked" formulation with 128/64/32-byte SWIZZLED K-major operands.
 //
 // Same algorithm as conv3d_tc_t.cu (N = 3*Cout stacks the kw taps, K loop over (kd, kh, Cin/16), kw shift by warp
-// shuffle in the epilogue), but the shared-memory operands use the UMMA swizzled canonical layouts instead of
+// shuffle in the epilogue), but the shared-memory operands use the wgmma swizzled canonical layouts instead of
 // SWIZZLE_NONE: every slab row is one voxel with all channels of a channel group contiguous (32 / 64 / 128 bytes)
 // and the 16-byte chunks of a row are XOR-swizzled with the row index (Swizzle<B,4,3>), which the cp.async loader
 // applies to its destination addresses and the weight packer applies on the host side of the operand.  The input
@@ -19,8 +19,8 @@ namespace tcs {
 using namespace vxm::tc;
 
 constexpr int WT = 32, WUSE = 30;      // tile: HT (4 or 8) rows x 32 columns (30 written), slab = (HT + 2) x 32 voxel rows
-constexpr int MAXSLOT = 16, MAXACC = 4;
-constexpr int NLOADER = 96, NTHREADS = 512, NGRP = 3;   // warps 0-3 epilogue group 0, 4 MMA issuer, 5-7 loader, 8-11 / 12-15 epilogue groups 1 / 2
+constexpr int MAXSLOT = 16;
+constexpr int NLOADER = 128, NTHREADS = 384, NGRP = 2;   // warps 0-3 / 4-7: MMA + epilogue groups 0 / 1, warps 8-11: loader
 
 struct ConvSArgs {
   const __nv_bfloat16* xa; const __nv_bfloat16* xb;
@@ -52,16 +52,14 @@ __device__ __forceinline__ uint64_t make_desc_kmajor_swz(uint32_t saddr, uint32_
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;                                   // LBO: unused for K inside one swizzle atom
   d |= (uint64_t)(((8u * width) >> 4) & 0x3FFF) << 32;      // SBO: 8 rows
-  d |= (uint64_t)1 << 46;                                   // descriptor version 1
-  d |= (uint64_t)(width == 128 ? 2 : (width == 64 ? 4 : 6)) << 61;   // SWIZZLE_128B / 64B / 32B
-  return d;
+  return d | desc_swizzle(width);
 }
 
 // HT = 8: one slab step feeds TWO 4-row accumulators (one per epilogue group), halving the per-step issue / barrier
 // overhead that bounds the thin layers and cutting the halo re-reads from 1.5x to 1.25x.
 // ACC: the split-precision epilogue (acc_in / out_mode 2, 3) is compiled in; the plain kernels (ACC = false) keep the
 // round-1 epilogue — with the extra live registers the 32-channel variants spilled and lost up to 1.8x.
-// EPI: epilogue specialisation (see conv3d_tc_s2.cu).  0 = generic run-time epilogue; 1 = forward (bias + LeakyReLU with
+// EPI: epilogue specialisation.  0 = generic run-time epilogue; 1 = forward (bias + LeakyReLU with
 // 0 <= slope <= 1, bf16 channels-last, all COUT channels real); 2 = dgrad (LeakyReLU derivative from the saved activation);
 // 3 = raw sums with an optional channel split at a multiple of 16 (single-pass dgrad of a concat layer).
 template <int KD, int G0, int G1, int COUT, int HT, bool ACC, int EPI>
@@ -71,40 +69,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
   constexpr int W0 = G0 * 2, W1 = G1 * 2;                 // row bytes of the two channel groups
   constexpr int NC8 = (G0 + G1) / 8;                      // 16-byte chunks per voxel
   constexpr uint32_t SLAB0 = SROWS * W0, SLAB1 = SROWS * W1;
-  constexpr int NN = 3 * COUT;   // MMA N: (kw, co)
-  // TMEM accumulators in flight = epilogue groups in use: group g owns accumulator g, so every mbarrier is waited on
-  // phase by phase (a group that skipped ahead on a barrier would alias its parity)
-  constexpr int NACC = (3 * NN <= 512) ? 3 : 2;
+  constexpr int NN = 3 * COUT;   // (kw, co) columns of the packed weights
   extern __shared__ __align__(1024) uint8_t smem[];
   const bool halfk = (a.Ca + a.Cb == 8);                  // 8 real channels in a 16-channel group: chunk 1 is zero-filled
   constexpr uint32_t slab_bytes = SLAB0 + SLAB1;
   const int NSLOT = a.nslot;
   uint8_t* s_w = smem;
   uint8_t* s_slab = smem + ((a.wbytes + 1023u) & ~1023u);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_slab + NSLOT * slab_bytes);
+  float* s_stage = reinterpret_cast<float*>(s_slab + NSLOT * slab_bytes);   // one accumulator read-out buffer per group
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + NGRP * ACC_STAGE_FLOATS);
   uint64_t* full = bars;
   uint64_t* empty = bars + MAXSLOT;
-  uint64_t* tfull = bars + 2 * MAXSLOT;
-  uint64_t* tempty = tfull + MAXACC;
-  uint64_t* wbar = tempty + MAXACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
+  uint64_t* wbar = empty + MAXSLOT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t tmem_cols = NACC * NN <= 128 ? 128u : (NACC * NN <= 256 ? 256u : 512u);
 
   const bool tma0 = a.tma_mask & 1, tma1 = (a.tma_mask & 2) != 0;
   const bool all_tma = tma0 && (G1 == 0 || tma1);        // no cp.async traffic at all: one producer thread
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], all_tma ? 1 : NLOADER); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < NACC; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 4); }     // one arrival per epilogue warp
+    // empty: one arrival per warp of every group (each group releases every slab once, see below)
+    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], all_tma ? 1 : NLOADER); mbar_init(&empty[i], 4 * NGRP); }
     mbar_init(wbar, 1);
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (threadIdx.x == 0) {
     mbar_expect_tx(wbar, a.wbytes);
@@ -115,9 +103,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
   }
   const int HW_tiles = a.tiles_h * a.tiles_w;
 
-  if (warp >= 5 && warp < 8) {
-    // ================================ LOADER (96 threads) ================================
-    const int lt = threadIdx.x - 5 * 32;
+  if (warp >= 8) {
+    // ================================ LOADER (128 threads) ================================
+    const int lt = threadIdx.x - 8 * 32;
     uint32_t slot = 0, lphase = 1;   // producer side: the first lap passes on the fresh barriers
     const int Da = a.upd ? a.D >> 1 : a.D, Ha = a.up ? a.H >> 1 : a.H, Wa = a.up ? a.W >> 1 : a.W;
     const int nca8 = a.Ca >> 3;
@@ -180,106 +168,105 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         if (++slot == (uint32_t)NSLOT) { slot = 0; lphase ^= 1; }
       }
     }
-  } else if (warp == 4) {
-    // ================================ MMA ISSUER (whole warp, one elected lane) ================================
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+  } else {
+    // ================================ MMA + EPILOGUE (2 warpgroups; warp = tile row hh, lane = w') ==================
+    // Tile event e (one per 4-row tile half, counted over the CTA's lifetime) belongs to group e % 2: the group issues
+    // its wgmma chain and drains the accumulators, so the tensor core works on one group's tile while the other runs its
+    // epilogue.  With 8-row tiles group g always takes half g of every slab step.
+    // Slab release: every group walks ALL slabs in order (waiting for each one's full phase) and arrives once on each
+    // slab's empty barrier after its last MMA reading it has completed, so a slot is refilled only after both groups
+    // are past it and no barrier phase can alias.
+    const int grp = warp >> 2;
+    const int wq = warp & 3;
+    float* stage = s_stage + grp * ACC_STAGE_FLOATS;
+    const int nbar = 1 + grp;
+    // MMA N per wgmma: the three kw taps stacked (N = 3 * COUT) up to COUT = 32; wider layers run in passes of 16
+    // output channels with one wgmma per kw (the accumulators of a pass stay within the register budget)
+    constexpr bool STACK = COUT <= 32;
+    constexpr int CW = STACK ? COUT : 16;            // output channels per pass
+    constexpr int NPASS = COUT / CW;
+    constexpr int NA = STACK ? NN : CW;              // N of one wgmma
+    constexpr int NW = STACK ? 1 : 3;                // wgmmas per K step and tile half
     const uint32_t slab_u32 = smem_u32(s_slab), w_u32 = smem_u32(s_w);
     constexpr uint32_t WSTEP = (uint32_t)NN * (W0 + W1);          // bytes of packed weights per (kd, kh) step
     mbar_wait(wbar, 0);
     const uint64_t bdesc0 = make_desc_kmajor_swz(w_u32, W0);
     const uint64_t bdesc1 = make_desc_kmajor_swz(w_u32 + NN * W0, W1 ? W1 : 32);
-    // slot / phase bookkeeping is incremental (no runtime modulo: the issue loop is the critical path of the thin layers)
-    uint32_t wslot = 0, wphase = 0;     // next slab to wait for
-    uint32_t hslot = 0;                 // head of the kd window
-    uint32_t acc = 0, aphase = 1;       // accumulator ring (consumer of tempty: first lap passes)
-    for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-      const int ch = (item / HW_tiles) % a.nchunks;
-      const int d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
-      const int nd = d1 - d0;
-      for (int j = 0; j < nd; ++j) {
-        const int nwait = (KD == 3 && j == 0) ? 3 : 1;
-        for (int q = 0; q < nwait; ++q) {
-          mbar_wait(&full[wslot], wphase);
-          if (++wslot == (uint32_t)NSLOT) { wslot = 0; wphase ^= 1; }
-        }
-        uint64_t adesc0_kd[KD], adesc1_kd[KD];
-        {
-          uint32_t sl = hslot;
+    uint32_t cnt_base = 0, ecnt = 0, wcur = 0;
+    auto observe = [&](uint32_t upto) {              // wait for every slab up to global index `upto`, in order
+      for (; wcur <= upto; ++wcur) mbar_wait(&full[wcur % NSLOT], (wcur / NSLOT) & 1);
+    };
+    // wgmma chain of tile half hb of the step whose kd window starts at ring slot `hslot`, output channels of `pass`
+    auto mma = [&](uint32_t hslot, int hb, int pass, float (&acc)[2][NW][NA / 2]) {
+      uint64_t adesc0_kd[KD], adesc1_kd[KD];
+      uint32_t sl = hslot;
 #pragma unroll
-          for (int kd = 0; kd < KD; ++kd) {
-            adesc0_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes, W0);
-            adesc1_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes + SLAB0, W1 ? W1 : 32);
-            if (++sl == (uint32_t)NSLOT) sl = 0;
-          }
-        }
+      for (int kd = 0; kd < KD; ++kd) {
+        adesc0_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes, W0);
+        adesc1_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes + SLAB0, W1 ? W1 : 32);
+        if (++sl == (uint32_t)NSLOT) sl = 0;
+      }
+      wg_fence();
 #pragma unroll
-        for (int hb = 0; hb < NH; ++hb) {
-        mbar_wait(&tempty[acc], aphase);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * (uint32_t)NN;
-        if (elect_one()) {
+      for (int kd = 0; kd < KD; ++kd) {
 #pragma unroll
-          for (int kd = 0; kd < KD; ++kd) {
+        for (int kh = 0; kh < 3; ++kh) {
+          const int st = kd * 3 + kh;
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
-              {
-                const int st = kd * 3 + kh;
+          for (int k = 0; k < (G0 + G1) / 16; ++k) {  // start-address field is in 16-byte units: kh rows, 32 B per K step
+            const bool g0 = k < G0 / 16;
+            const int kk = g0 ? k : k - G0 / 16;
+            const uint32_t wr = g0 ? W0 : W1;
+            const uint64_t adesc = (g0 ? adesc0_kd[kd] : adesc1_kd[kd]) + (uint64_t)(((hb * 4 + kh) * WT * wr + kk * 32) >> 4);
+            const uint64_t bdesc = (g0 ? bdesc0 : bdesc1) + (uint64_t)((st * WSTEP + kk * 32) >> 4);
 #pragma unroll
-                for (int k = 0; k < G0 / 16; ++k) {      // start-address field is in 16-byte units: kh rows, 32 B per K step
-                  const uint64_t adesc = adesc0_kd[kd] + (uint64_t)(((hb * 4 + kh) * WT * W0 + k * 32) >> 4);
-                  const uint64_t bdesc = bdesc0 + (uint64_t)((st * WSTEP + k * 32) >> 4);
-                  umma_f16(tmem_d, adesc, bdesc, idesc, (st | k) ? 1u : 0u);
-                }
+            for (int g = 0; g < NW; ++g) {
+              // non-stacked: weight rows kw * COUT + pass * 16 (whole 8-row swizzle atoms)
+              const uint64_t bd = STACK ? bdesc : bdesc + (uint64_t)(((g * COUT + pass * CW) * wr) >> 4);
 #pragma unroll
-                for (int k = 0; k < G1 / 16; ++k) {
-                  const uint64_t adesc = adesc1_kd[kd] + (uint64_t)(((hb * 4 + kh) * WT * W1 + k * 32) >> 4);
-                  const uint64_t bdesc = bdesc1 + (uint64_t)((st * WSTEP + k * 32) >> 4);
-                  umma_f16(tmem_d, adesc, bdesc, idesc, 1u);
-                }
-              }
+              for (int hf = 0; hf < 2; ++hf)            // rows 64-127 of the tile: two slab rows further
+                Wgmma<NA, 0, 0>::mma(acc[hf][g], adesc + (uint64_t)((hf * 2 * WT * wr) >> 4), bd, (st | k) ? 1u : 0u);
             }
           }
-          umma_commit(&tfull[acc]);
-          if (hb == NH - 1) umma_commit(&empty[hslot]);
         }
-        __syncwarp();
-        if (++acc == (uint32_t)NACC) { acc = 0; aphase ^= 1; }
-        }
-        if (++hslot == (uint32_t)NSLOT) hslot = 0;
       }
+      wg_commit();
+      wg_wait<0>();
+    };
+    // v[c] = out[w'][pass * CW + cc + c] = P0[w'-1] + P1[w'] + P2[w'+1] (kw partial sums, shuffled across lanes)
+    auto combine = [&](float (&acc)[2][NW][NA / 2], int cc, float (&v)[16]) {
+      uint32_t r[16];
+      acc_row16(acc[0][0], acc[1][0], STACK ? cc : 0, stage, nbar, r);
+#pragma unroll
+      for (int c = 0; c < 16; ++c) v[c] = __shfl_up_sync(0xffffffffu, __uint_as_float(r[c]), 1);
+      acc_row16(acc[0][NW > 1 ? 1 : 0], acc[1][NW > 1 ? 1 : 0], STACK ? COUT + cc : 0, stage, nbar, r);
+#pragma unroll
+      for (int c = 0; c < 16; ++c) v[c] += __uint_as_float(r[c]);
+      acc_row16(acc[0][NW - 1], acc[1][NW - 1], STACK ? 2 * COUT + cc : 0, stage, nbar, r);
+#pragma unroll
+      for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, __uint_as_float(r[c]), 1);
+    };
+    auto release = [&](int nd) {                     // end of an item: slabs nd and nd + 1 of a 3-D window
       if (KD == 3) {
-        const uint32_t h1 = hslot + 1 == (uint32_t)NSLOT ? 0 : hslot + 1;
-        if (elect_one()) {
-          umma_commit(&empty[hslot]);
-          umma_commit(&empty[h1]);
+        observe(cnt_base + (uint32_t)nd + 1u);
+        if (lane == 0) {
+          mbar_arrive(&empty[(cnt_base + nd) % NSLOT]);
+          mbar_arrive(&empty[(cnt_base + nd + 1) % NSLOT]);
         }
-        __syncwarp();
-        hslot = h1 + 1 == (uint32_t)NSLOT ? 0 : h1 + 1;
+        cnt_base += nd + 2;
+      } else {
+        cnt_base += nd;
       }
-    }
-  } else {
-    // ================================ EPILOGUE (3 groups x 4 warps; warp = tile row hh, lane = w') ==================
-    // Group g drains the accumulators with (accumulator counter % 3) == g: the per-tile epilogue is a ~1300-cycle
-    // dependent chain (TMEM load, 32 shuffles, bias / activation / mask, pack, store), so three tiles are kept in
-    // flight; with two groups the epilogue, not the tensor pipe, bounds the thin layers (profiles/r1_*).
-    const int grp = warp >= 12 ? 2 : (warp >= 8 ? 1 : 0);
-    uint32_t turn = 0, tphase = 0;   // accumulator counter % NACC; phase of this group's tfull barrier
-    const int wq = warp & 3;
+    };
     if constexpr (EPI != 0) {
       const float slope = a.slope;
-      [[maybe_unused]] float bs[EPI == 1 ? COUT : 1];
-      if constexpr (EPI == 1) {
-#pragma unroll
-        for (int c = 0; c < COUT; ++c) bs[c] = a.bias ? __ldg(a.bias + c) : 0.f;
-      }
-      const uint32_t acc = (uint32_t)grp;
-      const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * (uint32_t)NN;
       const int c1 = (EPI == 3 && a.out2) ? a.csplit : COUT;       // channels [0, c1) -> out, [c1, COUT) -> out2
       const size_t HWp = (size_t)a.H * a.W;
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
         const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
         const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
+        const int nd = d1 - d0;
         const bool wok = lane >= 1 && lane <= WUSE && w < a.W;
         bool ok[NH];
         size_t vx[NH];                                           // voxel index of this lane in slice d0
@@ -289,11 +276,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
           ok[hb] = wok && h < a.H;
           vx[hb] = (((size_t)b * a.D + d0) * a.H + h) * a.W + w;
         }
-        for (int d = d0; d < d1; ++d) {
+        for (int j = 0; j < nd; ++j) {
+          observe(cnt_base + (uint32_t)j + (KD == 3 ? 2u : 0u));
+          const uint32_t hslot = (cnt_base + j) % NSLOT;
 #pragma unroll
           for (int hb = 0; hb < NH; ++hb) {
-            const bool mine = (int)turn == grp;
-            if (++turn == (uint32_t)NACC) turn = 0;
+            const bool mine = (int)(ecnt++ % NGRP) == grp;
             const size_t vox = vx[hb];
             vx[hb] += HWp;
             if (!mine) continue;
@@ -305,116 +293,86 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                 for (int q = 0; q < COUT / 16; ++q) ld_global_nc_v8(a.mask + vox * COUT + q * 16, mreg[q]);
               }
             }
-            mbar_wait(&tfull[acc], tphase);
-            tphase ^= 1;
-            tc_fence_after();
 #pragma unroll
-            for (int c0 = 0; c0 < COUT; c0 += 16) {
-              uint32_t r0[16], r1[16], r2[16];
-              tmem_ld16(taddr + c0, r0);
-              tmem_ld16(taddr + COUT + c0, r1);
-              tmem_ld16(taddr + 2 * COUT + c0, r2);
-              tmem_ld_wait();
-              if (c0 + 16 >= COUT) {          // last TMEM read of this accumulator
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&tempty[acc]);
-              }
-              float v[16];
+            for (int pass = 0; pass < NPASS; ++pass) {
+              float acc[2][NW][NA / 2];
+              mma(hslot, hb, pass, acc);
 #pragma unroll
-              for (int c = 0; c < 16; ++c) {
-                const float p0 = __shfl_up_sync(0xffffffffu, __uint_as_float(r0[c]), 1);
-                const float p2 = __shfl_down_sync(0xffffffffu, __uint_as_float(r2[c]), 1);
-                v[c] = (p0 + __uint_as_float(r1[c])) + p2;      // out[w'] = P0[w'-1] + P1[w'] + P2[w'+1]
-              }
-              if constexpr (EPI == 1) {
+              for (int cc = 0; cc < CW; cc += 16) {
+                const int c0 = pass * CW + cc;
+                float v[16];
+                combine(acc, cc, v);
+                if constexpr (EPI == 1) {
 #pragma unroll
-                for (int c = 0; c < 16; ++c) {
-                  const float x = v[c] + bs[c0 + c];
-                  v[c] = fmaxf(x, x * slope);                    // LeakyReLU for 0 <= slope <= 1
+                  for (int c = 0; c < 16; ++c) {
+                    const float x = v[c] + (a.bias ? __ldg(a.bias + c0 + c) : 0.f);
+                    v[c] = fmaxf(x, x * slope);                    // LeakyReLU for 0 <= slope <= 1
+                  }
+                } else if constexpr (EPI == 2) {
+#pragma unroll
+                  for (int e = 0; e < 8; ++e) {                    // sign bits of the saved bf16 activations
+                    const uint32_t mw = mreg[c0 / 16][e];
+                    if (mw & 0x8000u) v[2 * e] *= slope;
+                    if (mw & 0x80000000u) v[2 * e + 1] *= slope;
+                  }
                 }
-              } else if constexpr (EPI == 2) {
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {                    // sign bits of the saved bf16 activations
-                  const uint32_t mw = mreg[c0 / 16][e];
-                  if (mw & 0x8000u) v[2 * e] *= slope;
-                  if (mw & 0x80000000u) v[2 * e + 1] *= slope;
+                if (valid) {
+                  __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
+                                                              : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + c0;
+                  st_global_v8(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
+                               pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
                 }
-              }
-              if (valid) {
-                __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
-                                                            : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + c0;
-                uint4* op = reinterpret_cast<uint4*>(dst);
-                st_global_v8(op, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
-                             pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
               }
             }
           }
+          if (lane == 0) mbar_arrive(&empty[hslot]);    // this group no longer reads slab j
         }
+        release(nd);
       }
     } else {
     const size_t HWp = (size_t)a.H * a.W;
-    constexpr int NBR = COUT <= 32 ? COUT : 1;     // bias kept in registers for the (forward) layer widths
-    float biasr[NBR];
-#pragma unroll
-    for (int c = 0; c < NBR; ++c) biasr[c] = (a.bias && c < a.Cout) ? __ldg(a.bias + c) : 0.f;
-    auto bias_at = [&](int c) -> float { return COUT <= 32 ? biasr[COUT <= 32 ? c : 0] : (a.bias ? __ldg(a.bias + c) : 0.f); };
+    auto bias_at = [&](int c) -> float { return a.bias ? __ldg(a.bias + c) : 0.f; };
     for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
       const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
       const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
       const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
-      for (int d = d0; d < d1; ++d) {
+      const int nd = d1 - d0;
+      for (int j = 0; j < nd; ++j) {
+        const int d = d0 + j;
+        observe(cnt_base + (uint32_t)j + (KD == 3 ? 2u : 0u));
+        const uint32_t hslot = (cnt_base + j) % NSLOT;
 #pragma unroll
         for (int hb = 0; hb < NH; ++hb) {
-        {
-          const bool mine = (int)turn == grp;
-          if (++turn == (uint32_t)NACC) turn = 0;
-          if (!mine) continue;
-        }
+        if ((int)(ecnt++ % NGRP) != grp) continue;
         const int h = ht * HT + hb * 4 + wq;
         const bool valid = lane >= 1 && lane <= WUSE && h < a.H && w < a.W;
-        const uint32_t acc = (uint32_t)grp;
         const size_t vox = (((size_t)b * a.D + d) * a.H + h) * a.W + w;
-        // prefetch the LeakyReLU-derivative mask of this voxel before waiting for the tensor core
+        // prefetch the LeakyReLU-derivative mask of this voxel before the MMAs
         uint4 mreg[COUT / 8];
         if (a.mask && valid) {
 #pragma unroll
           for (int q = 0; q < COUT / 8; ++q)
             if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * a.Cout) + q);
         }
-        mbar_wait(&tfull[acc], tphase);
-        tphase ^= 1;
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * (uint32_t)NN;
         const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
-        // 16 output channels at a time: 3 x 16 TMEM columns (kw = 0,1,2), shuffle-combine across lanes, store
 #pragma unroll
-        for (int c0 = 0; c0 < COUT; c0 += 16) {
-          uint32_t r0[16], r1[16], r2[16];
+        for (int pass = 0; pass < NPASS; ++pass) {
+        float acc[2][NW][NA / 2];
+        mma(hslot, hb, pass, acc);
+        // 16 output channels at a time: the kw = 0, 1, 2 partial sums, shuffle-combined across lanes, stored
+#pragma unroll
+        for (int cc = 0; cc < CW; cc += 16) {
+          const int c0 = pass * CW + cc;
           [[maybe_unused]] float4 ain[ACC ? 4 : 1];
           if constexpr (ACC) {
-            if (a.acc_in && valid) {      // partial sums of the earlier split-precision passes (issued before the TMEM wait)
+            if (a.acc_in && valid) {      // partial sums of the earlier split-precision passes
               const float4* ap = reinterpret_cast<const float4*>(a.acc_in + vox * COUT + c0);
 #pragma unroll
               for (int q = 0; q < 4; ++q) ain[q] = __ldg(ap + q);
             }
           }
-          tmem_ld16(taddr + c0, r0);
-          tmem_ld16(taddr + COUT + c0, r1);
-          tmem_ld16(taddr + 2 * COUT + c0, r2);
-          tmem_ld_wait();
-          if (c0 + 16 >= COUT) {          // last TMEM read of this accumulator
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
-          }
           float v[16];
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            const float p0 = __shfl_up_sync(0xffffffffu, __uint_as_float(r0[c]), 1);
-            const float p2 = __shfl_down_sync(0xffffffffu, __uint_as_float(r2[c]), 1);
-            v[c] = (p0 + __uint_as_float(r1[c])) + p2;      // out[w'] = P0[w'-1] + P1[w'] + P2[w'+1]
-          }
+          combine(acc, cc, v);
           bool handled = false;
           if constexpr (ACC) {
             if (a.acc_in && valid) {
@@ -489,15 +447,12 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
           }
         }
         }
+        }
+        if (lane == 0) mbar_arrive(&empty[hslot]);    // this group no longer reads slab j
       }
+      release(nd);
     }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -685,6 +640,12 @@ extern "C" int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wp
                          nullptr, nullptr, stream);
 }
 
+extern "C" int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
+                                   int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
+                                   float slope, void* out2, int csplit, void* stream) {
+  return vxm_conv3d_tcs_fwd(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, out2, csplit, stream);
+}
+
 extern "C" int vxm_conv3d_tcs_fwd_acc(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
                                       const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp,
                                       int kd, int out_mode, float slope, void* stream) {
@@ -715,8 +676,8 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   a.B = B; a.D = D; a.H = H; a.W = W; a.Ca = Ca; a.Cb = Cb; a.up = up; a.upd = (up && kd == 3) ? 1 : 0;
   a.Cout = Cout; a.out_mode = out_mode; a.slope = slope;
   a.wbytes = (uint32_t)vxm_conv3d_tcs_packed_bytes(cin, coutp, kd);
-  const size_t fixed = ((a.wbytes + 1023u) & ~1023u) + 1024 + 512;
-  // tile height: 8 rows (two accumulators per slab step) when the ring still holds >= 5 slabs and 4 accumulators fit TMEM
+  const size_t fixed = ((a.wbytes + 1023u) & ~1023u) + NGRP * ACC_STAGE_FLOATS * sizeof(float) + 1024 + 512;
+  // tile height: 8 rows (two tile halves per slab step, one per MMA warpgroup) when the ring still holds >= 5 slabs
   int HTv = 4;
   {
     const size_t slab8 = (size_t)10 * WT * (g0 + g1) * 2;
@@ -742,8 +703,8 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   const size_t slab = (size_t)(HTv + 2) * WT * (g0 + g1) * 2;
   int nslot = (int)((227 * 1024 - fixed) / slab);
   {
-    // ring depth: the slabs of up to 13 steps ahead (16-channel layers) hide the L2 / HBM latency of the tensor copies — with 8
-    // slots the issuers waited ~550 clk per step for slab data (profiles/r2_conv_ablation.md).  VXM_B200_RING=8: A/B switch.
+    // ring depth: the slabs of up to 13 steps ahead (16-channel layers) hide the L2 / HBM latency of the tensor copies.
+    // VXM_B200_RING=8: A/B switch.
     const char* e = getenv("VXM_B200_RING");
     const int cap = e ? atoi(e) : MAXSLOT;
     if (nslot > cap) nslot = cap;

@@ -1,18 +1,20 @@
-// Conv3d k=3 on tcgen05, "kw-stacked" formulation — the faster engine for layers with Cout <= 32
+// Conv3d k=3 on the Hopper tensor cores (wgmma), "kw-stacked" formulation with SWIZZLE_NONE operands
 // (reference voxelmorph/torch/networks.py:299-304, :211,257; forward and dgrad).
 //
-// conv3d_tc.cu issues one 128 x Cout x 16 MMA per (tap, 16 channels) and is bound by re-reading its 4 KB activation
-// operand 27 times.  Here the three kw taps are stacked along the MMA N dimension:
+// conv3d_tc.cu issues one 128 x Cout x 16 MMA per (tap, 16 channels) and re-reads its activation operand 27 times.
+// Here the three kw taps are stacked along the MMA N dimension:
 //     D[128 voxels][(kw, co) : N = 3*Cout] += X_(kd,kh)[128 voxels][16 ch] * Wt[(kw,co)][16 ch]
 //   * the K loop runs over (kd, kh, Cin/16) only: 9*Cin/16 MMAs of N = 96 (48) per tile instead of 27*Cin/16 of N = 32
-//     (16): the activation operand is read 9 times instead of 27;
+//     (16): the activation operand is read 9 times instead of 27 (layers wider than 32 output channels run in passes of
+//     16 channels, one wgmma per kw, to keep the accumulators within the register budget);
 //   * the 128 M rows are 4 (h) x 32 (w') voxels of one d-slice; the slab [Cin/8][6 x 32 rows][8 ch] has a row pitch of
 //     32 voxels, so a (kd, kh) tap is a whole-row (512-byte) shift of the A operand start address;
-//   * TMEM lane = voxel, so each epilogue warp owns one 32-voxel row and the kw shift is a warp shuffle:
-//     out[w'][co] = D[w'-1][(0,co)] + D[w'][(1,co)] + D[w'+1][(2,co)]; lanes 0 and 31 are halo (30 useful outputs per
-//     row).  No shared-memory staging in the epilogue;
-//   * everything else (persistent warp-specialised CTA, cp.async loader with fused upsample / concat / zero padding,
-//     bulk-TMA weight load, TMEM double buffering, slab ring sliding along D) is as in conv3d_tc.cu.
+//   * after the accumulators are transposed to one voxel per thread, each epilogue warp owns one 32-voxel row and the
+//     kw shift is a warp shuffle: out[w'][co] = D[w'-1][(0,co)] + D[w'][(1,co)] + D[w'+1][(2,co)]; lanes 0 and 31 are
+//     halo (30 useful outputs per row);
+//   * two MMA + epilogue warpgroups take alternate tiles; everything else (persistent warp-specialised CTA, cp.async
+//     loader with fused upsample / concat / zero padding, bulk-TMA weight load, slab ring sliding along D) is as in
+//     conv3d_tc.cu.
 #include "tc_common.cuh"
 
 namespace vxm {
@@ -23,8 +25,8 @@ using namespace vxm::tc;
 constexpr int HT = 4, WT = 32, WUSE = 30;
 constexpr int SROWS = (HT + 2) * WT;   // 192 voxels per slab plane
 constexpr int TPLANE = SROWS * 16;     // 3072 bytes
-constexpr int MAXSLOT = 8, MAXACC = 4, KMAX = 16;
-constexpr int NLOADER = 96, NTHREADS = 384;   // warps 0-3 epilogue group 0, 4 MMA issuer, 5-7 loader, 8-11 epilogue group 1
+constexpr int MAXSLOT = 8, KMAX = 12;
+constexpr int NLOADER = 128, NTHREADS = 384;   // warps 0-3 / 4-7: MMA + epilogue groups 0 / 1, warps 8-11: loader
 
 struct ConvTArgs {
   const __nv_bfloat16* xa; const __nv_bfloat16* xb;
@@ -39,8 +41,6 @@ struct ConvTArgs {
 
 template <int KD, int NK16, int COUT>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_tct_kernel(const ConvTArgs a) {
-  constexpr int NN = 3 * COUT;   // MMA N: (kw, co)
-  constexpr int NACC = (4 * NN <= 512) ? 4 : 2;   // TMEM accumulators in flight (two epilogue groups alternate tiles)
   extern __shared__ __align__(128) uint8_t smem[];
   const bool halfk = (a.Ca + a.Cb == 8);
   const int nc8 = halfk ? 1 : NK16 * 2;
@@ -49,30 +49,23 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tct_kernel(const ConvTArgs a
   uint8_t* s_w = smem;
   uint8_t* s_slab = smem + ((a.wbytes + 127u) & ~127u);
   uint8_t* s_zero = s_slab + NSLOT * slab_bytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s_zero + TPLANE);
+  float* s_stage = reinterpret_cast<float*>(s_zero + TPLANE);   // one accumulator read-out buffer per group
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + 2 * ACC_STAGE_FLOATS);
   uint64_t* full = bars;
   uint64_t* empty = bars + MAXSLOT;
-  uint64_t* tfull = bars + 2 * MAXSLOT;
-  uint64_t* tempty = tfull + MAXACC;
-  uint64_t* wbar = tempty + MAXACC;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(wbar + 1);
+  uint64_t* wbar = empty + MAXSLOT;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  constexpr uint32_t tmem_cols = NACC * NN <= 128 ? 128u : (NACC * NN <= 256 ? 256u : 512u);
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], NLOADER); mbar_init(&empty[i], 1); }
-    for (int i = 0; i < NACC; ++i) { mbar_init(&tfull[i], 1); mbar_init(&tempty[i], 128); }
+    // empty: one arrival per warp of both groups (each group releases every slab once, see below)
+    for (int i = 0; i < NSLOT; ++i) { mbar_init(&full[i], NLOADER); mbar_init(&empty[i], 8); }
     mbar_init(wbar, 1);
     fence_barrier_init();
   }
   for (int i = threadIdx.x; i < TPLANE / 16; i += NTHREADS) reinterpret_cast<uint4*>(s_zero)[i] = make_uint4(0, 0, 0, 0);
   fence_proxy_async();
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (threadIdx.x == 0) {
     mbar_expect_tx(wbar, a.wbytes);
@@ -83,9 +76,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tct_kernel(const ConvTArgs a
   }
   const int HW_tiles = a.tiles_h * a.tiles_w;
 
-  if (warp >= 5 && warp < 8) {
-    // ================================ LOADER (96 threads) ================================
-    const int lt = threadIdx.x - 5 * 32;
+  if (warp >= 8) {
+    // ================================ LOADER (128 threads) ================================
+    setmaxnreg_dec<64>();
+    const int lt = threadIdx.x - 8 * 32;
     uint32_t cnt = 0;
     const int Da = a.upd ? a.D >> 1 : a.D, Ha = a.up ? a.H >> 1 : a.H, Wa = a.up ? a.W >> 1 : a.W;
     const int nca8 = a.Ca >> 3;
@@ -133,167 +127,156 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tct_kernel(const ConvTArgs a
         ++cnt;
       }
     }
-  } else if (warp == 4) {
-    // ================================ MMA ISSUER (whole warp, one elected lane) ================================
-    constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(NN >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
+  } else {
+    // ================================ MMA + EPILOGUE (2 warpgroups; warp = tile row hh, lane = w') ==================
+    // Group g issues and drains the tiles with (tile counter & 1) == g, so the tensor core works on one group's tile
+    // while the other group runs its epilogue (global-memory latencies of mask prefetch and stores).
+    // Slab release: every group walks ALL slabs in order (waiting for each one's full phase) and arrives once on each
+    // slab's empty barrier after its last MMA reading it has completed, so a slot is refilled only after both groups
+    // are past it and no barrier phase can alias.
+    setmaxnreg_inc<216>();
+    const int grp = warp >> 2;
+    const int wq = warp & 3;
+    float* stage = s_stage + grp * ACC_STAGE_FLOATS;
+    const int nbar = 1 + grp;
+    // MMA N per wgmma: the three kw taps stacked (N = 3 * COUT) up to COUT = 32; wider layers run in passes of 16
+    // output channels with one wgmma per kw (the accumulators of a pass stay within the register budget)
+    constexpr bool STACK = COUT <= 32;
+    constexpr int CW = STACK ? COUT : 16;            // output channels per pass
+    constexpr int NPASS = COUT / CW;
+    constexpr int NA = STACK ? 3 * COUT : CW;        // N of one wgmma
+    constexpr int NW = STACK ? 1 : 3;                // wgmmas per K step and tile half
     const uint32_t slab_u32 = smem_u32(s_slab), w_u32 = smem_u32(s_w);
     const uint32_t a_lbo0 = halfk ? (smem_u32(s_zero) - slab_u32) : (uint32_t)TPLANE;
-    constexpr uint32_t b_step16 = (uint32_t)NN * 32u / 16u;
+    constexpr uint32_t NN = 3 * COUT;
+    constexpr uint32_t b_step16 = NN * 32u / 16u;
+    constexpr uint32_t half16 = 2u * WT;             // rows 64-127: two slab rows further, in 16-byte units
     mbar_wait(wbar, 0);
-    const uint64_t bdesc0 = make_desc_kmajor_noswz(w_u32, (uint32_t)NN * 16u, 128u);
-    uint32_t cnt_base = 0, acc_cnt = 0;
+    const uint64_t bdesc0 = make_desc_kmajor_noswz(w_u32, NN * 16u, 128u);
+    uint32_t cnt_base = 0, tcnt = 0, wcur = 0;
+    auto observe = [&](uint32_t upto) {              // wait for every slab up to global index `upto`, in order
+      for (; wcur <= upto; ++wcur) mbar_wait(&full[wcur % NSLOT], (wcur / NSLOT) & 1);
+    };
+    const size_t HWp = (size_t)a.H * a.W;
+    auto bias_at = [&](int c) -> float { return a.bias ? __ldg(a.bias + c) : 0.f; };
     for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-      const int ch = (item / HW_tiles) % a.nchunks;
-      const int d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
+      const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
+      const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
+      const int h = ht * HT + wq, w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
       const int nd = d1 - d0;
-      for (int j = 0; j < nd; ++j) {
-        if (KD == 3) {
-          if (j == 0) for (int q = 0; q < 2; ++q) { uint32_t c = cnt_base + q; mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1); }
-          uint32_t c = cnt_base + j + 2;
-          mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
-        } else {
-          uint32_t c = cnt_base + j;
-          mbar_wait(&full[c % NSLOT], (c / NSLOT) & 1);
-        }
-        const uint32_t acc = acc_cnt % NACC;
-        mbar_wait(&tempty[acc], ((acc_cnt / NACC) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t tmem_d = tmem_base + acc * (uint32_t)NN;
-        uint64_t adesc_kd[KD];
+      const bool valid = lane >= 1 && lane <= WUSE && h < a.H && w < a.W;
+      for (int j = 0; j < nd; ++j, ++tcnt) {
+        const int d = d0 + j;
+        observe(cnt_base + (uint32_t)j + (KD == 3 ? 2u : 0u));
+        if ((int)(tcnt & 1) == grp) {
+          const size_t vox = (((size_t)b * a.D + d) * a.H + h) * a.W + w;
+          // prefetch the LeakyReLU-derivative mask of this voxel before the MMAs
+          uint4 mreg[COUT / 8];
+          if (a.mask && valid) {
 #pragma unroll
-        for (int kd = 0; kd < KD; ++kd) {
-          const uint32_t sl = (cnt_base + j + kd) % NSLOT;
-          adesc_kd[kd] = make_desc_kmajor_noswz(slab_u32 + sl * slab_bytes, halfk ? (a_lbo0 - sl * slab_bytes) : a_lbo0, 128u);
-        }
-        if (elect_one()) {
+            for (int q = 0; q < COUT / 8; ++q)
+              if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * a.Cout) + q);
+          }
+          uint64_t adesc_kd[KD];
 #pragma unroll
           for (int kd = 0; kd < KD; ++kd) {
+            const uint32_t sl = (cnt_base + j + kd) % NSLOT;
+            adesc_kd[kd] = make_desc_kmajor_noswz(slab_u32 + sl * slab_bytes, halfk ? (a_lbo0 - sl * slab_bytes) : a_lbo0, 128u);
+          }
+          const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
 #pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
+          for (int pass = 0; pass < NPASS; ++pass) {
+            float acc[2][NW][NA / 2];
+            wg_fence();
 #pragma unroll
-              for (int k = 0; k < NK16; ++k) {
-                const int step = (kd * 3 + kh) * NK16 + k;
-                const uint64_t adesc = adesc_kd[kd] + (uint64_t)(kh * WT + k * (2 * TPLANE / 16));   // 16-byte units
-                const uint64_t bdesc = bdesc0 + (uint64_t)(step * b_step16);
-                umma_f16(tmem_d, adesc, bdesc, idesc, step ? 1u : 0u);
+            for (int kd = 0; kd < KD; ++kd) {
+#pragma unroll
+              for (int kh = 0; kh < 3; ++kh) {
+#pragma unroll
+                for (int k = 0; k < NK16; ++k) {
+                  const int step = (kd * 3 + kh) * NK16 + k;
+                  const uint64_t adesc = adesc_kd[kd] + (uint64_t)(kh * WT + k * (2 * TPLANE / 16));   // 16-byte units
+                  const uint64_t bdesc = bdesc0 + (uint64_t)(step * b_step16);
+#pragma unroll
+                  for (int g = 0; g < NW; ++g) {
+                    // non-stacked: rows kw * COUT + pass * 16 of the packed weights (8-row groups 128 bytes apart)
+                    const uint64_t bd = STACK ? bdesc : bdesc + (uint64_t)(((g * COUT + pass * CW) / 8) * 8);
+#pragma unroll
+                    for (int hf = 0; hf < 2; ++hf) Wgmma<NA, 0, 0>::mma(acc[hf][g], adesc + hf * half16, bd, step ? 1u : 0u);
+                  }
+                }
+              }
+            }
+            wg_commit();
+            wg_wait<0>();
+            // 16 output channels at a time: the kw = 0, 1, 2 partial sums, shuffle-combined across lanes, stored
+#pragma unroll
+            for (int cc = 0; cc < CW; cc += 16) {
+              const int c0 = pass * CW + cc;
+              // one 16-column read-out at a time (register budget): out[w'] = P0[w'-1] + P1[w'] + P2[w'+1]
+              uint32_t r[16];
+              float v[16];
+              acc_row16(acc[0][0], acc[1][0], STACK ? cc : 0, stage, nbar, r);
+#pragma unroll
+              for (int c = 0; c < 16; ++c) v[c] = __shfl_up_sync(0xffffffffu, __uint_as_float(r[c]), 1);
+              acc_row16(acc[0][NW > 1 ? 1 : 0], acc[1][NW > 1 ? 1 : 0], STACK ? COUT + cc : 0, stage, nbar, r);
+#pragma unroll
+              for (int c = 0; c < 16; ++c) v[c] += __uint_as_float(r[c]);
+              acc_row16(acc[0][NW - 1], acc[1][NW - 1], STACK ? 2 * COUT + cc : 0, stage, nbar, r);
+#pragma unroll
+              for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, __uint_as_float(r[c]), 1);
+              if (valid && c0 < a.Cout) {
+                if (a.out_mode == 0) {
+#pragma unroll
+                  for (int q = 0; q < 16; q += 8) {
+                    if (c0 + q < a.Cout) {
+                      float x[8];
+#pragma unroll
+                      for (int e = 0; e < 8; ++e) x[e] = v[q + e] + bias_at(c0 + q + e);
+                      if (a.mask) {
+                        const uint4 m4 = mreg[(c0 + q) / 8];
+                        const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) if (__bfloat162float(mb[e]) < 0.f) x[e] *= a.slope;
+                      } else if (a.slope >= 0.f) {
+#pragma unroll
+                        for (int e = 0; e < 8; ++e) x[e] = x[e] >= 0.f ? x[e] : x[e] * a.slope;
+                      }
+                      // a split never falls inside a group of 8 channels (csplit % 8 == 0)
+                      const int cg = c0 + q;
+                      __nv_bfloat16* oo = cg < c1 ? reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + cg
+                                                  : reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (a.Cout - c1) + (cg - c1);
+                      *reinterpret_cast<uint4*>(oo) = make_uint4(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]), pack_bf16x2(x[4], x[5]), pack_bf16x2(x[6], x[7]));
+                    }
+                  }
+                } else {
+                  float* o = reinterpret_cast<float*>(a.out);
+#pragma unroll
+                  for (int c = 0; c < 16; ++c) {
+                    if (c0 + c < a.Cout) {
+                      float x = v[c] + bias_at(c0 + c);
+                      if (a.slope >= 0.f) x = x >= 0.f ? x : x * a.slope;
+                      o[(((size_t)b * a.Cout + c0 + c) * a.D + d) * HWp + (size_t)h * a.W + w] = x;
+                    }
+                  }
+                }
               }
             }
           }
-          umma_commit(&tfull[acc]);
-          umma_commit(&empty[(cnt_base + j) % NSLOT]);
         }
-        __syncwarp();
-        ++acc_cnt;
+        if (lane == 0) mbar_arrive(&empty[(cnt_base + j) % NSLOT]);   // this group no longer reads slab j
       }
       if (KD == 3) {
-        if (elect_one()) {
-          umma_commit(&empty[(cnt_base + nd) % NSLOT]);
-          umma_commit(&empty[(cnt_base + nd + 1) % NSLOT]);
+        observe(cnt_base + (uint32_t)nd + 1u);
+        if (lane == 0) {
+          mbar_arrive(&empty[(cnt_base + nd) % NSLOT]);
+          mbar_arrive(&empty[(cnt_base + nd + 1) % NSLOT]);
         }
-        __syncwarp();
         cnt_base += nd + 2;
       } else {
         cnt_base += nd;
       }
     }
-  } else {
-    // ================================ EPILOGUE (2 groups x 4 warps; warp = tile row hh, lane = w') ==================
-    // Group g drains the tiles with (tile counter & 1) == g, so two tiles are in flight and the global-memory
-    // latencies of one (mask prefetch, stores) hide behind the other.
-    const int grp = warp >= 8 ? 1 : 0;
-    const int wq = warp & 3;
-    uint32_t acc_cnt = 0;
-    const size_t HWp = (size_t)a.H * a.W;
-    constexpr int NBR = COUT <= 32 ? COUT : 1;     // bias kept in registers for the (forward) layer widths
-    float biasr[NBR];
-#pragma unroll
-    for (int c = 0; c < NBR; ++c) biasr[c] = (a.bias && c < a.Cout) ? __ldg(a.bias + c) : 0.f;
-    auto bias_at = [&](int c) -> float { return COUT <= 32 ? biasr[COUT <= 32 ? c : 0] : (a.bias ? __ldg(a.bias + c) : 0.f); };
-    for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-      const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
-      const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
-      const int h = ht * HT + wq, w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
-      const bool valid = lane >= 1 && lane <= WUSE && h < a.H && w < a.W;
-      for (int d = d0; d < d1; ++d) {
-        if ((int)(acc_cnt & 1) != grp) { ++acc_cnt; continue; }
-        const uint32_t acc = acc_cnt % NACC;
-        const size_t vox = (((size_t)b * a.D + d) * a.H + h) * a.W + w;
-        // prefetch the LeakyReLU-derivative mask of this voxel before waiting for the tensor core
-        uint4 mreg[COUT / 8];
-        if (a.mask && valid) {
-#pragma unroll
-          for (int q = 0; q < COUT / 8; ++q)
-            if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * a.Cout) + q);
-        }
-        mbar_wait(&tfull[acc], (acc_cnt / NACC) & 1);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + ((uint32_t)(wq * 32) << 16) + acc * (uint32_t)NN;
-        const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
-        // 16 output channels at a time: 3 x 16 TMEM columns (kw = 0,1,2), shuffle-combine across lanes, store
-#pragma unroll
-        for (int c0 = 0; c0 < COUT; c0 += 16) {
-          uint32_t r0[16], r1[16], r2[16];
-          tmem_ld16(taddr + c0, r0);
-          tmem_ld16(taddr + COUT + c0, r1);
-          tmem_ld16(taddr + 2 * COUT + c0, r2);
-          tmem_ld_wait();
-          if (c0 + 16 >= COUT) {          // last TMEM read of this accumulator
-            tc_fence_before();
-            mbar_arrive(&tempty[acc]);
-          }
-          float v[16];
-#pragma unroll
-          for (int c = 0; c < 16; ++c) {
-            const float p0 = __shfl_up_sync(0xffffffffu, __uint_as_float(r0[c]), 1);
-            const float p2 = __shfl_down_sync(0xffffffffu, __uint_as_float(r2[c]), 1);
-            v[c] = (p0 + __uint_as_float(r1[c])) + p2;      // out[w'] = P0[w'-1] + P1[w'] + P2[w'+1]
-          }
-          if (valid && c0 < a.Cout) {
-            if (a.out_mode == 0) {
-#pragma unroll
-              for (int q = 0; q < 16; q += 8) {
-                if (c0 + q < a.Cout) {
-                  float x[8];
-#pragma unroll
-                  for (int e = 0; e < 8; ++e) x[e] = v[q + e] + bias_at(c0 + q + e);
-                  if (a.mask) {
-                    const uint4 m4 = mreg[(c0 + q) / 8];
-                    const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) if (__bfloat162float(mb[e]) < 0.f) x[e] *= a.slope;
-                  } else if (a.slope >= 0.f) {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) x[e] = x[e] >= 0.f ? x[e] : x[e] * a.slope;
-                  }
-                  // a split never falls inside a group of 8 channels (csplit % 8 == 0)
-                  const int cg = c0 + q;
-                  __nv_bfloat16* oo = cg < c1 ? reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + cg
-                                              : reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (a.Cout - c1) + (cg - c1);
-                  *reinterpret_cast<uint4*>(oo) = make_uint4(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]), pack_bf16x2(x[4], x[5]), pack_bf16x2(x[6], x[7]));
-                }
-              }
-            } else {
-              float* o = reinterpret_cast<float*>(a.out);
-#pragma unroll
-              for (int c = 0; c < 16; ++c) {
-                if (c0 + c < a.Cout) {
-                  float x = v[c] + bias_at(c0 + c);
-                  if (a.slope >= 0.f) x = x >= 0.f ? x : x * a.slope;
-                  o[(((size_t)b * a.Cout + c0 + c) * a.D + d) * HWp + (size_t)h * a.W + w] = x;
-                }
-              }
-            }
-          }
-        }
-        ++acc_cnt;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, tmem_cols);
   }
 }
 
@@ -375,7 +358,7 @@ extern "C" int vxm_conv3d_tct_fwd(const void* xa, const void* xb, const void* wp
   a.wbytes = (uint32_t)vxm_conv3d_tct_packed_bytes(nk16 * 16, coutp, kd);
   const int nc8 = cin == 8 ? 1 : cin / 8;
   VXM_REQUIRE(nc8 * SROWS <= KMAX * NLOADER, "conv3d_tct_fwd: slab too large for the loader table");
-  size_t fixed = ((a.wbytes + 127u) & ~127u) + TPLANE + 512;
+  size_t fixed = ((a.wbytes + 127u) & ~127u) + TPLANE + 2 * ACC_STAGE_FLOATS * sizeof(float) + 512;
   int nslot = (int)((227 * 1024 - fixed) / ((size_t)nc8 * TPLANE));
   if (nslot > MAXSLOT) nslot = MAXSLOT;
   VXM_REQUIRE(nslot >= 4, "conv3d_tct_fwd: not enough shared memory for the slab ring");

@@ -1,16 +1,19 @@
-// Weight gradient of the k=3 convolution on tcgen05 tensor cores:
+// Weight gradient of the k=3 convolution on the Hopper tensor cores (wgmma):
 //     gw[tap][ci][co] = sum_{b,v} x[b, v + tap - 1, ci] * gz[b, v, co]          (gz = grad wrt the conv output)
-// (autograd of nn.Conv3d at reference voxelmorph/torch/networks.py:299,211).
+// (autograd of nn.Conv3d at reference voxelmorph/torch/networks.py:299,211).  The general path: planar fp32 sources and
+// channel counts conv3d_tc_wgrad2.cu does not take.
 //
 // Per (tap, 16 voxels) one MMA  D[64 x N] += A^T[64 ch x 16 vox] * B[16 vox x N]  with both operands
 // "MN-major" straight out of the channels-last slabs the forward kernel also uses:
 //   A = x slab  [Cin/8][180 rows][8 ch]  (halo'd 18 x 10 voxels of one input slice; the tap is a start-address
 //       offset; K = voxels: 8 consecutive w are 16 B apart = one core matrix, the next K group is the next h row)
 //   B = gz tile [Cout/8][128 rows][8 ch] (16 x 8 voxels, no halo)
-// M = 64 accumulator tiles use 16 of every 32 TMEM lanes, so two taps share one column range (lane offset 16):
-// all 27 tap accumulators (27 x 64 x N fp32) stay resident in TMEM for the CTA's whole lifetime; each CTA
-// streams its share of the volume, then writes ONE partial [27][64][N]; a second kernel reduces the partials
-// over CTAs in fixed order (deterministic) into the fp32 (Cout,Cin,kd,3,3) gradient.
+// The nine (kh, kw) tap accumulators of one kd (9 x 64 x N fp32) stay in the registers of two MMA warpgroups for the
+// CTA's whole lifetime (grid.y = kd); each CTA streams its share of the volume, then writes its taps of ONE partial
+// [27][64][N]; a second kernel reduces the partials over CTAs in fixed order (deterministic) into the fp32
+// (Cout,Cin,kd,3,3) gradient.
+#include <type_traits>
+
 #include "tc_common.cuh"
 
 namespace vxm {
@@ -20,7 +23,7 @@ constexpr int WTH = 16, WTW = 8, WSW = WTW + 2, WSH = WTH + 2;
 constexpr int WROWS = WSH * WSW, WPLANE = WROWS * 16;   // x slab plane: 180 rows
 constexpr int GPLANE = 128 * 16;                        // gz tile plane: 128 rows
 constexpr int WMAXSLOT = 8, WNG = 4, WKMAX = 12;
-constexpr int WNLOADER = 128, WNTHREADS = 288;
+constexpr int WNLOADER = 128, WNTHREADS = 384;   // warps 0-3 / 4-7: MMA warpgroups (0-3 also sum the bias), 8-11: loader
 
 struct WgradTcArgs {
   const __nv_bfloat16* xa; const __nv_bfloat16* xb;
@@ -34,14 +37,12 @@ struct WgradTcArgs {
   int tiles_h, tiles_w, dchunk, nchunks, nitems, nslot;
 };
 
-// STK > 0 (= channel chunks per slab, 1/2/4; KD == 3 only): the three kd taps are STACKED along M — the slabs of
-// consecutive input slices are adjacent in shared memory, so one operand of 3*STK channel chunks (stride = one plane)
-// spans slices d-1, d, d+1 and a single MMA accumulates all three kd taps: 72 MMAs per 128-voxel tile instead of 216.
-// The ring carries two mirror slots (copies of slots 0 and 1) so that a 3-slab window never wraps.
-template <int KD, int NP, int STK>
+// Grid (gx, KD): CTA (x, kd) accumulates the nine (kh, kw) taps of input-slice offset kd over its share x of the volume
+// (the x slabs of a share are staged once per kd), split over its two MMA warpgroups (taps 0-4 / 5-8): all nine
+// M = 64 x N = NP accumulators stay in registers for the CTA's lifetime.
+template <int KD, int NP>
 __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArgs a) {
-  constexpr int SM = STK == 0 ? 64 : (3 * STK <= 8 ? 64 : 128);   // MMA M
-  constexpr int NMIRROR = STK ? 2 : 0;
+  constexpr int NTAP = 5;                                  // accumulators per warpgroup (taps 5g .. 5g + 4, < 9)
   extern __shared__ __align__(128) uint8_t smem[];
   const bool px = a.nplanar_x > 0, pg = a.nplanar_g > 0;
   const int nc8 = px ? 1 : (a.Ca + a.Cb) / 8;
@@ -51,37 +52,30 @@ __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArg
   uint8_t* s_slab = smem;
   const int WNSLOT = a.nslot;
   // tail padding so that the M=64 operand (8 channel planes) never reads past the allocation
-  uint8_t* s_g = s_slab + (WNSLOT + NMIRROR) * slab_bytes + 16 * WPLANE;
+  uint8_t* s_g = s_slab + WNSLOT * slab_bytes + 16 * WPLANE;
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_g + WNG * gt_bytes + 4 * GPLANE);
   uint64_t* xfull = bars;
   uint64_t* xempty = bars + WMAXSLOT;
   uint64_t* gfull = bars + 2 * WMAXSLOT;
   uint64_t* gempty = gfull + WNG;
-  uint64_t* done = gempty + WNG;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int T = KD * 9, npairs = STK ? 5 : (T + 1) / 2;
-  const uint32_t need_cols = (STK && SM == 128) ? 9u * NP : (uint32_t)npairs * NP;
-  const uint32_t tmem_cols = need_cols <= 32 ? 32u : need_cols <= 64 ? 64u : need_cols <= 128 ? 128u : need_cols <= 256 ? 256u : 512u;
+  const int T = KD * 9;
+  const int kdc = blockIdx.y;                              // this CTA's kd tap
 
   if (threadIdx.x == 0) {
-    for (int i = 0; i < WNSLOT; ++i) { mbar_init(&xfull[i], WNLOADER); mbar_init(&xempty[i], 1); }
-    for (int i = 0; i < WNG; ++i) { mbar_init(&gfull[i], WNLOADER); mbar_init(&gempty[i], 1 + 128); }
-    mbar_init(done, 1);
+    // one arrival per warp of both MMA warpgroups, after its last MMA reading the slab has completed
+    for (int i = 0; i < WNSLOT; ++i) { mbar_init(&xfull[i], WNLOADER); mbar_init(&xempty[i], 8); }
+    for (int i = 0; i < WNG; ++i) { mbar_init(&gfull[i], WNLOADER); mbar_init(&gempty[i], 8); }
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int HW_tiles = a.tiles_h * a.tiles_w;
   const bool has_work = blockIdx.x < a.nitems;
 
-  if (warp >= 5) {
+  if (warp >= 8) {
     // ================================ LOADER ================================
-    const int lt = threadIdx.x - 5 * 32;
+    const int lt = threadIdx.x - 8 * 32;
     uint32_t xcnt = 0, gcnt = 0;
     const int Da = a.upd ? a.D >> 1 : a.D, Ha = a.up ? a.H >> 1 : a.H, Wa = a.up ? a.W >> 1 : a.W;
     const int nca8 = a.Ca >> 3;
@@ -143,7 +137,6 @@ __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArg
               const bool ok = dok && soff[k] >= 0;
               const __nv_bfloat16* src = ok ? ((soff[k] & 1) ? baseB : baseA) + (soff[k] >> 1) : dummy;
               cp_async16(slab + doff[k], src, ok ? 16u : 0u);
-              if (STK && slot < NMIRROR) cp_async16(slab + (size_t)WNSLOT * slab_bytes + doff[k], src, ok ? 16u : 0u);
             }
           }
           cp_async_arrive_noinc(&xfull[slot]);
@@ -159,7 +152,6 @@ __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArg
             }
             const uint4 q = make_uint4(pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), 0u, 0u);
             *reinterpret_cast<uint4*>(slab + row * 16) = q;
-            if (STK && slot < NMIRROR) *reinterpret_cast<uint4*>(slab + (size_t)WNSLOT * slab_bytes + row * 16) = q;
           }
           fence_proxy_async();
           mbar_arrive(&xfull[slot]);
@@ -198,13 +190,21 @@ __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArg
         }
       }
     }
-  } else if (warp == 4) {
-    // ================================ MMA ISSUER ================================
-    if (has_work) {   // whole warp, warp-uniform; one elected lane issues
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(64 >> 4) << 24);
+  } else {
+    // ================================ MMA WARPGROUPS ================================
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;
+    const int tap0 = wg * NTAP, ntap = wg == 0 ? NTAP : 9 - NTAP;
+    float acc[NTAP][NP / 2];
+    // warpgroup 0 of the kd = 0 CTAs also folds the bias gradient out of the staged gz tiles: thread t owns tile row t
+    float bsum[NP];
+#pragma unroll
+    for (int c = 0; c < NP; ++c) bsum[c] = 0.f;
+    const bool do_bias = wg == 0 && kdc == 0;
+    if (has_work) {
       const uint32_t slab_u32 = smem_u32(s_slab), g_u32 = smem_u32(s_g);
       uint32_t xbase = 0, gcnt = 0;
-      bool first_tile = true;
+      uint32_t acc0 = 0;                // 0 only for the very first tile of this CTA
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int ch = (item / HW_tiles) % a.nchunks;
         const int d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
@@ -220,194 +220,93 @@ __global__ void __launch_bounds__(WNTHREADS, 1) wgrad_tc_kernel(const WgradTcArg
           }
           const uint32_t gs = gcnt % WNG;
           mbar_wait(&gfull[gs], (gcnt / WNG) & 1);
-          tc_fence_after();
           const uint64_t bdesc0 = make_desc_mnmajor_noswz(g_u32 + gs * gt_bytes, 128u, (uint32_t)GPLANE);
-          uint64_t adesc_kd[KD];
+          const uint64_t adesc = make_desc_mnmajor_noswz(slab_u32 + ((xbase + j + kdc) % WNSLOT) * slab_bytes, (uint32_t)WSW * 16u, (uint32_t)WPLANE);
+          // one straight-line wgmma chain per warpgroup (no warpgroup-divergent branch inside a chain): NT taps from tap0
+          auto chain = [&](auto nt) {
+            constexpr int NT = decltype(nt)::value;
+            wg_fence();
 #pragma unroll
-          for (int kd = 0; kd < KD; ++kd)
-            adesc_kd[kd] = make_desc_mnmajor_noswz(slab_u32 + ((xbase + j + kd) % WNSLOT) * slab_bytes, (uint32_t)WSW * 16u, (uint32_t)WPLANE);
-          const uint32_t acc0 = first_tile ? 0u : 1u;
-          if constexpr (STK > 0) {
-            constexpr uint32_t idesc_s = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NP >> 3) << 17) | ((uint32_t)(SM >> 4) << 24);
-            // window = slabs of slices j, j+1, j+2, contiguous thanks to the mirror slots
-            const uint64_t adesc_w = make_desc_mnmajor_noswz(slab_u32 + ((xbase + j) % WNSLOT) * slab_bytes, (uint32_t)WSW * 16u, (uint32_t)WPLANE);
-            if (elect_one()) {
+            for (int s = 0; s < NT; ++s) {
+              const int t9 = tap0 + s, kh = t9 / 3, kw = t9 % 3;
 #pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-#pragma unroll
-                for (int kw = 0; kw < 3; ++kw) {
-                  const int t9 = kh * 3 + kw;
-                  const uint32_t tmem_d = SM == 128 ? tmem_base + (uint32_t)(t9 * NP)
-                                                    : tmem_base + ((uint32_t)((t9 & 1) * 16) << 16) + (uint32_t)((t9 >> 1) * NP);
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) {
-                    const uint64_t adesc = adesc_w + (uint64_t)((kh + 2 * i) * WSW + kw);
-                    const uint64_t bdesc = bdesc0 + (uint64_t)(2 * i * 128 / 16);
-                    umma_f16(tmem_d, adesc, bdesc, idesc_s, i == 0 ? acc0 : 1u);
-                  }
-                }
-              }
-              umma_commit(&xempty[(xbase + j) % WNSLOT]);
-              umma_commit(&gempty[gs]);
-            }
-          } else
-          if (elect_one()) {
-#pragma unroll
-            for (int kd = 0; kd < KD; ++kd) {
-#pragma unroll
-              for (int kh = 0; kh < 3; ++kh) {
-#pragma unroll
-                for (int kw = 0; kw < 3; ++kw) {
-                  const int tap = (kd * 3 + kh) * 3 + kw;
-                  const uint32_t tmem_d = tmem_base + ((uint32_t)((tap & 1) * 16) << 16) + (uint32_t)((tap >> 1) * NP);
-#pragma unroll
-                  for (int i = 0; i < 8; ++i) {   // 8 x 16 voxels = the 128-voxel tile; 16-byte address units
-                    const uint64_t adesc = adesc_kd[kd] + (uint64_t)((kh + 2 * i) * WSW + kw);
-                    const uint64_t bdesc = bdesc0 + (uint64_t)(2 * i * 128 / 16);
-                    umma_f16(tmem_d, adesc, bdesc, idesc, i == 0 ? acc0 : 1u);
-                  }
-                }
+              for (int i = 0; i < 8; ++i) {   // 8 x 16 voxels = the 128-voxel tile; 16-byte address units
+                const uint64_t ad = adesc + (uint64_t)((kh + 2 * i) * WSW + kw);
+                const uint64_t bd = bdesc0 + (uint64_t)(2 * i * 128 / 16);
+                Wgmma<NP, 1, 1>::mma(acc[s], ad, bd, i == 0 ? acc0 : 1u);
               }
             }
-            umma_commit(&xempty[(xbase + j) % WNSLOT]);
-            umma_commit(&gempty[gs]);
+            wg_commit();
+          };
+          if (wg == 0) chain(std::integral_constant<int, NTAP>{});
+          else chain(std::integral_constant<int, 9 - NTAP>{});
+          if (do_bias) {
+            const uint8_t* gt = s_g + (size_t)gs * gt_bytes + t * 16;
+#pragma unroll
+            for (int c8 = 0; c8 < NP / 8; ++c8) {
+              const uint4 q = *reinterpret_cast<const uint4*>(gt + (size_t)c8 * GPLANE);
+              const __nv_bfloat162* hq = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 f = __bfloat1622float2(hq[e]);
+                bsum[c8 * 8 + 2 * e] += f.x;
+                bsum[c8 * 8 + 2 * e + 1] += f.y;
+              }
+            }
           }
-          __syncwarp();
-          first_tile = false;
+          wg_wait<0>();
+          if (lane == 0) {
+            mbar_arrive(&xempty[(xbase + j) % WNSLOT]);
+            mbar_arrive(&gempty[gs]);
+          }
+          acc0 = 1u;
           ++gcnt;
         }
         if (KD == 3) {
-          if (elect_one()) {
-            umma_commit(&xempty[(xbase + nd) % WNSLOT]);
-            umma_commit(&xempty[(xbase + nd + 1) % WNSLOT]);
+          if (lane == 0) {
+            mbar_arrive(&xempty[(xbase + nd) % WNSLOT]);
+            mbar_arrive(&xempty[(xbase + nd + 1) % WNSLOT]);
           }
-          __syncwarp();
           xbase += nd + 2;
         } else {
           xbase += nd;
         }
       }
-      if (elect_one()) umma_commit(done);
-      __syncwarp();
     }
-  } else {
-    // ================================ EPILOGUE WARPS ================================
-    // While the tensor core works they fold the bias gradient (sum of gz over voxels) out of the staged gz tiles:
-    // thread r owns tile row r and accumulates its NP channels in registers.
-    float bsum[NP];
-#pragma unroll
-    for (int c = 0; c < NP; ++c) bsum[c] = 0.f;
-    if (has_work) {
-      uint32_t gcnt = 0;
-      const int rowi = warp * 32 + lane;
-      for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-        const int ch = (item / HW_tiles) % a.nchunks;
-        const int nd = min(ch * a.dchunk + a.dchunk, a.D) - ch * a.dchunk;
-        for (int j = 0; j < nd; ++j) {
-          const uint32_t gs = gcnt % WNG;
-          mbar_wait(&gfull[gs], (gcnt / WNG) & 1);
-          const uint8_t* gt = s_g + (size_t)gs * gt_bytes + rowi * 16;
-#pragma unroll
-          for (int c8 = 0; c8 < NP / 8; ++c8) {
-            const uint4 q = *reinterpret_cast<const uint4*>(gt + (size_t)c8 * GPLANE);
-            const __nv_bfloat162* hq = reinterpret_cast<const __nv_bfloat162*>(&q);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 f = __bfloat1622float2(hq[e]);
-              bsum[c8 * 8 + 2 * e] += f.x;
-              bsum[c8 * 8 + 2 * e + 1] += f.y;
-            }
-          }
-          mbar_arrive(&gempty[gs]);
-          ++gcnt;
-        }
-      }
-    }
+    // partial[x][tap][ci][co]: fragment (row ci, column co) of the accumulator of tap kd * 9 + t9
     float* part = a.partial + (size_t)blockIdx.x * T * 64 * NP;
-    const int ci = warp * 16 + (lane & 15);
-    if (has_work && STK > 0 && SM == 128) {
-      // rows = kd * (8*STK) + ci on TMEM lanes 0..127; columns t9 * NP
-      mbar_wait(done, 0);
-      tc_fence_after();
-      const int rowm = warp * 32 + lane, kd = rowm / (8 * STK), cis = rowm % (8 * STK);
-      for (int t9 = 0; t9 < 9; ++t9) {
-        for (int c0 = 0; c0 < NP; c0 += 8) {
-          uint32_t r[8];
-          const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)t9 * NP + c0;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                       : "r"(taddr) : "memory");
-          tmem_ld_wait();
-          if (kd < 3) {
-            float4* o = reinterpret_cast<float4*>(part + ((size_t)(kd * 9 + t9) * 64 + cis) * NP + c0);
-            o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-            o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-          }
-        }
-      }
-    } else if (has_work && STK > 0) {
-      // M = 64: rows kd * (8*STK) + ci on lanes (m % 16) + 32 * (m / 16); tap pairs share columns (lane offset 16)
-      mbar_wait(done, 0);
-      tc_fence_after();
-      const int rowm = warp * 16 + (lane & 15), kd = rowm / (8 * STK), cis = rowm % (8 * STK);
-      for (int p = 0; p < 5; ++p) {
-        const int t9 = 2 * p + (lane >> 4);
-        for (int c0 = 0; c0 < NP; c0 += 8) {
-          uint32_t r[8];
-          const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)p * NP + c0;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                       : "r"(taddr) : "memory");
-          tmem_ld_wait();
-          if (t9 < 9 && kd < 3) {
-            float4* o = reinterpret_cast<float4*>(part + ((size_t)(kd * 9 + t9) * 64 + cis) * NP + c0);
-            o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-            o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-          }
-        }
-      }
-    } else if (has_work) {
-      mbar_wait(done, 0);
-      tc_fence_after();
-      for (int p = 0; p < npairs; ++p) {
-        const int tap = 2 * p + (lane >> 4);
-        for (int c0 = 0; c0 < NP; c0 += 8) {
-          uint32_t r[8];
-          const uint32_t taddr = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)p * NP + c0;
-          asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                       : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-                       : "r"(taddr) : "memory");
-          tmem_ld_wait();
-          if (tap < T) {
-            float4* o = reinterpret_cast<float4*>(part + ((size_t)tap * 64 + ci) * NP + c0);
-            o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-            o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-          }
-        }
-      }
-    } else {
-      for (int i = threadIdx.x; i < T * 64 * NP; i += 128) part[i] = 0.f;
-    }
-    // bias partial of this CTA: deterministic reduction over the 128 rows through shared memory (the slab ring is idle now)
-    {
-      float* s_b = reinterpret_cast<float*>(s_slab);
-      const int rowi = warp * 32 + lane;
-      asm volatile("bar.sync 1, 128;" ::: "memory");
+    const int w4 = t >> 5, qr = lane >> 2, pc = lane & 3;
 #pragma unroll
-      for (int c = 0; c < NP; ++c) s_b[rowi * (NP + 1) + c] = bsum[c];
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (rowi < NP) {
-        float t = 0.f;
-        for (int r2 = 0; r2 < 128; ++r2) t += s_b[r2 * (NP + 1) + rowi];
-        a.bias_partial[(size_t)blockIdx.x * NP + rowi] = t;
+    for (int s = 0; s < NTAP; ++s) {
+      if (s >= ntap) break;
+      const int tap = kdc * 9 + tap0 + s;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int ci = 16 * w4 + 8 * i + qr;
+#pragma unroll
+        for (int jn = 0; jn < NP / 8; ++jn) {
+          const int co = 8 * jn + 2 * pc;
+          *reinterpret_cast<float2*>(part + ((size_t)tap * 64 + ci) * NP + co) =
+              has_work ? make_float2(acc[s][4 * jn + 2 * i], acc[s][4 * jn + 2 * i + 1]) : make_float2(0.f, 0.f);
+        }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, tmem_cols);
+    // bias partial of this CTA: deterministic reduction over the 128 rows through shared memory (the slab ring is idle
+    // once both warpgroups have passed their last wgmma wait)
+    if (kdc == 0) {
+      named_bar(1, 256);
+      if (wg == 0) {
+        float* s_b = reinterpret_cast<float*>(s_slab);
+#pragma unroll
+        for (int c = 0; c < NP; ++c) s_b[t * (NP + 1) + c] = bsum[c];
+        named_bar(2, 128);
+        if (t < NP) {
+          float sum = 0.f;
+          for (int r2 = 0; r2 < 128; ++r2) sum += s_b[r2 * (NP + 1) + t];
+          a.bias_partial[(size_t)blockIdx.x * NP + t] = sum;
+        }
+      }
+    }
   }
 }
 
@@ -538,26 +437,23 @@ extern "C" int vxm_conv3d_tc_wgrad(const void* xa, const void* xb, const float* 
   a.bias_partial = (float*)work + (size_t)256 * kd * 9 * 64 * 32;
   int nc8 = nplanar_x > 0 ? 1 : Cin / 8, ncg = nplanar_g > 0 ? 1 : Cg / 8;
   VXM_REQUIRE(nc8 * WROWS <= WKMAX * WNLOADER && ncg * 128 <= 4 * WNLOADER, "conv3d_tc_wgrad: tile too large for the loader table");
-  const int stk = (kd == 3 && (nc8 == 1 || nc8 == 2 || nc8 == 4)) ? nc8 : 0;
-  size_t fixed = 16 * WPLANE + (size_t)(stk ? 2 : 0) * nc8 * WPLANE + (size_t)WNG * ncg * GPLANE + 4 * GPLANE + 512;
+  size_t fixed = 16 * WPLANE + (size_t)WNG * ncg * GPLANE + 4 * GPLANE + 512;
   int nslot = (int)((200 * 1024 - fixed) / ((size_t)nc8 * WPLANE));
   if (nslot > WMAXSLOT) nslot = WMAXSLOT;
   VXM_REQUIRE(nslot >= 4, "conv3d_tc_wgrad: not enough shared memory for the slab ring");
   a.nslot = nslot;
   size_t smem = fixed + (size_t)nslot * nc8 * WPLANE;
   cudaStream_t st = as_stream(stream);
-#define VXM_WG_LAUNCH(KD_, NP_, STK_)                                                                                        \
-  do {                                                                                                                       \
-    VXM_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<KD_, NP_, STK_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    wgrad_tc_kernel<KD_, NP_, STK_><<<grid, WNTHREADS, smem, st>>>(a);                                                        \
+  const dim3 grid2(grid, kd);
+#define VXM_WG_LAUNCH(KD_, NP_)                                                                                        \
+  do {                                                                                                                 \
+    VXM_CUDA(cudaFuncSetAttribute(wgrad_tc_kernel<KD_, NP_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    wgrad_tc_kernel<KD_, NP_><<<grid2, WNTHREADS, smem, st>>>(a);                                                       \
   } while (0)
-#define VXM_WG_NP(KD_, STK_)                                                                                            \
-  do { if (a.NP == 8) VXM_WG_LAUNCH(KD_, 8, STK_); else if (a.NP == 16) VXM_WG_LAUNCH(KD_, 16, STK_); else VXM_WG_LAUNCH(KD_, 32, STK_); } while (0)
-  if (kd == 3) {
-    if (stk == 1) VXM_WG_NP(3, 1); else if (stk == 2) VXM_WG_NP(3, 2); else if (stk == 4) VXM_WG_NP(3, 4); else VXM_WG_NP(3, 0);
-  } else {
-    VXM_WG_NP(1, 0);
-  }
+#define VXM_WG_NP(KD_)                                                                                            \
+  do { if (a.NP == 8) VXM_WG_LAUNCH(KD_, 8); else if (a.NP == 16) VXM_WG_LAUNCH(KD_, 16); else VXM_WG_LAUNCH(KD_, 32); } while (0)
+  if (kd == 3) VXM_WG_NP(3);
+  else VXM_WG_NP(1);
   int rc = check_launch("conv3d_tc_wgrad");
   if (rc) return rc;
   int T = kd * 9;

@@ -1,10 +1,10 @@
-// Weight gradient of the k=3 convolution on tcgen05 tensor cores, "kw-stacked Toeplitz" formulation:
+// Weight gradient of the k=3 convolution on the Hopper tensor cores (wgmma), "kw-stacked Toeplitz" formulation:
 //     gw[kd][kh][kw][ci][co] = sum_{b,v} x[b, v + (kd,kh,kw) - 1, ci] * gz[b, v, co]
 // (autograd of nn.Conv3d at reference voxelmorph/torch/networks.py:299,211; gz = grad wrt the conv output).
 //
 // Both operands are staged exactly like the forward kernel's A operand (conv3d_tc_s.cu): one shared-memory row per
 // voxel, the channels of the row contiguous (32 or 64 bytes) and XOR-swizzled, rows of a 32-voxel-wide (h, w) tile
-// in linear order.  Read "MN-major" (MN = channels, K = voxels) the same bytes are a valid UMMA operand, and a
+// in linear order.  Read "MN-major" (MN = channels, K = voxels) the same bytes are a valid wgmma operand, and a
 // one-voxel shift of the window is a one-row shift of the start address.  One MMA then covers 16 voxels (K) and
 //   M = (kd, ci) : the x slabs of input slices d-1, d, d+1 are adjacent in the ring, so the three kd taps are three
 //                  MN atoms one slab apart (leading byte offset = slab pitch);
@@ -14,10 +14,13 @@
 // 24 MMAs per (tile, slice) instead of 72-216 in conv3d_tc_wgrad.cu, each with N = 48 or 96 instead of 16 or 32.
 // The x slab keeps its halo columns, the gz slab has ZERO halo columns (and zero pad rows before and after), so the
 // products that pair a voxel with a neighbour across the tile-row wrap vanish.
-// All 3 (kh) x [M x 3*GOUT] fp32 accumulators stay in TMEM for the CTA's whole lifetime; each CTA writes ONE partial
-// [27][G][GOUT]; wgrad2_reduce_kernel sums the partials in fixed order (deterministic).  The otherwise idle epilogue
-// warps fold the bias gradient (sum of gz) out of the staged gz rows.
+// All 3 (kh) x [M x 3*GOUT] fp32 accumulators stay in the registers of two MMA warpgroups for the CTA's whole lifetime
+// (M = 128: one m64 half each; M = 64: kh 0-1 / kh 2); each CTA writes ONE partial
+// [27][G][GOUT]; wgrad2_reduce_kernel sums the partials in fixed order (deterministic).  The first MMA warpgroup also
+// folds the bias gradient (sum of gz) out of the staged gz rows while its wgmma chain runs.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -30,7 +33,7 @@ constexpr int TH = 4, TWR = 32, TUSE = 30;
 constexpr int XROWS = (TH + 2) * TWR;                       // 192 voxel rows per x slab
 constexpr int GPAD = 16, GROWS = TH * TWR, GSROWS = GROWS + 2 * GPAD;   // gz slab: 16 zero rows, 128 rows, 16 zero rows
 constexpr int MAXSLOT = 8, NGS = 4;
-constexpr int NLOADER = 128, NTHREADS = 288;   // warps 0-3 bias + final epilogue, 4 MMA issuer, 5-8 loader
+constexpr int NLOADER = 128, NTHREADS = 384;   // warps 0-3 / 4-7: MMA warpgroups (0-3 also sum the bias), 8-11: loader
 
 struct Wgrad2Args {
   const __nv_bfloat16* x; int Cx, up, upd;   // (B, Dx, Hx, Wx, Cx) bf16, Cx in {8,16,32}; up: nearest x2 (H, W), upd: also D
@@ -39,7 +42,7 @@ struct Wgrad2Args {
   float* bias_partial;                       // [grid][GOUT] or null
   int B, D, H, W;
   int tiles_h, tiles_w, dchunk, nchunks, nitems, nslot;
-  int dbg;      // profiling only (VXM_B200_WGRAD_DBG): 1 = no MMAs issued, 2 = no slab copies, 4 = no bias sums
+  int dbg;      // profiling only (VXM_B200_WGRAD_DBG): 2 = no slab copies, 4 = no bias sums
 };
 
 __host__ __device__ inline uint32_t swz(uint32_t off, uint32_t width) { return off ^ (((off >> 7) & (width / 16 - 1)) << 4); }
@@ -47,21 +50,12 @@ __host__ __device__ inline uint32_t swz(uint32_t off, uint32_t width) { return o
 // MN-major swizzled operand: rows of WIDTH bytes (one voxel, WIDTH/2 channels = one MN atom), 8-row K groups contiguous
 // (SBO = 8 * WIDTH), MN atoms `lbo_bytes` apart.  cute make_umma_desc<Major::MN>: LBO = atom stride, SBO = K-group stride.
 template <int WIDTH>
-__device__ __forceinline__ uint64_t make_desc_mn_swz(uint32_t saddr, uint32_t lbo_bytes, uint32_t boff) {
+__device__ __forceinline__ uint64_t make_desc_mn_swz(uint32_t saddr, uint32_t lbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)(((8u * WIDTH) >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(boff & 7u) << 49;
-  d |= (uint64_t)(WIDTH == 128 ? 2 : (WIDTH == 64 ? 4 : 6)) << 61;
-  return d;
-}
-
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr) : "memory");
+  return d | desc_swizzle(WIDTH);    // base offset 0: the swizzle is a function of the absolute address
 }
 
 // KHM ("kh in M", KD == 1 only): the three kh taps become three MN atoms of the A operand ONE TILE ROW (32 voxel rows) apart —
@@ -80,8 +74,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
   constexpr int T = KD * 9;
   constexpr int KX = XROWS * (G / 8) / NLOADER, KG = GROWS * (GOUT / 8) / NLOADER;
   static_assert(XROWS * (G / 8) % NLOADER == 0 && GROWS * (GOUT / 8) % NLOADER == 0, "loader tables");
-  constexpr uint32_t need_cols = KHM ? NN : (MM == 128 ? 3 * NN : 2 * NN);
-  constexpr uint32_t tmem_cols = need_cols <= 128 ? 128u : (need_cols <= 256 ? 256u : 512u);
+  // Accumulators (fp32, registers): MM = 128 -> warpgroup g owns rows 64g..64g+63 of all three kh accumulators;
+  // MM = 64 -> warpgroup 0 owns kh = 0, 1 and warpgroup 1 kh = 2; KHM -> warpgroup 0 owns the single accumulator.
+  constexpr int NPART = KHM ? 1 : 2;                          // warpgroups that issue MMAs
+  constexpr int NKH = KHM ? 1 : (MM == 128 ? 3 : 2);          // accumulators per warpgroup
 
   extern __shared__ __align__(1024) uint8_t smem[];
   const int NS = a.nslot;
@@ -92,8 +88,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
   uint64_t* xempty = bars + MAXSLOT;
   uint64_t* gfull = bars + 2 * MAXSLOT;
   uint64_t* gempty = gfull + NGS;
-  uint64_t* done = gempty + NGS;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(done + 1);
+  float* s_bsum = reinterpret_cast<float*>(bars) + 128;     // [128 rows][GOUT + 1]: bias sums (after 512 bytes of barriers)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -104,22 +99,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
       *reinterpret_cast<uint4*>(s_x + (size_t)(NS + NMIRROR) * XSLAB + i) = make_uint4(0u, 0u, 0u, 0u);
   fence_proxy_async();
   if (threadIdx.x == 0) {
-    for (int i = 0; i < NS; ++i) { mbar_init(&xfull[i], NLOADER); mbar_init(&xempty[i], 1); }
-    for (int i = 0; i < NGS; ++i) { mbar_init(&gfull[i], NLOADER); mbar_init(&gempty[i], 1 + 128); }
-    mbar_init(done, 1);
+    // one arrival per warp of every MMA warpgroup, after its last MMA reading the slab has completed
+    for (int i = 0; i < NS; ++i) { mbar_init(&xfull[i], NLOADER); mbar_init(&xempty[i], 4 * NPART); }
+    for (int i = 0; i < NGS; ++i) { mbar_init(&gfull[i], NLOADER); mbar_init(&gempty[i], 4 * NPART); }
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(tmem_slot, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   const int HW_tiles = a.tiles_h * a.tiles_w;
   const bool has_work = blockIdx.x < a.nitems;
 
-  if (warp >= 5) {
+  if (warp >= 8) {
     // ================================ LOADER (128 threads) ================================
-    const int lt = threadIdx.x - 5 * 32;
+    setmaxnreg_dec<64>();
+    const int lt = threadIdx.x - 8 * 32;
     uint32_t xslot = 0, xphase = 1, gslot = 0, gphase = 1;    // producer side: first lap passes on the fresh barriers
     const int Dx = a.upd ? a.D >> 1 : a.D, Hx = a.up ? a.H >> 1 : a.H, Wx = a.up ? a.W >> 1 : a.W;
     const int ncx = a.Cx >> 3, ncg = a.Cg >> 3;
@@ -183,15 +175,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
         }
       }
     }
-  } else if (warp == 4) {
-    // ================================ MMA ISSUER (whole warp, one elected lane) ================================
-    if (has_work) {
-      constexpr uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(NN >> 3) << 17) | ((uint32_t)(MM >> 4) << 24);
+  } else {
+    // ================================ MMA WARPGROUPS ================================
+    setmaxnreg_inc<216>();
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;
+    float acc[NKH][NN / 2];
+    // warpgroup 0 also folds the bias gradient out of the staged gz slabs: thread t owns gz slab row t and its row of
+    // s_bsum (shared memory, not registers: the accumulators of the widest layer need them all)
+    float* bsum = s_bsum + t * (GOUT + 1);
+    if (wg == 0)
+#pragma unroll
+      for (int c = 0; c < GOUT; ++c) bsum[c] = 0.f;
+    const bool do_bias = wg == 0 && a.bias_partial && !(a.dbg & 4);
+    uint32_t roff[GOUT / 8];
+#pragma unroll
+    for (int c8 = 0; c8 < GOUT / 8; ++c8) roff[c8] = swz((uint32_t)(GPAD + t) * WG + (uint32_t)c8 * 16u, WG);
+    if (has_work && wg < NPART) {
       const uint32_t x_u32 = smem_u32(s_x), g_u32 = smem_u32(s_g);
       uint32_t wslot = 0, wphase = 0;   // next x slab to wait for
       uint32_t hslot = 0;               // head of the kd window
       uint32_t gs = 0, gph = 0;
       uint32_t acc0 = 0;                // 0 only for the very first (tile, slice) of this CTA
+      // MM = 128: rows 64-127 (warpgroup 1) are M atoms 2 and 3 of the kd window, two atom strides further
+      const uint32_t m_off = (MM == 128 && wg == 1) ? 2u * XSLAB : 0u;
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int ch = (item / HW_tiles) % a.nchunks;
         const int nd = min(ch * a.dchunk + a.dchunk, a.D) - ch * a.dchunk;
@@ -202,185 +209,94 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
             if (++wslot == (uint32_t)NS) { wslot = 0; wphase ^= 1; }
           }
           mbar_wait(&gfull[gs], gph);
-          tc_fence_after();
-          const uint32_t a_start = x_u32 + hslot * XSLAB;
+          const uint32_t a_start = x_u32 + hslot * XSLAB + m_off;
           const uint32_t b_start = g_u32 + gs * GSLAB + (uint32_t)(GPAD - 1) * WG;
-          const uint64_t adesc0 = make_desc_mn_swz<WA>(a_start, KHM ? (uint32_t)(TWR * WA) : (KD == 3 ? XSLAB : 0u), 0u);
-          const uint64_t bdesc0 = make_desc_mn_swz<WG>(b_start, (uint32_t)WG, 0u);   // base offset 0: the swizzle is a function of the absolute address (verified on B200: the matrix-base-offset form gives wrong sums)
-          if (KHM) {
-            if (elect_one()) {
+          const uint64_t adesc0 = make_desc_mn_swz<WA>(a_start, KHM ? (uint32_t)(TWR * WA) : (KD == 3 ? XSLAB : 0u));
+          const uint64_t bdesc0 = make_desc_mn_swz<WG>(b_start, (uint32_t)WG);
+          // one straight-line wgmma chain per warpgroup role (no warpgroup-divergent branch inside a chain): NK
+          // accumulators for the consecutive kh taps kh0 .. kh0 + NK - 1
+          auto chain = [&](auto nk, int kh0) {
+            constexpr int NK = decltype(nk)::value;
+            wg_fence();
+#pragma unroll
+            for (int s = 0; s < NK; ++s) {
 #pragma unroll
               for (int i = 0; i < GROWS / 16; ++i) {
-                if (a.dbg & 1) break;
-                const uint64_t adesc = adesc0 + (uint64_t)(((16 * i) * WA) >> 4);
+                const uint64_t adesc = adesc0 + (uint64_t)((((kh0 + s) * TWR + 16 * i) * WA) >> 4);
                 const uint64_t bdesc = bdesc0 + (uint64_t)((16 * i * WG) >> 4);
-                umma_f16(tmem_base, adesc, bdesc, idesc, i == 0 ? acc0 : 1u);
-              }
-              umma_commit(&xempty[hslot]);
-              umma_commit(&gempty[gs]);
-            }
-          } else if (elect_one()) {
-#pragma unroll
-            for (int kh = 0; kh < 3; ++kh) {
-              if (a.dbg & 1) break;
-              const uint32_t tmem_d = MM == 128 ? tmem_base + (uint32_t)(kh * NN)
-                                                : tmem_base + ((uint32_t)((kh & 1) * 16) << 16) + (uint32_t)((kh >> 1) * NN);
-#pragma unroll
-              for (int i = 0; i < GROWS / 16; ++i) {
-                const uint64_t adesc = adesc0 + (uint64_t)(((kh * TWR + 16 * i) * WA) >> 4);
-                const uint64_t bdesc = bdesc0 + (uint64_t)((16 * i * WG) >> 4);
-                umma_f16(tmem_d, adesc, bdesc, idesc, i == 0 ? acc0 : 1u);
+                Wgmma<NN, 1, 1>::mma(acc[s], adesc, bdesc, i == 0 ? acc0 : 1u);
               }
             }
-            umma_commit(&xempty[hslot]);
-            umma_commit(&gempty[gs]);
+            wg_commit();
+          };
+          if (MM == 128 || KHM || wg == 0) chain(std::integral_constant<int, NKH>{}, 0);
+          else chain(std::integral_constant<int, 1>{}, 2);    // warpgroup 1 of an M = 64 layer: kh = 2
+          if (do_bias) {
+            const uint8_t* gt = s_g + (size_t)gs * GSLAB;
+#pragma unroll
+            for (int c8 = 0; c8 < GOUT / 8; ++c8) {
+              const uint4 q = *reinterpret_cast<const uint4*>(gt + roff[c8]);
+              const __nv_bfloat162* hq = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const float2 f = __bfloat1622float2(hq[e]);
+                bsum[c8 * 8 + 2 * e] += f.x;
+                bsum[c8 * 8 + 2 * e + 1] += f.y;
+              }
+            }
           }
-          __syncwarp();
+          wg_wait<0>();
+          if (lane == 0) {
+            mbar_arrive(&xempty[hslot]);
+            mbar_arrive(&gempty[gs]);
+          }
           acc0 = 1u;
           if (++hslot == (uint32_t)NS) hslot = 0;
           if (++gs == NGS) { gs = 0; gph ^= 1; }
         }
         if (KD == 3) {
-          if (elect_one()) {
-            umma_commit(&xempty[hslot]);
-            umma_commit(&xempty[hslot + 1 == (uint32_t)NS ? 0 : hslot + 1]);
+          if (lane == 0) {
+            mbar_arrive(&xempty[hslot]);
+            mbar_arrive(&xempty[hslot + 1 == (uint32_t)NS ? 0 : hslot + 1]);
           }
-          __syncwarp();
           hslot = hslot + 2 >= (uint32_t)NS ? hslot + 2 - NS : hslot + 2;
-        }
-      }
-      if (elect_one()) umma_commit(done);
-      __syncwarp();
-    }
-  } else {
-    // ================================ BIAS + FINAL EPILOGUE (warps 0-3) ================================
-    // thread r owns gz slab row r: sums its GOUT channels over all staged slabs (halo / out-of-volume rows are zero)
-    float bsum[GOUT];
-#pragma unroll
-    for (int c = 0; c < GOUT; ++c) bsum[c] = 0.f;
-    const int rowi = warp * 32 + lane;
-    if (has_work && a.bias_partial && !(a.dbg & 4)) {
-      uint32_t gs = 0, gph = 0;
-      uint32_t roff[GOUT / 8];
-#pragma unroll
-      for (int c8 = 0; c8 < GOUT / 8; ++c8) roff[c8] = swz((uint32_t)(GPAD + rowi) * WG + (uint32_t)c8 * 16u, WG);
-      for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-        const int ch = (item / HW_tiles) % a.nchunks;
-        const int nd = min(ch * a.dchunk + a.dchunk, a.D) - ch * a.dchunk;
-        for (int j = 0; j < nd; ++j) {
-          mbar_wait(&gfull[gs], gph);
-          const uint8_t* gt = s_g + (size_t)gs * GSLAB;
-#pragma unroll
-          for (int c8 = 0; c8 < GOUT / 8; ++c8) {
-            const uint4 q = *reinterpret_cast<const uint4*>(gt + roff[c8]);
-            const __nv_bfloat162* hq = reinterpret_cast<const __nv_bfloat162*>(&q);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float2 f = __bfloat1622float2(hq[e]);
-              bsum[c8 * 8 + 2 * e] += f.x;
-              bsum[c8 * 8 + 2 * e + 1] += f.y;
-            }
-          }
-          mbar_arrive(&gempty[gs]);
-          if (++gs == NGS) { gs = 0; gph ^= 1; }
-        }
-      }
-    } else if (has_work) {
-      // no bias wanted: still release the gz slabs
-      uint32_t gs = 0, gph = 0;
-      for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
-        const int ch = (item / HW_tiles) % a.nchunks;
-        const int nd = min(ch * a.dchunk + a.dchunk, a.D) - ch * a.dchunk;
-        for (int j = 0; j < nd; ++j) {
-          mbar_wait(&gfull[gs], gph);
-          mbar_arrive(&gempty[gs]);
-          if (++gs == NGS) { gs = 0; gph ^= 1; }
         }
       }
     }
     float* part = a.partial + (size_t)blockIdx.x * T * G * GOUT;
-    if (has_work) {
-      mbar_wait(done, 0);
-      tc_fence_after();
-      if (KHM) {
-        // accumulator row m = kh * 16 + ci on TMEM lane (m % 16) + 32 * (m / 16): warp = kh, lanes 0..15 = ci; columns q * GOUT + co
-        const int kh = warp, ci = lane & 15;
-#pragma unroll 1
-        for (int q = 0; q < 3; ++q)
+    if (!has_work) {
+      if (wg == 0)
+        for (int i = t; i < T * G * GOUT; i += 128) part[i] = 0.f;
+    } else if (wg < NPART) {
+      // fragment (row m, column n) of accumulator s: m = (kd, ci) (KHM: (kh, ci)), n = q * GOUT + co with kw = 2 - q
+      const int w4 = t >> 5, qr = lane >> 2, pc = lane & 3;
 #pragma unroll
-          for (int c0 = 0; c0 < GOUT; c0 += 8) {
-            uint32_t r[8];
-            tmem_ld8(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(q * GOUT + c0), r);
-            tmem_ld_wait();
-            if (kh < 3 && lane < 16) {
-              const int tap = kh * 3 + (2 - q);
-              float4* o = reinterpret_cast<float4*>(part + ((size_t)tap * G + ci) * GOUT + c0);
-              o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-              o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-            }
+      for (int s = 0; s < NKH; ++s) {
+        const int kh = KHM ? 0 : (MM == 128 ? s : (wg == 0 ? s : 2));
+        if (MM != 128 && !KHM && wg == 1 && s > 0) break;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int m = (MM == 128 ? 64 * wg : 0) + 16 * w4 + 8 * i + qr;
+          const int kd = KHM ? 0 : m / G, ci = m % G, khm = KHM ? m / G : kh;
+          if (kd >= KD || khm >= 3) continue;
+#pragma unroll
+          for (int jn = 0; jn < NN / 8; ++jn) {
+            const int n = 8 * jn + 2 * pc, q = n / GOUT, co = n % GOUT;
+            const int tap = (kd * 3 + khm) * 3 + (2 - q);
+            *reinterpret_cast<float2*>(part + ((size_t)tap * G + ci) * GOUT + co) = make_float2(acc[s][4 * jn + 2 * i], acc[s][4 * jn + 2 * i + 1]);
           }
-      } else if (MM == 128) {
-        // accumulator row m = kd * G + ci on TMEM lane m; columns kh * NN + q * GOUT + co, q = 2 - kw
-        const int m = warp * 32 + lane, kd = m / G, ci = m % G;
-#pragma unroll 1
-        for (int kh = 0; kh < 3; ++kh)
-#pragma unroll 1
-          for (int q = 0; q < 3; ++q)
-#pragma unroll
-            for (int c0 = 0; c0 < GOUT; c0 += 8) {
-              uint32_t r[8];
-              tmem_ld8(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(kh * NN + q * GOUT + c0), r);
-              tmem_ld_wait();
-              if (kd < KD) {
-                const int tap = (kd * 3 + kh) * 3 + (2 - q);
-                float4* o = reinterpret_cast<float4*>(part + ((size_t)tap * G + ci) * GOUT + c0);
-                o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-                o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-              }
-            }
-      } else {
-        // M = 64: row m on lane (m % 16) + 32 * (m / 16); kh = 0 / 1 share columns [0, NN) at lane offsets 0 / 16, kh = 2 in [NN, 2NN)
-        const int m = warp * 16 + (lane & 15), kd = m / G, ci = m % G, half = lane >> 4;
-#pragma unroll 1
-        for (int blk = 0; blk < 2; ++blk)
-#pragma unroll 1
-          for (int q = 0; q < 3; ++q)
-#pragma unroll
-            for (int c0 = 0; c0 < GOUT; c0 += 8) {
-              uint32_t r[8];
-              tmem_ld8(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(blk * NN + q * GOUT + c0), r);
-              tmem_ld_wait();
-              const int kh = blk == 0 ? half : 2;
-              if (kd < KD && !(blk == 1 && half == 1)) {
-                const int tap = (kd * 3 + kh) * 3 + (2 - q);
-                float4* o = reinterpret_cast<float4*>(part + ((size_t)tap * G + ci) * GOUT + c0);
-                o[0] = make_float4(__uint_as_float(r[0]), __uint_as_float(r[1]), __uint_as_float(r[2]), __uint_as_float(r[3]));
-                o[1] = make_float4(__uint_as_float(r[4]), __uint_as_float(r[5]), __uint_as_float(r[6]), __uint_as_float(r[7]));
-              }
-            }
-      }
-    } else {
-      for (int i = threadIdx.x; i < T * G * GOUT; i += 128) part[i] = 0.f;
-    }
-    if (a.bias_partial) {
-      // bias partial of this CTA: fixed-order reduction over the 128 rows through shared memory (the x ring is idle now)
-      float* s_b = reinterpret_cast<float*>(s_x);
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-#pragma unroll
-      for (int c = 0; c < GOUT; ++c) s_b[rowi * (GOUT + 1) + c] = bsum[c];
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (rowi < GOUT) {
-        float t = 0.f;
-        for (int r2 = 0; r2 < 128; ++r2) t += s_b[r2 * (GOUT + 1) + rowi];
-        a.bias_partial[(size_t)blockIdx.x * GOUT + rowi] = t;
+        }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    __syncwarp();
-    tmem_dealloc(tmem_base, tmem_cols);
+    if (wg == 0 && a.bias_partial) {
+      // bias partial of this CTA: fixed-order reduction over the 128 rows
+      named_bar(1, 128);
+      if (t < GOUT) {
+        float sum = 0.f;
+        for (int r2 = 0; r2 < 128; ++r2) sum += s_bsum[r2 * (GOUT + 1) + t];
+        a.bias_partial[(size_t)blockIdx.x * GOUT + t] = sum;
+      }
+    }
   }
 }
 
@@ -520,7 +436,7 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
   if (nslot > MAXSLOT) nslot = MAXSLOT;
   VXM_REQUIRE(nslot >= 4, "conv3d_tc_wgrad: not enough shared memory for the slab ring");
   a.nslot = nslot;
-  const size_t smem = (size_t)(nslot + extra) * xslab + NGS * gslab + 512;
+  const size_t smem = (size_t)(nslot + extra) * xslab + NGS * gslab + 512 + 128 * (GOUT + 1) * sizeof(float);   // + bias rows
 #define VXM_W2_LAUNCH(KD_, G_, GO_)                                                                                          \
   do {                                                                                                                       \
     VXM_CUDA(cudaFuncSetAttribute(wgrad2_kernel<KD_, G_, GO_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));     \

@@ -204,15 +204,16 @@ __global__ void __launch_bounds__(256) planar_fold_kd_kernel(PlanarSrc src, __nv
     if (d + 1 < D) r[2 * NP + p] = __ldg(q + HW);
   }
   __nv_bfloat16* o = out + (((size_t)b * D + d) * HW + hw) * COUT;
-  if constexpr (COUT == 16) {     // one 256-bit store per voxel: whole sectors
+  if constexpr (COUT == 16) {     // two adjacent 128-bit stores per voxel: one whole 32-byte sector
     uint32_t w[8];
 #pragma unroll
     for (int e = 0; e < 8; ++e) {
       __nv_bfloat162 h = __floats2bfloat162_rn(r[2 * e], r[2 * e + 1]);
       w[e] = *reinterpret_cast<uint32_t*>(&h);
     }
-    asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(o), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]),
-                 "r"(w[6]), "r"(w[7]) : "memory");
+    uint4* o4 = reinterpret_cast<uint4*>(o);
+    o4[0] = make_uint4(w[0], w[1], w[2], w[3]);
+    o4[1] = make_uint4(w[4], w[5], w[6], w[7]);
   } else {
     V8 t;
 #pragma unroll

@@ -1,10 +1,11 @@
-// Thin PTX wrappers for the sm_100a tensor-core path: mbarrier, cp.async, bulk (TMA) copies,
-// tcgen05 alloc / mma / commit / ld, and UMMA descriptor encoders.
+// Thin PTX wrappers for the sm_90a tensor-core path: mbarrier, cp.async, bulk (TMA) copies, wgmma and its
+// shared-memory descriptor encoders.
 #pragma once
 #include <cuda.h>        // CUtensorMap (types only: the encoder is resolved at run time, libcuda is not linked)
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace vxm {
 namespace tc {
@@ -34,14 +35,12 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.
+// Bounded wait: a protocol bug traps (the launch fails with an error) instead of hanging the GPU.  No printf here: a
+// function call in a kernel that issues wgmma makes ptxas serialise the wgmma pipeline.
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
-    if (++spins > (1u << 26)) {
-      printf("vxm: mbarrier wait timed out (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-      __trap();
-    }
+    if (++spins > (1u << 26)) __trap();
   }
 }
 
@@ -54,8 +53,6 @@ __device__ __forceinline__ bool elect_one() {
 
 // ---------------------------------------------------------------- proxies / fences ---------
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 // ---------------------------------------------------------------- cp.async (LDGSTS) --------
 // 16-byte copy, zero-filled when src_bytes == 0 (padding / out-of-volume voxels)
@@ -80,7 +77,7 @@ __device__ __forceinline__ void bulk_g2s(void* dst_smem, const void* src, uint32
 // ---------------------------------------------------------------- tiled tensor copy (TMA, 5-D) ------
 // A bf16 channels-last activation (B, D, H, W, C) is described to the TMA unit as the 5-D tensor {C, W, H, D, B}; one
 // copy moves a box {G channels, 32 columns, rows, 1 slice, 1 batch item} into shared memory with the 32 / 64 / 128-byte
-// swizzle the UMMA K-major operand layouts use (row = voxel, channels contiguous).  Coordinates may lie outside the
+// swizzle the wgmma K-major operand layouts use (row = voxel, channels contiguous).  Coordinates may lie outside the
 // tensor (negative, or >= the extent): those elements arrive as zeros, which is exactly the convolution's zero padding.
 __device__ __forceinline__ void tma_prefetch_desc(const void* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(tmap)) : "memory");
@@ -100,83 +97,85 @@ __device__ __forceinline__ void mbar_expect_tx_noarrive(uint64_t* bar, uint32_t 
 // is the shared-memory row width (32 / 64 / 128) and selects the swizzle mode.  Returns 0, or -1 with vxm_last_error set.
 int make_act_tmap(CUtensorMap* out, const void* base, int B, int D, int H, int W, int C, int boxC, int boxW, int boxH);
 
-// ---------------------------------------------------------------- TMEM ----------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
+// ---------------------------------------------------------------- wgmma (warpgroup MMA) ------
+// The four warps of a warpgroup issue wgmma.mma_async together; the accumulators live in their registers (m64nNk16
+// fragment layout, see Wgmma in wgmma.cuh).  A 128-row tile is two m64 halves, rows 0-63 in d0 and 64-127 in d1.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// register budget moved between warpgroups (every warp of the warpgroup executes it): producers give registers up,
+// MMA warpgroups take them.  ptxas still compiles every role within the __launch_bounds__ budget (168 registers at 384
+// threads), so this only pays where the producer needs few registers: it is used by the kernels whose spill counts
+// (-Xptxas -v) it lowers (conv_tct_kernel, wgrad2_kernel) and left out where it raises them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+__device__ __forceinline__ void named_bar(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single thread
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+// Accumulator read-out in row form: thread t of the warpgroup (t = threadIdx.x % 128) receives row t, columns
+// [c0, c0 + 16) of the 128 x N accumulator held as two m64 fragments d0 / d1 (c0: a multiple of 16 known at compile time
+// after unrolling, so the fragments stay in registers).  The fragments pass through `stage` (ACC_STAGE_FLOATS floats of
+// shared memory per warpgroup); `bar` is a named barrier owned by the warpgroup.
+constexpr int ACC_STAGE_LD = 17;                     // padded row: conflict-free row reads
+constexpr int ACC_STAGE_FLOATS = 128 * ACC_STAGE_LD;
+__device__ __forceinline__ void acc_row16(const float* d0, const float* d1, int c0, float* stage, int bar, uint32_t* r) {
+  const int t = threadIdx.x & 127, w = t >> 5, q = (t & 31) >> 2, p = t & 3;
+  named_bar(bar, 128);                                // the previous read-out of `stage` is complete
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float* d = h ? d1 : d0;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float* srow = stage + (64 * h + 16 * w + 8 * i + q) * ACC_STAGE_LD + 2 * p;
+#pragma unroll
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = c0 / 8 + jj;
+        srow[8 * jj] = d[4 * j + 2 * i];
+        srow[8 * jj + 1] = d[4 * j + 2 * i + 1];
+      }
+    }
+  }
+  named_bar(bar, 128);
+  const float* mine = stage + t * ACC_STAGE_LD;
+#pragma unroll
+  for (int k = 0; k < 16; ++k) r[k] = __float_as_uint(mine[k]);
 }
-// mbarrier arrives once all tcgen05 ops issued so far by this thread have completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-
-// 32 lanes x 32 bit, N consecutive columns: thread i of the warp receives TMEM lane (base_lane + i)
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // ---------------------------------------------------------------- descriptors ---------------
-// Shared-memory matrix descriptor, K-major, SWIZZLE_NONE ("interleave"): core matrix = 8 rows x 16 B,
-// rows 16 B apart; LBO = byte distance between the two 16-byte K chunks of one MMA (K = 16 bf16),
-// SBO = byte distance between consecutive 8-row groups.  (cute/arch/mma_sm100_desc.hpp SmemDescriptor)
+// wgmma shared-memory matrix descriptor (sm_90): start address, LBO, SBO in 16-byte units; bits 62-63 = swizzle
+// (0 none, 1 = 128 B, 2 = 64 B, 3 = 32 B).
+// K-major, SWIZZLE_NONE: core matrix = 8 rows x 16 B, rows 16 B apart; LBO = byte distance between the two 16-byte
+// K chunks of one MMA (K = 16 bf16), SBO = byte distance between consecutive 8-row groups.
 __device__ __forceinline__ uint64_t make_desc_kmajor_noswz(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;  // descriptor version 1 (Blackwell)
-  return d;                // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
+  return d;                // base_offset 0, layout_type 0 (SWIZZLE_NONE)
 }
 // MN-major, SWIZZLE_NONE: core matrix = 8 (K) x 8 (MN, 16 B contiguous); the 8 K-rows are 16 B apart.
-// LBO/SBO roles per cute make_umma_desc<Major::MN> for SWIZZLE_NONE: SBO = stride between 8-element MN
-// chunks, LBO = stride between 8-row K groups.
+// SBO = stride between 8-element MN chunks, LBO = stride between 8-row K groups.
 __device__ __forceinline__ uint64_t make_desc_mnmajor_noswz(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   return make_desc_kmajor_noswz(saddr, lbo_bytes, sbo_bytes);
 }
-
-// Instruction descriptor for kind::f16, BF16 x BF16 -> F32  (cute/arch/mma_sm100_desc.hpp InstrDescriptor)
-__host__ __device__ inline uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  uint32_t d = 0;
-  d |= 1u << 4;                        // c_format  = F32
-  d |= 1u << 7;                        // a_format  = BF16
-  d |= 1u << 10;                       // b_format  = BF16
-  d |= (uint32_t)(a_mn_major & 1) << 15;
-  d |= (uint32_t)(b_mn_major & 1) << 16;
-  d |= (uint32_t)(N >> 3) << 17;       // n_dim
-  d |= (uint32_t)(M >> 4) << 24;       // m_dim
-  return d;
+// swizzle field of a `width`-byte swizzled row (32, 64 or 128)
+__host__ __device__ constexpr uint64_t desc_swizzle(uint32_t width) {
+  return (uint64_t)(width == 128 ? 1 : (width == 64 ? 2 : 3)) << 62;
 }
 
-// 256-bit global accesses (sm_100: LDG.256 / STG.256): one instruction moves a lane's 16 bf16 channels, and a warp's store
-// covers whole 32-byte sectors instead of two half-sector passes.  `p` must be 32-byte aligned.
+// A lane's 16 bf16 channels (32 bytes, one sector) as two adjacent 128-bit accesses (the widest global access on sm_90).
+// `p` must be 32-byte aligned.
 __device__ __forceinline__ void st_global_v8(void* p, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4, uint32_t r5, uint32_t r6,
                                              uint32_t r7) {
-  asm volatile("st.global.v8.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8};" ::"l"(p), "r"(r0), "r"(r1), "r"(r2), "r"(r3), "r"(r4), "r"(r5), "r"(r6), "r"(r7)
-               : "memory");
+  uint4* q = reinterpret_cast<uint4*>(p);
+  q[0] = make_uint4(r0, r1, r2, r3);
+  q[1] = make_uint4(r4, r5, r6, r7);
 }
 __device__ __forceinline__ void ld_global_nc_v8(const void* p, uint32_t (&r)[8]) {
-  asm volatile("ld.global.nc.v8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "l"(p));
+  const uint4 a = __ldg(reinterpret_cast<const uint4*>(p)), b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
+  r[0] = a.x; r[1] = a.y; r[2] = a.z; r[3] = a.w; r[4] = b.x; r[5] = b.y; r[6] = b.z; r[7] = b.w;
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {

@@ -290,7 +290,7 @@ __device__ __forceinline__ float4 blend8(const Foot& f, const float4 (&u)[8]) {
 // Work decomposition of both fast kernels: the field is cut into 512-voxel blocks; CTA c owns the contiguous run of blocks
 // [c * nblk / grid, (c + 1) * nblk / grid) (so consecutive iterations of a CTA touch neighbouring rows: L1 reuse), and a thread
 // carries TWO voxels (blocks blk, blk + 1) per iteration with all 16 gathers in flight — at 16 warps per SM the kernel is bound by
-// the L2 round trip of its gathers otherwise (ncu: long scoreboard 45 %, issue slots 19 % busy, profiles/r2_memory_kernels.md).
+// the L2 round trip of its gathers otherwise.
 // SAVE: every intermediate field v_0 .. v_{n-1} is kept (states, for the backward); otherwise two buffers ping-pong
 template <bool SAVE>
 __global__ void __launch_bounds__(512) vecint_fwd_fast_kernel(const float* __restrict__ vel, float* __restrict__ out, float4* buf,

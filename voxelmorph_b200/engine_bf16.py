@@ -1,7 +1,7 @@
 """The tensor-core (bf16 operands / fp32 accumulation) execution engine of Unet + flow head.
 
 `unet_flow(model, source, target)` computes `model.flow(model.unet_model(cat(source, target)))`
-(reference voxelmorph/torch/networks.py:253-257) entirely with the tcgen05 convolution kernels and the
+(reference voxelmorph/torch/networks.py:253-257) entirely with the wgmma convolution kernels and the
 channels-last bf16 glue kernels: every activation between the fp32 input images and the fp32 flow field is a
 bf16 (B,D,H,W,C) tensor, the concat / upsample / bias / LeakyReLU / LeakyReLU-derivative are fused into the
 convolution kernels, and the backward pass (dgrad, wgrad, pooling and skip routing) is written out by hand —

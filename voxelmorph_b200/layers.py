@@ -1,5 +1,5 @@
 """SpatialTransformer / VecInt / ResizeTransform with the reference's surface
-(reference voxelmorph/torch/layers.py) over the sm_100a kernels of libvxm_b200.so.
+(reference voxelmorph/torch/layers.py) over the sm_90a kernels of libvxm_b200.so.
 
 Same class names, constructor arguments, forward signatures and error behaviour as the
 reference; the arithmetic runs in hand-written CUDA kernels reached through the C ABI

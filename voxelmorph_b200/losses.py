@@ -1,7 +1,7 @@
 """NCC / MSE / Dice / Grad losses with the reference's surface
 (reference voxelmorph/torch/losses.py): plain classes whose bound `.loss(y_true, y_pred)`
 returns a 0-d tensor supporting `.item()`, `*`, `+`, `.backward()`.
-Each loss is one fused sm_100a kernel (plus a fused backward) from libvxm_b200.so.
+Each loss is one fused sm_90a kernel (plus a fused backward) from libvxm_b200.so.
 """
 import numpy as np
 import torch
@@ -62,7 +62,7 @@ class NCC:
         ndims = len(list(y_true.size())) - 2
         assert ndims in [1, 2, 3], "volumes should be 1 to 3 dimensions. found: %d" % ndims
         if ndims == 1:
-            raise _lib.VxmError("NCC: 1-D volumes are not supported by the B200 path")
+            raise _lib.VxmError("NCC: 1-D volumes are not supported by the GPU path")
         win = [9] * ndims if self.win is None else list(self.win)
         return _NccFn.apply(y_true, y_pred, tuple(int(w) for w in win))
 

@@ -2,7 +2,7 @@
 (reference voxelmorph/torch/networks.py): same class names, constructor arguments, attributes
 (`unet_model`, `flow`, `resize`, `fullsize`, `integrate`, `transformer`, `bidir`, `config`,
 `Unet.final_nf`), forward signatures / return tuples and `state_dict` keys — so reference
-checkpoints load unchanged — with every operator running in sm_100a kernels.
+checkpoints load unchanged — with every operator running in sm_90a kernels.
 """
 import numpy as np
 import torch

@@ -24,7 +24,7 @@ def set_default_engine(name):
 
 def conv_engine():
     """'f32'    — CUDA-core fp32 engine (FFMA; every U-Net shape);
-    'bf16'   — tcgen05/TMEM implicit-GEMM engine, bf16 operands / fp32 accumulation (the throughput mode bench.py times);
+    'bf16'   — wgmma implicit-GEMM engine, bf16 operands / fp32 accumulation (the throughput mode bench.py times);
     'bf16x3' — the same tensor-core kernels with every operand split into a bf16 hi + lo pair and three MMAs per tile
                (hi*hi + lo*hi + hi*lo): fp32-grade products, flow / moved image within 1e-4 of the reference;
     'tc'     — 'bf16x3' where the tensor-core engine supports the model, else 'f32'."""

@@ -1,4 +1,4 @@
-"""Host wrappers of the tcgen05 implicit-GEMM convolution engine (csrc/conv3d_tc.cu, csrc/conv3d_tc_wgrad.cu).
+"""Host wrappers of the wgmma implicit-GEMM convolution engine (csrc/conv3d_tc.cu, csrc/conv3d_tc_wgrad.cu).
 
 Activations of this engine are bf16, channels-last: a (B, C, D, H, W) logical tensor is held as a contiguous
 (B, D, H, W, C) bf16 tensor (`ndhwc`).  Weights stay fp32 in the nn.Module (reference layout
@@ -22,7 +22,7 @@ def np_for(cout):
         return 48
     if cout <= 64:
         return 64
-    raise _lib.VxmError("tcgen05 conv engine: at most 64 output channels per launch (got %d)" % cout)
+    raise _lib.VxmError("tensor-core conv engine: at most 64 output channels per launch (got %d)" % cout)
 
 
 def to_ndhwc_bf16(x):
@@ -101,7 +101,7 @@ _ws_lock = threading.Lock()      # workspace tables are shared by the per-GPU th
 
 def conv_wgrad(xa, xb, gz, cin, cout, kd, up=False, planar_x=None, planar_g=None, need_bias=True, out_w=None, out_b=None, batch=None):
     """fp32 grad_w (cout, cin, kd, 3, 3) and grad_b (cout) from the layer input (xa/xb or planar_x) and gz.
-    `batch` (a WgradBatch): only the tcgen05 partial-sum kernels are launched now, the reduction into gw / gb happens at
+    `batch` (a WgradBatch): only the wgmma partial-sum kernels are launched now, the reduction into gw / gb happens at
     `batch.flush()` together with every other layer's."""
     lib = _lib.load()
     if batch is not None and wgrad_deferrable(xa, xb, gz, planar_x, planar_g):
@@ -218,19 +218,6 @@ def _use_s(ca, cb, cout):
     return _variant() in ("auto", "s") and bool(_lib.load().vxm_conv3d_tcs_supported(ca, cb, cout))
 
 
-def _use_s2(xa, xb, coutp, full, up, kd):
-    """The two-issuer variant (conv3d_tc_s2.cu) wherever the one-issuer kernel would pick 8-row tiles; VXM_B200_TCS2=0
-    switches back to the single issuer (A/B)."""
-    import os
-    if os.environ.get("VXM_B200_TCS2", "1") != "1":      # default on: +5 % step throughput on B200 (profiles/r2_tcs2_ab.md)
-        return False
-    cin = (0 if xa is None else xa.shape[-1]) + (0 if xb is None else xb.shape[-1])
-    H = full.shape[2] * (2 if (xb is None and up) else 1)
-    if coutp == 48:          # the single-pass dgrad of the 48-channel concat layer (32 -> 32 + 16 channels)
-        return cin == 32 and H > 4 and os.environ.get("VXM_B200_TCS2_48", "1") == "1"
-    return coutp in (16, 32) and cin in (8, 16, 32, 48) and H > 4 and not (cin == 48 and coutp == 32)
-
-
 def pack_weights_t(w, transposed=False, variant=None):
     """Packed weights for a kw-stacked kernel.  Returns (tensor, (coutp, variant))."""
     lib = _lib.load()
@@ -256,8 +243,6 @@ def conv_fwd_t(xa, xb, wpk, coutp, bias, cout, kd, up=False, out_fp32_planar=Fal
     coutp, variant = coutp if isinstance(coutp, tuple) else (coutp, "t")
     fwd = lib.vxm_conv3d_tcs_fwd if variant == "s" else lib.vxm_conv3d_tct_fwd
     full = xb if xb is not None else xa
-    if variant == "s" and _use_s2(xa, xb, coutp, full, up, kd):
-        fwd = lib.vxm_conv3d_tcs2_fwd
     B, D, H, W = full.shape[0], full.shape[1], full.shape[2], full.shape[3]
     if xb is None and up:
         D, H, W = (D * 2 if kd == 3 else D), H * 2, W * 2
@@ -304,7 +289,7 @@ def planar_to_ndhwc8_split(planes):
 
 
 def conv_fwd_split(xa, xb, packs, bias, cout, kd, up=False, out_fp32_planar=False, slope=None):
-    """One convolution layer in split precision: three passes of the kw-stacked tcgen05 kernel accumulating
+    """One convolution layer in split precision: three passes of the kw-stacked wgmma kernel accumulating
     x_lo*w_hi + x_hi*w_lo + x_hi*w_hi in an fp32 channels-last buffer.  xa / xb: (hi, lo) pairs (or None);
     packs: ((wpk_hi, meta), (wpk_lo, meta)) from pack_weights_t.  Returns a (hi, lo) pair of bf16 NDHWC tensors, or the
     fp32 planar tensor when out_fp32_planar."""
@@ -359,7 +344,7 @@ def pool_split(x, nd):
 # ---- deferred weight-gradient reduction: every layer's partials reduced by ONE launch at the end of the backward pass ----
 
 class WgradBatch:
-    """Collects the pending reductions of the tcgen05 weight-gradient kernels of one backward pass
+    """Collects the pending reductions of the wgmma weight-gradient kernels of one backward pass
     (vxm_conv3d_tc_wgrad2_partial) and reduces them all in one launch (`flush`).  One instance per (device, stream);
     the workspace is persistent (512 MB: the default 3-D U-Net at 160x192x224 needs ~200 MB of per-CTA partials)."""
 
