@@ -196,6 +196,10 @@ int vxm_conv3d_tcs_pack_desc(void* desc_host, const float* w, void* wpk, int Cou
                              int begin);
 /* descriptor of a kd-folded 2-D operand of the 3-D weight w (Cout, Cin, 3, 3, 3): operand input channel kd * r + c is tap kd of
  * real channel c, r = Cin (Cout when transposed), 3 r <= 16; packed size = vxm_conv3d_tcs_packed_bytes(3 r, coutp, 1) */
+/* descriptor of one channel block of an operand: operand output channels [n0, n0 + nb), input channels [k0, k0 + kb) (the
+ * operand's orientation: transposed swaps Cout and Cin); packed size = vxm_conv3d_tcs_packed_bytes(kb, coutp, kd) */
+int vxm_conv3d_tcs_pack_desc_blk(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int kd, int coutp, int transposed,
+                                 int n0, int nb, int k0, int kb, int begin);
 int vxm_conv3d_tcs_pack_desc_fold(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int coutp, int transposed, int begin);
 int vxm_conv3d_tcs_pack_multi(const void* descs_dev, int ndesc, int total, void* stream);
 int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
@@ -217,6 +221,15 @@ int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const f
 int vxm_conv3d_tcs_fwd_acc(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
                            const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp,
                            int kd, int out_mode, float slope, void* stream);
+/* 1 when one launch of the kernel has the shared memory for a (cin -> coutp, kd) operand; wider layers run in channel blocks. */
+int vxm_conv3d_tcs_fits(int cin, int coutp, int kd);
+/* One channel block of a layer too wide for one launch.  out_mode 0: bf16 act(acc_in + conv + bias) (acc_in may be NULL;
+ * mask: LeakyReLU derivative from the saved activation, as vxm_conv3d_tcs_fwd); 2 and 3: as vxm_conv3d_tcs_fwd_acc.
+ * opitch: channels per voxel of out / out_lo / mask when the block is part of a wider tensor (the pointers are offset to
+ * the block's first channel; 0 = dense).  acc_in and the out_mode 2 output are dense with `coutp` channels. */
+int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
+                           const void* mask, const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout,
+                           int coutp, int kd, int out_mode, float slope, int opitch, void* stream);
 /* Weight (and bias) gradient on tensor cores.  x sources as in vxm_conv3d_tc_fwd (the layer's forward input);
  * gz = gradient w.r.t. the convolution output (already multiplied by the activation derivative): bf16 NDHWC with
  * Cg in {8,16,32} channels, or nplanar_g (<= 4) planar fp32 volumes (flow head).  grad_w: fp32
@@ -231,7 +244,8 @@ int vxm_conv3d_tc_wgrad(const void* xa, const void* xb, const float* const* xf, 
  * one layer into caller-provided workspace (`work_used` bytes of it are then owned by this layer until the flush) and
  * appends the pending reductions to a HOST array of descriptors (vxm_conv3d_tc_wgrad2_desc_bytes() each, at most
  * vxm_conv3d_tc_wgrad2_max_pending()); `_flush` reduces every pending layer in ONE launch, in a fixed order
- * (deterministic).  Arguments as vxm_conv3d_tc_wgrad. */
+ * (deterministic).  Arguments as vxm_conv3d_tc_wgrad, except that Ca, Cb and Cg may also be 64: such a layer runs as
+ * 32-channel slices of both operands, one pending reduction per slice pair. */
 size_t vxm_conv3d_tc_wgrad2_desc_bytes(void);
 int vxm_conv3d_tc_wgrad2_max_pending(void);
 size_t vxm_conv3d_tc_wgrad2_partial_bytes(int kd);

@@ -59,11 +59,14 @@ SIGNATURES = {
     "vxm_conv3d_tcs_supported": (c_i, [c_i] * 3),
     "vxm_conv3d_tcs_pack_desc_bytes": (c_sz, []),
     "vxm_conv3d_tcs_pack_desc": (c_i, [c_f, c_f, c_f] + [c_i] * 6),
+    "vxm_conv3d_tcs_pack_desc_blk": (c_i, [c_f, c_f, c_f] + [c_i] * 10),
     "vxm_conv3d_tcs_pack_desc_fold": (c_i, [c_f, c_f, c_f] + [c_i] * 5),
     "vxm_conv3d_tcs_pack_multi": (c_i, [c_f, c_i, c_i, c_f]),
     "vxm_conv3d_tcs_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f, c_i, c_f]),
     "vxm_conv3d_tcs2_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f, c_i, c_f]),
     "vxm_conv3d_tcs_fwd_acc": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f]),
+    "vxm_conv3d_tcs_fits": (c_i, [c_i] * 3),
+    "vxm_conv3d_tcs_fwd_blk": (c_i, [c_f] * 8 + [c_i] * 11 + [c_fl, c_i, c_f]),
     "vxm_conv3d_tc_wgrad_workspace_bytes": (c_sz, [c_i]),
     "vxm_conv3d_tc_wgrad": (c_i, [c_f, c_f, c_f, c_f, c_i, c_f, c_f, c_f, c_i, c_f, c_f, c_f] + [c_i] * 12 + [c_f]),
     "vxm_conv3d_tc_wgrad2_desc_bytes": (c_sz, []),

@@ -40,6 +40,9 @@ struct ConvSArgs {
   // zero padding is the copy's out-of-bounds fill.  Groups read through the nearest-neighbour upsampler (decoder concat
   // layers), the 64-channel group that interleaves two sources and the 8-plane image input stay on the cp.async loader.
   int tma_mask, tc0[2];
+  // channel pitch of out / out_lo / mask in the OP kernels: one block of output channels of a wider tensor (the caller
+  // offsets the pointers to the block's first channel); acc_in and the out_mode 2 sums stay dense (COUT per voxel)
+  int opitch;
   alignas(64) CUtensorMap tm[2];
 };
 
@@ -62,7 +65,9 @@ __device__ __forceinline__ uint64_t make_desc_kmajor_swz(uint32_t saddr, uint32_
 // EPI: epilogue specialisation.  0 = generic run-time epilogue; 1 = forward (bias + LeakyReLU with
 // 0 <= slope <= 1, bf16 channels-last, all COUT channels real); 2 = dgrad (LeakyReLU derivative from the saved activation);
 // 3 = raw sums with an optional channel split at a multiple of 16 (single-pass dgrad of a concat layer).
-template <int KD, int G0, int G1, int COUT, int HT, bool ACC, int EPI>
+// OP: the bf16 outputs and the mask are one channel block of a wider tensor (pitch a.opitch, no out2); the channel-blocked
+// execution of the layers whose weights do not fit shared memory in one piece (64 -> 64, 128 -> 64, ...).
+template <int KD, int G0, int G1, int COUT, int HT, bool ACC, int EPI, bool OP = false>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_constant__ ConvSArgs a) {
   constexpr int SROWS = (HT + 2) * WT;
   constexpr int NH = HT / 4;
@@ -290,7 +295,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
             if constexpr (EPI == 2) {
               if (valid) {
 #pragma unroll
-                for (int q = 0; q < COUT / 16; ++q) ld_global_nc_v8(a.mask + vox * COUT + q * 16, mreg[q]);
+                for (int q = 0; q < COUT / 16; ++q) ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + q * 16, mreg[q]);
               }
             }
 #pragma unroll
@@ -318,7 +323,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                 }
                 if (valid) {
                   __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
-                                                              : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + c0;
+                                                              : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + c0;
                   st_global_v8(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
                                pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
                 }
@@ -352,7 +357,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         if (a.mask && valid) {
 #pragma unroll
           for (int q = 0; q < COUT / 8; ++q)
-            if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * a.Cout) + q);
+            if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * (OP ? a.opitch : a.Cout)) + q);
         }
         const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
 #pragma unroll
@@ -364,7 +369,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         for (int cc = 0; cc < CW; cc += 16) {
           const int c0 = pass * CW + cc;
           [[maybe_unused]] float4 ain[ACC ? 4 : 1];
-          if constexpr (ACC) {
+          if constexpr (ACC && !OP) {     // (OP: read after the combine, the prefetch would spill)
             if (a.acc_in && valid) {      // partial sums of the earlier split-precision passes
               const float4* ap = reinterpret_cast<const float4*>(a.acc_in + vox * COUT + c0);
 #pragma unroll
@@ -376,6 +381,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
           bool handled = false;
           if constexpr (ACC) {
             if (a.acc_in && valid) {
+              if constexpr (OP) {
+                const float4* ap = reinterpret_cast<const float4*>(a.acc_in + vox * COUT + c0);
+#pragma unroll
+                for (int q = 0; q < 4; ++q) ain[q] = __ldg(ap + q);
+              }
 #pragma unroll
               for (int q = 0; q < 4; ++q) { v[4 * q] += ain[q].x; v[4 * q + 1] += ain[q].y; v[4 * q + 2] += ain[q].z; v[4 * q + 3] += ain[q].w; }
             }
@@ -401,7 +411,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                       hi[e >> 1] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
                       lo[e >> 1] = pack_bf16x2(x0 - __bfloat162float(h0), x1 - __bfloat162float(h1));
                     }
-                    const size_t o = vox * a.Cout + c0 + q;
+                    const size_t o = vox * (OP ? a.opitch : a.Cout) + c0 + q;
                     *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out) + o) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
                     *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(a.out_lo) + o) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
                   }
@@ -428,7 +438,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                   }
                   // a split never falls inside a group of 8 channels (csplit % 8 == 0)
                   const int cg = c0 + q;
-                  __nv_bfloat16* oo = cg < c1 ? reinterpret_cast<__nv_bfloat16*>(a.out) + vox * c1 + cg
+                  __nv_bfloat16* oo = cg < c1 ? reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + cg
                                               : reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (a.Cout - c1) + (cg - c1);
                   *reinterpret_cast<uint4*>(oo) = make_uint4(pack_bf16x2(x[0], x[1]), pack_bf16x2(x[2], x[3]), pack_bf16x2(x[4], x[5]), pack_bf16x2(x[6], x[7]));
                 }
@@ -492,6 +502,9 @@ struct PackDesc {
   // (KD = 1 here): operand input channel kd * fold + c <-> (tap kd, real channel c), fold = real channel count of the
   // operand's input side (Cin forward, Cout transposed)
   int fold;
+  // channel block of an unfolded operand: operand output channels [n0, n0 + nb), input channels [k0, k0 + kb) (in the
+  // operand's own orientation: transposed swaps the weight's Cout and Cin)
+  int n0, nb, k0, kb;
 };
 __global__ void pack_weights_multi_kernel(const PackDesc* __restrict__ descs, int ndesc, int total) {
   for (int gi = blockIdx.x * blockDim.x + threadIdx.x; gi < total; gi += gridDim.x * blockDim.x) {
@@ -514,10 +527,9 @@ __global__ void pack_weights_multi_kernel(const PackDesc* __restrict__ descs, in
         if (!d.transposed) { if (co < d.Cout) v = d.w[((size_t)co * d.Cin + c) * 27 + tap3]; }
         else if (co < d.Cin) v = d.w[((size_t)c * d.Cin + co) * 27 + (26 - tap3)];
       }
-    } else if (!d.transposed) {
-      if (co < d.Cout && ci < d.Cin) v = d.w[((size_t)co * d.Cin + ci) * T + tap];
-    } else {
-      if (co < d.Cin && ci < d.Cout) v = d.w[((size_t)ci * d.Cin + co) * T + (T - 1 - tap)];
+    } else if (co < d.nb && ci < d.kb) {
+      if (!d.transposed) v = d.w[((size_t)(d.n0 + co) * d.Cin + d.k0 + ci) * T + tap];
+      else v = d.w[((size_t)(d.k0 + ci) * d.Cin + d.n0 + co) * T + (T - 1 - tap)];
     }
     const uint32_t W0 = d.G0 * 2, W1 = d.G1 * 2;
     uint32_t off;
@@ -585,19 +597,28 @@ extern "C" int vxm_conv3d_tcs_pack(const float* w, void* wpk, int Cout, int Cin,
 extern "C" size_t vxm_conv3d_tcs_pack_desc_bytes(void) { return sizeof(PackDesc); }
 
 // Fill one host-side descriptor (the caller uploads the array once and keeps it while the pointers stay valid).
-extern "C" int vxm_conv3d_tcs_pack_desc(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int kd, int coutp, int transposed,
-                                        int begin) {
+extern "C" int vxm_conv3d_tcs_pack_desc_blk(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int kd, int coutp, int transposed,
+                                            int n0, int nb, int k0, int kb, int begin) {
   VXM_REQUIRE(desc_host && w && wpk && Cout > 0 && Cin > 0 && (kd == 1 || kd == 3) && (coutp == 16 || coutp == 32 || coutp == 48 || coutp == 64),
               "conv3d_tcs_pack_desc: bad argument");
   const int cin_eff = transposed ? Cout : Cin, nout = transposed ? Cin : Cout;
-  VXM_REQUIRE(nout <= coutp && cin_eff <= 64, "conv3d_tcs_pack_desc: channel counts do not fit");
+  VXM_REQUIRE(n0 >= 0 && nb > 0 && n0 + nb <= nout && k0 >= 0 && kb > 0 && k0 + kb <= cin_eff, "conv3d_tcs_pack_desc: block out of range");
+  VXM_REQUIRE(nb <= coutp && kb <= 64, "conv3d_tcs_pack_desc: channel counts do not fit");
   int g0, g1;
-  groups_of(cin_eff <= 8 ? 8 : (cin_eff <= 16 ? 16 : (cin_eff <= 32 ? 32 : (cin_eff <= 48 ? 48 : 64))), &g0, &g1);
+  groups_of(kb <= 8 ? 8 : (kb <= 16 ? 16 : (kb <= 32 ? 32 : (kb <= 48 ? 48 : 64))), &g0, &g1);
   PackDesc d;
   d.w = w; d.out = (__nv_bfloat16*)wpk; d.Cout = Cout; d.Cin = Cin; d.KD = kd; d.COUT = coutp; d.NN = 3 * coutp; d.G0 = g0; d.G1 = g1;
   d.transposed = transposed; d.begin = begin; d.count = kd * 3 * d.NN * (g0 + g1); d.fold = 0;
+  d.n0 = n0; d.nb = nb; d.k0 = k0; d.kb = kb;
   memcpy(desc_host, &d, sizeof(d));
   return d.count;      // elements of this operand (>= 0), so the caller can chain `begin`
+}
+
+extern "C" int vxm_conv3d_tcs_pack_desc(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int kd, int coutp, int transposed,
+                                        int begin) {
+  VXM_REQUIRE(Cout > 0 && Cin > 0, "conv3d_tcs_pack_desc: bad argument");
+  return vxm_conv3d_tcs_pack_desc_blk(desc_host, w, wpk, Cout, Cin, kd, coutp, transposed, 0, transposed ? Cin : Cout, 0,
+                                      transposed ? Cout : Cin, begin);
 }
 
 // Descriptor of a kd-folded 2-D operand of the 3-D weight w (Cout, Cin, 3, 3, 3): the operand has 3 * (Cin | Cout if
@@ -611,6 +632,7 @@ extern "C" int vxm_conv3d_tcs_pack_desc_fold(void* desc_host, const float* w, vo
   PackDesc d;
   d.w = w; d.out = (__nv_bfloat16*)wpk; d.Cout = Cout; d.Cin = Cin; d.KD = 1; d.COUT = coutp; d.NN = 3 * coutp; d.G0 = g0; d.G1 = g1;
   d.transposed = transposed; d.begin = begin; d.count = 3 * d.NN * (g0 + g1); d.fold = real_in;
+  d.n0 = d.nb = d.k0 = d.kb = 0;
   memcpy(desc_host, &d, sizeof(d));
   return d.count;
 }
@@ -630,14 +652,34 @@ extern "C" int vxm_conv3d_tcs_supported(int Ca, int Cb, int Cout) {
 
 static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                            int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, void* stream);
+                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, void* stream);
+
+// shared memory of one launch outside the slab ring: packed weights, accumulator read-out buffers, barriers
+static size_t fixed_smem(uint32_t wbytes) { return ((wbytes + 1023u) & ~1023u) + NGRP * ACC_STAGE_FLOATS * sizeof(float) + 1024 + 512; }
+
+extern "C" int vxm_conv3d_tcs_fits(int cin, int coutp, int kd) {
+  int g0, g1;
+  groups_of(cin <= 8 ? 8 : (cin <= 16 ? 16 : (cin <= 32 ? 32 : (cin <= 48 ? 48 : 64))), &g0, &g1);
+  const size_t slab4 = (size_t)6 * WT * (g0 + g1) * 2;
+  return fixed_smem((uint32_t)vxm_conv3d_tcs_packed_bytes(cin, coutp, kd)) + 4 * slab4 <= 227 * 1024;
+}
 
 extern "C" int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                                   int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
                                   float slope, void* out2, int csplit, void* stream) {
   VXM_REQUIRE(out_mode == 0 || out_mode == 1, "conv3d_tcs_fwd: out_mode must be 0 (bf16 channels-last) or 1 (fp32 planar)");
   return conv_tcs_launch(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, out2, csplit,
-                         nullptr, nullptr, stream);
+                         nullptr, nullptr, 0, stream);
+}
+
+extern "C" int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
+                                      const void* mask, const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout,
+                                      int coutp, int kd, int out_mode, float slope, int opitch, void* stream) {
+  VXM_REQUIRE(out_mode == 0 || out_mode == 2 || out_mode == 3, "conv3d_tcs_fwd_blk: out_mode must be 0 (bf16), 2 (fp32 partial sums) or 3 (bf16 hi/lo pair)");
+  VXM_REQUIRE(out_mode != 3 || out_lo, "conv3d_tcs_fwd_blk: out_mode 3 needs out_lo");
+  VXM_REQUIRE(opitch == 0 || (opitch >= Cout && opitch % 8 == 0 && out_mode != 2), "conv3d_tcs_fwd_blk: bad output pitch %d", opitch);
+  return conv_tcs_launch(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, nullptr, 0,
+                         acc_in, out_lo, opitch == Cout ? 0 : opitch, stream);
 }
 
 extern "C" int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
@@ -652,12 +694,12 @@ extern "C" int vxm_conv3d_tcs_fwd_acc(const void* xa, const void* xb, const void
   VXM_REQUIRE(out_mode >= 1 && out_mode <= 3, "conv3d_tcs_fwd_acc: out_mode must be 1 (fp32 planar), 2 (fp32 partial sums) or 3 (bf16 hi/lo pair)");
   VXM_REQUIRE(out_mode != 3 || out_lo, "conv3d_tcs_fwd_acc: out_mode 3 needs out_lo");
   return conv_tcs_launch(xa, xb, wpk, bias, out, nullptr, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, nullptr, 0,
-                         acc_in, out_lo, stream);
+                         acc_in, out_lo, 0, stream);
 }
 
 static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                            int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, void* stream) {
+                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, void* stream) {
   VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0 && wpk && out, "conv3d_tcs_fwd: bad argument");
   VXM_REQUIRE(kd == 1 || kd == 3, "conv3d_tcs_fwd: kd must be 1 or 3");
   VXM_REQUIRE(coutp == 16 || coutp == 32 || coutp == 48 || coutp == 64, "conv3d_tcs_fwd: padded Cout must be 16, 32, 48 or 64");
@@ -674,16 +716,19 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   a.out = out; a.mask = (const __nv_bfloat16*)mask; a.out2 = out2; a.csplit = csplit;
   a.acc_in = acc_in; a.out_lo = out_lo;
   a.B = B; a.D = D; a.H = H; a.W = W; a.Ca = Ca; a.Cb = Cb; a.up = up; a.upd = (up && kd == 3) ? 1 : 0;
-  a.Cout = Cout; a.out_mode = out_mode; a.slope = slope;
+  a.Cout = Cout; a.out_mode = out_mode; a.slope = slope; a.opitch = opitch;
+  // the channel-blocked launches: 32-channel blocks of a 3-D layer, K groups of 64 or 32 + 16 channels (see tc.conv_blocks)
+  VXM_REQUIRE(!opitch || (!out2 && out_mode != 1 && kd == 3 && coutp == 32 && ((g0 == 64 && g1 == 0) || (g0 == 32 && g1 == 16))),
+              "conv3d_tcs_fwd: no blocked kernel for (%d,%d)->%d/%d, kd %d", Ca, Cb, Cout, coutp, kd);
   a.wbytes = (uint32_t)vxm_conv3d_tcs_packed_bytes(cin, coutp, kd);
-  const size_t fixed = ((a.wbytes + 1023u) & ~1023u) + NGRP * ACC_STAGE_FLOATS * sizeof(float) + 1024 + 512;
+  const size_t fixed = fixed_smem(a.wbytes);
   // tile height: 8 rows (two tile halves per slab step, one per MMA warpgroup) when the ring still holds >= 5 slabs
   int HTv = 4;
   {
     const size_t slab8 = (size_t)10 * WT * (g0 + g1) * 2;
     const int ns8 = (int)((227 * 1024 - fixed) / slab8);
     const char* e = getenv("VXM_B200_TCS_HT");
-    if (g0 <= 32 && coutp <= 32 && ns8 >= (kd == 3 ? 5 : 3) && H > 4 && !(e && e[0] == '4')) HTv = 8;
+    if (g0 <= 32 && coutp <= 32 && ns8 >= (kd == 3 ? 5 : 3) && H > 4 && !(e && e[0] == '4') && !opitch) HTv = 8;
   }
   a.tiles_h = (H + HTv - 1) / HTv; a.tiles_w = (W + WUSE - 1) / WUSE;
   int nsm = sm_count();
@@ -726,10 +771,19 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     else if (plain && !out2 && mask && !bias) epi = 2;
     else if (plain && !mask && !bias && slope < 0.f && (!out2 || csplit % 16 == 0)) epi = 3;
   }
-#define VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, ACC_, E_)                                                                       \
+#define VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, ACC_, E_, ...)                                                                  \
   do {                                                                                                                            \
-    VXM_CUDA(cudaFuncSetAttribute(conv_tcs_kernel<KD_, G0_, G1_, CO_, HT_, ACC_, E_>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    conv_tcs_kernel<KD_, G0_, G1_, CO_, HT_, ACC_, E_><<<grid, NTHREADS, smem, st>>>(a);                                          \
+    VXM_CUDA(cudaFuncSetAttribute(conv_tcs_kernel<KD_, G0_, G1_, CO_, HT_, ACC_, E_, ##__VA_ARGS__>,                              \
+                                  cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                                       \
+    conv_tcs_kernel<KD_, G0_, G1_, CO_, HT_, ACC_, E_, ##__VA_ARGS__><<<grid, NTHREADS, smem, st>>>(a);                           \
+  } while (0)
+#define VXM_TCS_LAUNCH_OP(G0_, G1_)                                                                                               \
+  do {                                                                                                                            \
+    if (acc_epi) VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, true, 0, true);                                                             \
+    else if (epi == 1) VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 1, true);                                                      \
+    else if (epi == 2) VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 2, true);                                                      \
+    else if (epi == 3) VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 3, true);                                                      \
+    else VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 0, true);                                                                    \
   } while (0)
 #define VXM_TCS_LAUNCH(KD_, G0_, G1_, CO_, HT_)                                                                                   \
   do {                                                                                                                            \
@@ -752,7 +806,9 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     else if (g0 == 32) VXM_TCS_LAUNCH(KD_, 32, 16, CO_, 4);                   \
     else VXM_TCS_LAUNCH(KD_, 64, 0, CO_, 4);                                  \
   } while (0)
-  if (HTv == 8) {
+  if (opitch) {
+    if (g0 == 64) VXM_TCS_LAUNCH_OP(64, 0); else VXM_TCS_LAUNCH_OP(32, 16);
+  } else if (HTv == 8) {
     if (kd == 3) { if (coutp == 16) VXM_TCS_G8(3, 16); else VXM_TCS_G8(3, 32); }
     else { if (coutp == 16) VXM_TCS_G8(1, 16); else VXM_TCS_G8(1, 32); }
   } else if (kd == 3) { if (coutp == 16) VXM_TCS_G(3, 16); else if (coutp == 32) VXM_TCS_G(3, 32); else if (coutp == 48) VXM_TCS_G(3, 48); else VXM_TCS_G(3, 64); }

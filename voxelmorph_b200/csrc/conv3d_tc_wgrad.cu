@@ -366,7 +366,7 @@ bool wgrad2_supported(int Ca, int Cb, int Cg);
 struct ReduceDesc;
 int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
                   int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer = nullptr,
-                  size_t* work_used = nullptr, bool khm = false);
+                  size_t* work_used = nullptr, bool khm = false, int x_pitch = 0, int g_pitch = 0, int co_off = 0);
 }
 }
 

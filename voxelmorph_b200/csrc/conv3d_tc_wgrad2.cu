@@ -43,6 +43,7 @@ struct Wgrad2Args {
   int B, D, H, W;
   int tiles_h, tiles_w, dchunk, nchunks, nitems, nslot;
   int dbg;      // profiling only (VXM_B200_WGRAD_DBG): 2 = no slab copies, 4 = no bias sums
+  int xpitch, gpitch;   // channels per voxel of the x / gz tensors (> Cx / Cg: a channel slice of a wider tensor)
 };
 
 __host__ __device__ inline uint32_t swz(uint32_t off, uint32_t width) { return off ^ (((off >> 7) & (width / 16 - 1)) << 4); }
@@ -129,7 +130,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
         const int h = h0 - 1 + (row >> 5), w = w0 - 1 + (row & 31);
         doff[k] = swz((uint32_t)row * WA + (uint32_t)c8 * 16u, WA);
         soff[k] = -1;
-        if (h >= 0 && h < a.H && w >= 0 && w < a.W && c8 < ncx) soff[k] = ((a.up ? h >> 1 : h) * Wx + (a.up ? w >> 1 : w)) * a.Cx + c8 * 8;
+        if (h >= 0 && h < a.H && w >= 0 && w < a.W && c8 < ncx) soff[k] = ((a.up ? h >> 1 : h) * Wx + (a.up ? w >> 1 : w)) * a.xpitch + c8 * 8;
       }
       int goff[KG];
       uint32_t gdoff[KG];
@@ -140,14 +141,14 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
         const int jj = row & 31, h = h0 + (row >> 5), w = w0 - 1 + jj;
         gdoff[k] = swz((uint32_t)(GPAD + row) * WG + (uint32_t)c8 * 16u, WG);
         goff[k] = -1;
-        if (jj >= 1 && jj <= TUSE && h < a.H && w < a.W && c8 < ncg) goff[k] = (h * a.W + w) * a.Cg + c8 * 8;
+        if (jj >= 1 && jj <= TUSE && h < a.H && w < a.W && c8 < ncg) goff[k] = (h * a.W + w) * a.gpitch + c8 * 8;
       }
       for (int ds = s_begin; ds < s_end; ++ds) {
         // ---- x slab of input slice ds ----
         mbar_wait(&xempty[xslot], xphase);
         uint8_t* slab = s_x + (size_t)xslot * XSLAB;
         const bool dok = ds >= 0 && ds < a.D;
-        const __nv_bfloat16* base = a.x + (((size_t)b * Dx + (dok ? (a.upd ? ds >> 1 : ds) : 0)) * Hx * Wx) * a.Cx;
+        const __nv_bfloat16* base = a.x + (((size_t)b * Dx + (dok ? (a.upd ? ds >> 1 : ds) : 0)) * Hx * Wx) * a.xpitch;
 #pragma unroll
         for (int k = 0; k < KX; ++k) {
           const bool ok = dok && soff[k] >= 0;
@@ -163,7 +164,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
         if (dg >= d0 && dg < d1) {
           mbar_wait(&gempty[gslot], gphase);
           uint8_t* gt = s_g + (size_t)gslot * GSLAB;
-          const __nv_bfloat16* baseG = a.gz + (((size_t)b * a.D + dg) * a.H * a.W) * a.Cg;
+          const __nv_bfloat16* baseG = a.gz + (((size_t)b * a.D + dg) * a.H * a.W) * a.gpitch;
 #pragma unroll
           for (int k = 0; k < KG; ++k) {
             const bool ok = goff[k] >= 0;
@@ -336,6 +337,7 @@ __global__ void __launch_bounds__(256) wgrad2_reduce_kernel(const float* __restr
 struct ReduceDesc {
   const float* partial; float* gw; const float* bias_partial; float* gb;
   int ncta, T, G, GOUT, Cout, Cin_total, ci_off, ci_cnt, accumulate, blk_begin;
+  int co_off;            // first output channel of a gz slice (gw rows co_off .. co_off + Cout - 1; gb already offset)
 };
 constexpr int MAXRED = 40;
 struct ReduceBatch {
@@ -367,7 +369,7 @@ __global__ void __launch_bounds__(256) wgrad2_reduce_multi_kernel(const ReduceBa
     const int co = j % r.GOUT, ci = (j / r.GOUT) % r.G, tap = j / (r.GOUT * r.G);
     if (co < r.Cout && ci < r.ci_cnt) {
       const float tot = ((sh[0][tx] + sh[1][tx]) + sh[2][tx]) + sh[3][tx];
-      float* dst = r.gw + ((size_t)co * r.Cin_total + r.ci_off + ci) * r.T + tap;
+      float* dst = r.gw + ((size_t)(r.co_off + co) * r.Cin_total + r.ci_off + ci) * r.T + tap;
       *dst = (r.accumulate ? *dst : 0.f) + tot;
     }
   }
@@ -393,10 +395,12 @@ bool wgrad2_supported(int Ca, int Cb, int Cg) {
 // one source tensor (C channels, optionally nearest-x2 upsampled) against gz; weights [ci_off, ci_off + ci_cnt) of Cin_total
 int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
                   int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer,
-                  size_t* work_used, bool khm) {
+                  size_t* work_used, bool khm, int x_pitch, int g_pitch, int co_off) {
+  VXM_REQUIRE(defer || co_off == 0, "conv3d_tc_wgrad2: gz slices need the deferred reduction");
   Wgrad2Args a{};
   a.x = (const __nv_bfloat16*)x; a.Cx = Cx; a.up = up; a.upd = (up && kd == 3) ? 1 : 0;
   a.gz = (const __nv_bfloat16*)gz; a.Cg = Cg;
+  a.xpitch = x_pitch ? x_pitch : Cx; a.gpitch = g_pitch ? g_pitch : Cg;
   a.B = B; a.D = D; a.H = H; a.W = W;
   a.tiles_h = (H + TH - 1) / TH; a.tiles_w = (W + TUSE - 1) / TUSE;
   {
@@ -459,6 +463,7 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
     defer->partial = a.partial; defer->gw = grad_w; defer->bias_partial = a.bias_partial; defer->gb = grad_b;
     defer->ncta = grid; defer->T = T; defer->G = G; defer->GOUT = GOUT; defer->Cout = Cout_real; defer->Cin_total = Cin_total;
     defer->ci_off = ci_off; defer->ci_cnt = ci_cnt; defer->accumulate = accumulate; defer->blk_begin = (per_cta + 63) / 64;   // block count, turned into an offset by the flush
+    defer->co_off = co_off;
     return VXM_OK;
   }
   wgrad2_reduce_kernel<<<(per_cta + 63) / 64, 256, 0, st>>>(a.partial, grad_w, grid, T, G, GOUT, Cout_real, Cin_total, ci_off, ci_cnt,
@@ -480,33 +485,46 @@ extern "C" size_t vxm_conv3d_tc_wgrad2_partial_bytes(int kd) {
   return 2 * ((size_t)256 * kd * 9 * 32 * 32 + 256 * 32) * sizeof(float) + 1024;
 }
 
+static bool chan_ok64(int c) { return chan_ok(c) || c == 64; }
+
+// A 64-channel x source or gz runs as 32-channel slices of both operands (every kernel launch one of the existing
+// <= 32 x 32 instantiations), each slice pair with its own pending reduction into its block of grad_w.  Workspace per
+// layer: at most vxm_conv3d_tc_wgrad2_partial_bytes(kd) per two slice pairs.
 extern "C" int vxm_conv3d_tc_wgrad2_partial(const void* xa, const void* xb, const void* gz, float* grad_w, float* grad_b, void* work,
                                             size_t work_bytes, size_t* work_used, void* descs_host, int* ndesc, int B, int D, int H, int W,
                                             int Ca, int Cb, int up, int Cin_real, int Cg, int Cout_real, int kd, int accumulate, void* stream) {
   VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0 && grad_w && work && work_used && descs_host && ndesc && gz, "conv3d_tc_wgrad2_partial: bad argument");
   VXM_REQUIRE(kd == 1 || kd == 3, "conv3d_tc_wgrad2_partial: kd must be 1 or 3");
-  VXM_REQUIRE(wgrad2_supported(Ca, Cb, Cg), "conv3d_tc_wgrad2_partial: channel counts (%d,%d | %d) unsupported", Ca, Cb, Cg);
+  const char* e = getenv("VXM_B200_WGRAD");
+  VXM_REQUIRE(!(e && e[0] == 'o') && (Ca == 0 || chan_ok64(Ca)) && (Cb == 0 || chan_ok64(Cb)) && Ca + Cb > 0 && chan_ok64(Cg),
+              "conv3d_tc_wgrad2_partial: channel counts (%d,%d | %d) unsupported", Ca, Cb, Cg);
   VXM_REQUIRE((Ca == 0 || xa) && (Cb == 0 || xb), "conv3d_tc_wgrad2_partial: missing source tensor");
-  VXM_REQUIRE(*ndesc + 2 <= MAXRED, "conv3d_tc_wgrad2_partial: too many pending reductions (flush first)");
+  const int nsub = ((Ca + 31) / 32 + (Cb + 31) / 32) * ((Cg + 31) / 32);
+  VXM_REQUIRE(*ndesc + (nsub > 2 ? nsub : 2) <= MAXRED, "conv3d_tc_wgrad2_partial: too many pending reductions (flush first)");
   VXM_REQUIRE(Cout_real > 0 && Cout_real <= Cg, "conv3d_tc_wgrad2_partial: Cout_real out of range");
   ReduceDesc* d = (ReduceDesc*)descs_host;
   cudaStream_t st = as_stream(stream);
-  size_t used = 0, total = 0;
+  size_t total = 0;
   char* wp = (char*)work;
-  if (Ca) {
-    const int cnt = Cin_real < Ca ? Cin_real : Ca;
-    int rc = wgrad2_launch(xa, Ca, up, gz, Cg, grad_w, grad_b, wp, B, D, H, W, kd, Cout_real, Cin_real, 0, cnt, accumulate, st, &d[*ndesc], &used, false);
-    if (rc) return rc;
-    VXM_REQUIRE(used <= work_bytes, "conv3d_tc_wgrad2_partial: workspace too small");
-    ++*ndesc; wp += used; total += used;
-  }
-  if (Cb && Cin_real > Ca) {
-    const int cnt = Cin_real - Ca < Cb ? Cin_real - Ca : Cb;
-    int rc = wgrad2_launch(xb, Cb, 0, gz, Cg, grad_w, Ca ? nullptr : grad_b, wp, B, D, H, W, kd, Cout_real, Cin_real, Ca, cnt, accumulate, st,
-                           &d[*ndesc], &used, false);
-    if (rc) return rc;
-    VXM_REQUIRE(total + used <= work_bytes, "conv3d_tc_wgrad2_partial: workspace too small");
-    ++*ndesc; total += used;
+  const void* src[2] = {xa, xb};
+  const int C[2] = {Ca, Cb}, ci0[2] = {0, Ca}, sup[2] = {up, 0};
+  for (int s = 0; s < 2; ++s) {
+    for (int xs = 0; xs < C[s] && ci0[s] + xs < Cin_real; xs += 32) {
+      const int cx = C[s] - xs < 32 ? C[s] - xs : 32;
+      const int cnt = Cin_real - ci0[s] - xs < cx ? Cin_real - ci0[s] - xs : cx;
+      for (int gs = 0; gs < Cg && gs < Cout_real; gs += 32) {
+        const int cg = Cg - gs < 32 ? Cg - gs : 32;
+        const int cout = Cout_real - gs < cg ? Cout_real - gs : cg;
+        // the bias gradient (sum of gz) is taken once per gz slice, with the first x slice
+        float* gb = (grad_b && ci0[s] + xs == 0) ? grad_b + gs : nullptr;
+        size_t used = 0;
+        int rc = wgrad2_launch((const __nv_bfloat16*)src[s] + xs, cx, sup[s], (const __nv_bfloat16*)gz + gs, cg, grad_w, gb, wp, B, D, H, W,
+                               kd, cout, Cin_real, ci0[s] + xs, cnt, accumulate, st, &d[*ndesc], &used, false, C[s], Cg, gs);
+        if (rc) return rc;
+        VXM_REQUIRE(total + used <= work_bytes, "conv3d_tc_wgrad2_partial: workspace too small");
+        ++*ndesc; wp += used; total += used;
+      }
+    }
   }
   *work_used = total;
   return VXM_OK;
@@ -524,7 +542,7 @@ extern "C" int vxm_conv3d_tc_wgrad2_partial_khm(const void* x, const void* gz, f
   ReduceDesc* d = (ReduceDesc*)descs_host;
   size_t used = 0;
   int rc = wgrad2_launch(x, Cx, 0, gz, Cg, grad_w, grad_b, work, B, D, H, W, 1, Cout_real, Cin_real, 0, Cin_real, accumulate, as_stream(stream),
-                         &d[*ndesc], &used, true);
+                         &d[*ndesc], &used, true, 0, 0, 0);
   if (rc) return rc;
   VXM_REQUIRE(used <= work_bytes, "conv3d_tc_wgrad2_partial_khm: workspace too small");
   ++*ndesc;

@@ -54,7 +54,7 @@ class _PackPlan:
         self.params = [c.weight for c in convs]
         dev = self.params[0].device
         dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-        host = ctypes.create_string_buffer(dsz * (2 * len(convs) + 2))
+        host = ctypes.create_string_buffer(dsz * (16 * len(convs) + 2))      # <= 2 K x 4 N blocks per operand
         self.table = {}
         self.keep = []
         n, begin = 0, 0
@@ -79,10 +79,20 @@ class _PackPlan:
         for li, w in enumerate(self.params):
             w5 = w if w.dim() == 5 else w.unsqueeze(2)
             Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
+            # a concatenating layer (decoder, after an upsample) reads the previous layer's output first, then the skip
+            ca = self.params[li - 1].shape[0] if li and Cin > self.params[li - 1].shape[0] else Cin
             for transposed in (False, True):
                 if transposed and li == 0:
                     continue                      # the images need no gradient: no dgrad of the first layer
                 cin_eff, nout = (Cout, Cin) if transposed else (Cin, Cout)
+                if li and Cout <= 64 and ca <= 64 and Cin - ca <= 64:
+                    blocks = tc.conv_blocks(Cout, 0, Cin, int(kd), ca if ca < Cin else None) if transposed else \
+                        tc.conv_blocks(ca, Cin - ca, Cout, int(kd))
+                    if blocks is not None:        # channel-blocked layer: one operand per (K block, N block)
+                        packs, n, begin = tc.block_descs(w, transposed, blocks, host, n, begin, dsz)
+                        self.table[(id(w), transposed, "blk")] = (blocks, packs)
+                        self.keep.extend(p[0] for p in packs.values())
+                        continue
                 if nout > 64 or cin_eff > 64:
                     continue
                 coutp = 16 if nout <= 16 else (32 if nout <= 32 else (48 if nout <= 48 else 64))
@@ -114,6 +124,11 @@ class _PackPlan:
     def lookup(self, w, transposed):
         return self.table.get((id(w), transposed))
 
+    def lookup_blocks(self, w, transposed, blocks):
+        """Block operands of `w` packed for `blocks` (tc.conv_blocks), or None."""
+        hit = self.table.get((id(w), transposed, "blk"))
+        return hit[1] if hit is not None and hit[0] == blocks else None
+
     def lookup_fold(self, w, transposed):
         return self.table.get((id(w), transposed, "fold"))
 
@@ -131,8 +146,10 @@ def _plan_of(model):
 
 
 def supports(model):
-    """True when every convolution of `model` (a VxmDense) has a shape the tensor-core kernels implement: feature
-    counts in {8, 16, 32}, concatenated inputs a multiple of 16 and at most 64 channels, at most 8 image planes."""
+    """True when every convolution of `model` (a VxmDense) runs in one launch per layer on the tensor-core kernels: feature
+    counts in {8, 16, 32}, concatenated inputs a multiple of 16 and at most 64 channels, at most 8 image planes.  This is
+    what VXM_B200_CONV_ENGINE=tc selects the tensor cores for; VXM_B200_CONV_ENGINE=bf16 | bf16x3 also run U-Nets with
+    64-channel layers and concatenations of up to 128 channels, in channel blocks (tc.conv_blocks)."""
     try:
         unet = model.unet_model
         convs = [b.main for lvl in unet.encoder for b in lvl] + [b.main for lvl in unet.decoder for b in lvl] + \
@@ -153,8 +170,8 @@ def supports(model):
 
 
 def _check_cout(c, what):
-    if c not in (8, 16, 32):
-        raise _lib.VxmError("bf16 tensor-core engine: %s has %d channels; supported feature counts are 8, 16 and 32 "
+    if c not in (8, 16, 32, 64):
+        raise _lib.VxmError("bf16 tensor-core engine: %s has %d channels; supported feature counts are 8, 16, 32 and 64 "
                             "(use VXM_B200_CONV_ENGINE=f32 for other U-Net shapes)" % (what, c))
 
 
@@ -200,6 +217,17 @@ def _run_conv_split(cv, kd):
     def packs():
         wh, wl = tc.split_weights(cv.w)
         return tc.pack_weights_t(wh, variant="s"), tc.pack_weights_t(wl, variant="s")
+    blocks = None if cv.planar_out else tc.conv_blocks(_width(cv.xa), _width(cv.xb), cv.cout, kd)
+    if blocks is not None:
+        def block_packs():
+            sp = getattr(cv.w, "_vxm_split_blocks", None)       # persistent buffers: the refresh stays graph-capturable
+            if sp is None or sp.blocks != blocks:
+                sp = tc.SplitBlockPacks(cv.w, blocks)
+                cv.w._vxm_split_blocks = sp
+            return sp.refresh(cv.w)
+        sp = _cache.get(cv.w, "fwd_split_blk", block_packs)
+        return tc.conv_fwd_blocked(cv.xa, cv.xb, blocks, sp.hi, cv.b.detach() if cv.b is not None else None, cv.cout, kd, up=cv.up,
+                                   slope=cv.slope, lo=(cv.xa_lo, cv.xb_lo, sp.lo))
     pk = _cache.get(cv.w, "fwd_split", packs)
     xa = None if cv.xa is None else (cv.xa, cv.xa_lo)
     xb = None if cv.xb is None else (cv.xb, cv.xb_lo)
@@ -207,10 +235,26 @@ def _run_conv_split(cv, kd):
                              out_fp32_planar=cv.planar_out, slope=cv.slope)
 
 
+def _width(x):
+    return 0 if x is None else x.shape[-1]
+
+
+def _block_packs(plan, cv, transposed, blocks):
+    packs = plan.lookup_blocks(cv.w, transposed, blocks) if plan is not None else None
+    if packs is None:
+        raise _lib.VxmError("bf16 engine: the %d -> %d convolution runs in channel blocks, which need the swizzled kw-stacked "
+                            "kernel (VXM_B200_TC_KERNEL=auto|s)" % (cv.cin, cv.cout))
+    return packs
+
+
 def _run_conv(cv, kd, plan=None):
     """Forward of one tape entry."""
     ca = 0 if cv.xa is None else cv.xa.shape[-1]
     cb = 0 if cv.xb is None else cv.xb.shape[-1]
+    blocks = None if (cv.planar is not None or cv.fold == "x" or cv.planar_out) else tc.conv_blocks(ca, cb, cv.cout, kd)
+    if blocks is not None:
+        return tc.conv_fwd_blocked(cv.xa, cv.xb, blocks, _block_packs(plan, cv, False, blocks), cv.b.detach() if cv.b is not None else None,
+                                   cv.cout, kd, up=cv.up, slope=cv.slope)
     if cv.fold == "x":
         # kd folded into the input channels: a 2-D convolution per slice (3 instead of 9 MMA steps per tile)
         wpk, cp = plan.lookup_fold(cv.w, False)
@@ -269,9 +313,9 @@ def forward_tape(model, source, target, split=False):
             if first_layer:
                 if ca != 8 or cb or cv.cin > 8 or (cv.fold == "x" and 3 * cv.cin > 8):
                     raise _lib.VxmError("bf16 engine: the first convolution takes at most 8 input feature planes")
-            elif ca + cb != cv.cin or (ca + cb) % 16 or ca + cb > 64:
-                raise _lib.VxmError("bf16 engine: unsupported convolution input channels %d (+%d); need a multiple of 16, at most 64"
-                                    % (ca, cb))
+            elif ca + cb != cv.cin or (ca + cb) % 16 or ca + cb > (64 if planar_out else 128):
+                raise _lib.VxmError("bf16 engine: unsupported convolution input channels %d (+%d); need a multiple of 16, at most 128 "
+                                    "(64 into the flow head) (use VXM_B200_CONV_ENGINE=f32 for other U-Net shapes)" % (ca, cb))
         out = _run_conv_split(cv, kd) if split else _run_conv(cv, kd, plan)
         cv.out_id = new_id()
         if split and not planar_out:
@@ -392,7 +436,10 @@ def backward_tape(ctx, g_flow):
             # first layer over the kd-folded images: 2-D weight gradient with kh in M, no dgrad
             gwf = torch.empty((cv.cout, 3 * cv.cin, 1, 3, 3), dtype=torch.float32, device=dev)
             gbf = torch.empty(cv.cout, dtype=torch.float32, device=dev) if cv.b is not None else None
-            batch.add_khm(cv.xa, g_in, gwf, gbf, 3 * cv.cin, cv.cout)
+            if g_in.shape[-1] <= 16:
+                batch.add_khm(cv.xa, g_in, gwf, gbf, 3 * cv.cin, cv.cout)
+            else:      # kh-in-M takes at most 16 output channels: a wider first layer runs the plain 2-D kernel
+                batch.add(cv.xa, None, g_in, gwf, gbf, 3 * cv.cin, cv.cout, 1, False, False)
             folded.append((cv, gwf, gbf, "x"))
             continue
         # parameters whose .grad is a view of FusedAdam's flat gradient buffer (optim.FlatParams marks them)
@@ -416,7 +463,10 @@ def backward_tape(ctx, g_flow):
             t = cv.a_id
             msk = tensors[t] if producer[t] == "conv" else None
             sl = _slope_of(ctx, t) if producer[t] == "conv" else None
-            if tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
+            blocks = tc.conv_blocks(g_in.shape[-1], 0, cv.cin, kd)
+            if blocks is not None:
+                res = tc.conv_fwd_blocked(g_in, None, blocks, _block_packs(plan, cv, True, blocks), None, cv.cin, kd, slope=sl, mask=msk)
+            elif tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
                 hit = plan.lookup(cv.w, True) if (plan is not None and tc._use_s(g_in.shape[-1], 0, cv.cin)) else None
                 wpk, cp = hit if hit is not None else _cache.get(cv.w, "dgrad_t", lambda: tc.pack_weights_t(w, transposed=True))
                 res = tc.conv_fwd_t(g_in, None, wpk, cp, None, cv.cin, kd, slope=sl, mask=msk)
@@ -430,7 +480,10 @@ def backward_tape(ctx, g_flow):
         else:
             ca = cv.xa.shape[-1]
             # single dgrad pass over the whole concat input: N = Ca + Cb output channels, split on store
-            if tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
+            blocks = tc.conv_blocks(g_in.shape[-1], 0, cv.cin, kd, ca)
+            if blocks is not None:
+                g_up, g_sk = tc.conv_fwd_blocked(g_in, None, blocks, _block_packs(plan, cv, True, blocks), None, cv.cin, kd, split=ca)
+            elif tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
                 hit = plan.lookup(cv.w, True) if (plan is not None and tc._use_s(g_in.shape[-1], 0, cv.cin)) else None
                 wpk, cp = hit if hit is not None else _cache.get(cv.w, "dgrad_t", lambda: tc.pack_weights_t(w, transposed=True))
                 g_up, g_sk = tc.conv_fwd_t(g_in, None, wpk, cp, None, cv.cin, kd, split=ca)

@@ -5,6 +5,7 @@ Activations of this engine are bf16, channels-last: a (B, C, D, H, W) logical te
 (Cout, Cin, 3, 3, 3)); packed bf16 copies are refreshed whenever the parameter version changes.
 """
 import ctypes
+import functools
 import threading
 
 import torch
@@ -13,7 +14,7 @@ from . import _lib
 
 
 def np_for(cout):
-    """MMA N (16 or 32) for a layer with `cout` output channels."""
+    """MMA N (16, 32, 48 or 64) for a launch with `cout` output channels (wider layers: conv_blocks)."""
     if cout <= 16:
         return 16
     if cout <= 32:
@@ -264,6 +265,146 @@ def conv_fwd_t(xa, xb, wpk, coutp, bias, cout, kd, up=False, out_fp32_planar=Fal
     return (out, out2) if split else out
 
 
+# ---- channel-blocked execution of the layers one launch cannot hold (64 -> 64, 128 -> 64, ...) -------------------------
+
+@functools.lru_cache(maxsize=None)
+def conv_blocks(ca, cb, nout, kd, split=None):
+    """Channel blocks of a convolution with inputs xa (ca channels) + xb (cb) and `nout` outputs (split: the first
+    `split` outputs go to one tensor, the rest to another), or None when one launch of the kw-stacked kernel takes it.
+    Returns (K blocks [(src, k0, kb)], N blocks [(n0, nb, dst, doff)]): src 0 = xa alone, 1 = xb alone, 2 = both; output
+    channels [n0, n0 + nb) land in output `dst` at channel `doff`.  A concatenation over 64 channels is split at the
+    source boundary (sources have at most 64 channels), the 64-channel source last: its launch runs the epilogue.  Output
+    blocks are 64 channels wide where the packed weights of one leave room for the slab ring, else 32 (3-D, 64-channel K)."""
+    lib = _lib.load()
+    cin = ca + cb
+    if cin <= 64 and nout <= 64 and lib.vxm_conv3d_tcs_fits(cin, np_for(nout), kd):
+        return None
+    if cin <= 64:
+        ks = ((2, 0, cin),)
+    else:
+        ks = ((0, 0, ca), (1, ca, cb))
+        if ca == 64 and cb != 64:
+            ks = ks[::-1]
+    nbmax = 64 if lib.vxm_conv3d_tcs_fits(max(k[2] for k in ks), 64, kd) else 32
+    pieces = [(0, split, 0), (split, nout - split, 1)] if split else [(0, nout, 0)]
+    return ks, tuple((p0 + j, min(nbmax, pn - j), dst, j) for p0, pn, dst in pieces for j in range(0, pn, nbmax))
+
+
+def block_descs(w, transposed, blocks, host, n, begin, dsz):
+    """Appends the pack descriptors of every (K block, N block) operand of `w` to the host array `host` (n filled so far,
+    element offset `begin`).  Returns ({(ki, ni): (tensor, coutp)}, n, begin)."""
+    lib = _lib.load()
+    w5 = w if w.dim() == 5 else w.unsqueeze(2)
+    Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
+    ks, ns = blocks
+    packs = {}
+    for ki, (_, k0, kb) in enumerate(ks):
+        for ni, (n0, nb, _, _) in enumerate(ns):
+            coutp = np_for(nb)
+            out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(kb, coutp, kd)) // 2, dtype=torch.bfloat16, device=w.device)
+            cnt = lib.vxm_conv3d_tcs_pack_desc_blk(ctypes.cast(ctypes.addressof(host) + n * dsz, ctypes.c_void_p), _lib.ptr(w5), _lib.ptr(out),
+                                                   Cout, Cin, kd, coutp, 1 if transposed else 0, n0, nb, k0, kb, begin)
+            if cnt <= 0:
+                raise _lib.VxmError("vxm_conv3d_tcs_pack_desc_blk: %s" % _lib.last_error())
+            packs[(ki, ni)] = (out, coutp)
+            n, begin = n + 1, begin + cnt
+    return packs, n, begin
+
+
+def pack_weights_blocks(w, transposed, blocks):
+    """Packed block operands of one weight (one launch).  Returns {(ki, ni): (tensor, coutp)}; the descriptor table stays
+    referenced by the result (key None) until the launch has read it."""
+    lib = _lib.load()
+    w = w.contiguous()
+    dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
+    host = ctypes.create_string_buffer(dsz * len(blocks[0]) * len(blocks[1]))
+    packs, n, total = block_descs(w, transposed, blocks, host, 0, 0, dsz)
+    descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(w.device)
+    _lib.check(lib.vxm_conv3d_tcs_pack_multi(_lib.ptr(descs), n, total, _lib.stream_ptr()), "vxm_conv3d_tcs_pack_multi")
+    packs[None] = (descs, w)
+    return packs
+
+
+class SplitBlockPacks:
+    """Split-precision (bf16x3) operands of a channel-blocked layer: the bf16 hi and lo parts of the weights (see
+    split_weights), packed per block into `hi` / `lo` ({(ki, ni): (tensor, coutp)}).  The descriptor table is uploaded once
+    and points at persistent fp32 buffers, so `refresh` (two elementwise kernels and one pack launch) can be captured in a
+    CUDA graph."""
+
+    def __init__(self, w, blocks):
+        lib = _lib.load()
+        self.blocks = blocks
+        self.w_hi, self.w_lo = torch.empty_like(w.detach()), torch.empty_like(w.detach())
+        dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
+        host = ctypes.create_string_buffer(dsz * 2 * len(blocks[0]) * len(blocks[1]))
+        self.hi, n, begin = block_descs(self.w_hi, False, blocks, host, 0, 0, dsz)
+        self.lo, self.n, self.total = block_descs(self.w_lo, False, blocks, host, n, begin, dsz)
+        self.descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(w.device)
+
+    def refresh(self, w):
+        w = w.detach()
+        self.w_hi.copy_(w.to(torch.bfloat16))
+        torch.sub(w, self.w_hi, out=self.w_lo)
+        _lib.check(_lib.load().vxm_conv3d_tcs_pack_multi(_lib.ptr(self.descs), self.n, self.total, _lib.stream_ptr()),
+                   "vxm_conv3d_tcs_pack_multi")
+        return self
+
+
+def _ptr_at(t, off):
+    return None if t is None else ctypes.c_void_p(t.data_ptr() + off * t.element_size())
+
+
+def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None, mask=None, split=None, lo=None):
+    """One convolution in channel blocks (see conv_blocks); packs[(ki, ni)] = (operand, coutp) of K block ki, N block ni.
+    Every N block accumulates its K blocks in an fp32 channels-last buffer (out_mode 2) and the last launch adds bias and
+    activation (or the LeakyReLU-derivative mask) and stores its channels into the full-width bf16 output.
+    lo = (xa_lo, xb_lo, packs_lo): split precision, three passes per K block; returns the (hi, lo) pair.
+    split: returns the outputs [0, split) and [split, nout) as two tensors (dgrad of a concatenation)."""
+    lib = _lib.load()
+    ks, ns = blocks
+    full = xb if xb is not None else xa
+    B, D, H, W = full.shape[0], full.shape[1], full.shape[2], full.shape[3]
+    if xb is None and up:
+        D, H, W = (D * 2 if kd == 3 else D), H * 2, W * 2
+    if mask is not None and split:
+        raise _lib.VxmError("conv_fwd_blocked: a mask with a split output is not implemented")
+    outs = [torch.empty((B, D, H, W, c), dtype=torch.bfloat16, device=full.device) for c in ([split, nout - split] if split else [nout])]
+    outs_lo = [torch.empty_like(o) for o in outs] if lo is not None else [None] * len(outs)
+    s = -1.0 if slope is None else float(slope)
+    ca = 0 if xa is None else xa.shape[-1]
+    for ni, (n0, nb, dst, doff) in enumerate(ns):
+        out, pitch = outs[dst], outs[dst].shape[-1]
+        passes = [(ki, 0, False) for ki in range(len(ks))] if lo is None else \
+                 [p for ki in range(len(ks)) for p in ((ki, 1, False), (ki, 0, True), (ki, 0, False))]   # x_lo w_hi, x_hi w_lo, x_hi w_hi
+        acc = None
+        for pi, (ki, xlo, wlo) in enumerate(passes):
+            src, _, kb = ks[ki]
+            pa = xa if not xlo else lo[0]
+            pb = xb if not xlo else lo[1]
+            if src == 0:
+                x0, x1, c0, c1, u = pa, None, kb, 0, up
+            elif src == 1:
+                x0, x1, c0, c1, u = pb, None, kb, 0, False
+            else:
+                x0, x1, c0, c1, u = pa, pb, ca, kb - ca, up
+            wpk, coutp = (lo[2] if wlo else packs)[(ki, ni)]
+            if pi + 1 < len(passes):
+                ain = acc
+                if acc is None:
+                    acc = torch.empty((B, D, H, W, coutp), dtype=torch.float32, device=full.device)
+                o, olo, m, mode, op, bptr = _lib.ptr(acc), None, None, 2, 0, None
+            else:
+                ain = acc
+                o, olo, m = _ptr_at(out, doff), _ptr_at(outs_lo[dst], doff), _ptr_at(mask, n0)
+                mode, op, bptr = (3 if lo is not None else 0), pitch, _ptr_at(bias, n0)
+            _lib.check(lib.vxm_conv3d_tcs_fwd_blk(_lib.ptr(x0), _lib.ptr(x1), _lib.ptr(wpk), bptr, o, olo, m, _lib.ptr(ain),
+                                                  B, D, H, W, c0, c1, 1 if u else 0, nb, coutp, kd, mode, s, op, _lib.stream_ptr()),
+                       "vxm_conv3d_tcs_fwd_blk")
+    if lo is not None:
+        return outs[0], outs_lo[0]
+    return tuple(outs) if split else outs[0]
+
+
 # ---- split-precision (bf16x3) passes ----------------------------------------------------------------------------------
 
 def split_weights(w):
@@ -375,12 +516,14 @@ class WgradBatch:
 
     def add(self, xa, xb, gz, gw, gb, cin, cout, kd, up, accumulate):
         lib = _lib.load()
-        need = int(lib.vxm_conv3d_tc_wgrad2_partial_bytes(kd))
-        if self.off + need > self.WORK_BYTES or self.n.value + 2 > self.maxn:
-            self.flush()
         B, D, H, W, Cg = gz.shape
         Ca = 0 if xa is None else xa.shape[-1]
         Cb = 0 if xb is None else xb.shape[-1]
+        # 64-channel operands run as 32-channel slices: one pending reduction per slice pair, partial_bytes per two pairs
+        nsub = ((Ca + 31) // 32 + (Cb + 31) // 32) * ((Cg + 31) // 32)
+        need = int(lib.vxm_conv3d_tc_wgrad2_partial_bytes(kd)) * ((nsub + 1) // 2)
+        if self.off + need > self.WORK_BYTES or self.n.value + max(2, nsub) > self.maxn:
+            self.flush()
         _lib.check(lib.vxm_conv3d_tc_wgrad2_partial(_lib.ptr(xa), _lib.ptr(xb), _lib.ptr(gz), _lib.ptr(gw), _lib.ptr(gb),
                                                     ctypes.c_void_p(self.work.data_ptr() + self.off), self.WORK_BYTES - self.off,
                                                     ctypes.byref(self.used), ctypes.cast(self.host, ctypes.c_void_p), ctypes.byref(self.n),
@@ -422,7 +565,7 @@ def wgrad_deferrable(xa, xb, gz, planar_x=None, planar_g=None):
         return False
     if gz is None or planar_x is not None or planar_g is not None:
         return False
-    ok = lambda c: c in (8, 16, 32)  # noqa: E731
+    ok = lambda c: c in (8, 16, 32, 64)  # noqa: E731
     ca = 0 if xa is None else xa.shape[-1]
     cb = 0 if xb is None else xb.shape[-1]
     return (ca == 0 or ok(ca)) and (cb == 0 or ok(cb)) and ca + cb > 0 and ok(gz.shape[-1])
