@@ -395,6 +395,7 @@ def test_wide_multi_tile_step_vs_oracle(cuda, monkeypatch, engine):
     [[4, 8, 8, 8], [8, 8, 8, 8, 8, 4, 4]],
     [[16, 24, 24, 24], [24, 24, 24, 24, 24, 16, 16]],
     [[32, 128, 64, 64], [64, 64, 64, 64, 64, 32, 32]],
+    [[16, 32, 32, 32], [32, 16, 32, 32, 32, 16, 16]],          # a 16 + 32 concatenation: no kernel takes it
 ])
 def test_wide_refusals_name_the_fp32_engine(vxm_env, cuda, feats):
     vxm = vxm_env("bf16")

@@ -44,7 +44,8 @@ def test_tc_default_still_picks_fp32_for_wide_models():
     prev = ops._default_engine
     try:
         ops.set_default_engine("tc")
-        for kw in (KW, dict(inshape=(32, 32, 48), nb_unet_features=16, nb_unet_levels=3, unet_feat_mult=2)):
+        for kw in (KW, dict(inshape=(32, 32, 48), nb_unet_features=16, nb_unet_levels=3, unet_feat_mult=2),
+                   dict(inshape=(32, 32, 32), nb_unet_features=[[16, 32, 32, 32], [32, 16, 32, 32, 32, 16, 16]])):   # 16 + 32 concat
             assert ops.resolve_engine(vxm.networks.VxmDense(**kw)) == "f32"
         assert ops.resolve_engine(vxm.networks.VxmDense((32, 32, 32))) == "bf16x3"
     finally:

@@ -1,11 +1,11 @@
-"""Localise non-finite gradients in the bf16 engine: per kernel variant, per parameter; then per tape convolution."""
+"""Localise non-finite gradients in the bf16 engine: per convolution launch, then per parameter."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
 import numpy as np, torch
 os.environ["VXM_B200_CONV_ENGINE"] = "bf16"
 import voxelmorph_b200 as vxm
-from voxelmorph_b200 import tc, engine_bf16
+from voxelmorph_b200 import tc
 from oracle import cases, ref_torch
 from test_oracle import full_cfg
 dev = torch.device("cuda:0")
@@ -31,26 +31,15 @@ def wrap(name):
             print("      non-finite counts of inputs:", ins)
         return out
     setattr(tc, name, f)
-for n in ("conv_fwd", "conv_fwd_t", "conv_wgrad"):
+for n in ("conv_fwd_t", "conv_fwd_blocked", "conv_wgrad"):
     wrap(n)
 
-ref = None
-for variant in ("n", "t", "s", "auto"):
-    os.environ["VXM_B200_TC_KERNEL"] = variant
-    engine_bf16.bump_weights_epoch()
-    model = vxm.networks.VxmDense(**kw)
-    model.load_state_dict(sd, strict=False)
-    model.to(dev).train()
-    print("variant", variant)
-    out = model(S, T)
-    loss = out[-1].square().sum() + out[0].square().sum()
-    loss.backward()
-    torch.cuda.synchronize()
-    g = {k: p.grad.detach().clone() for k, p in model.named_parameters()}
-    nbad = {k: int((~torch.isfinite(v)).sum()) for k, v in g.items()}
-    print("  nonfinite grads:", {k: v for k, v in nbad.items() if v})
-    if ref is None:
-        ref = g
-    else:
-        worst = max(((float((g[k] - ref[k]).abs().max() / ref[k].abs().max().clamp_min(1e-30)), k) for k in g if nbad[k] == 0), default=None)
-        print("  worst rel diff vs variant n:", worst)
+model = vxm.networks.VxmDense(**kw)
+model.load_state_dict(sd, strict=False)
+model.to(dev).train()
+out = model(S, T)
+loss = out[-1].square().sum() + out[0].square().sum()
+loss.backward()
+torch.cuda.synchronize()
+nbad = {k: int((~torch.isfinite(p.grad)).sum()) for k, p in model.named_parameters()}
+print("nonfinite grads:", {k: v for k, v in nbad.items() if v})

@@ -13,11 +13,10 @@ ash = (D // 2, H // 2, W // 2) if up else shape
 xa = torch.randn((1,) + ash + (Ca,), device=dev).to(torch.bfloat16)
 xb = torch.randn((1,) + shape + (Cb,), device=dev).to(torch.bfloat16) if Cb else None
 w = torch.randn((Cout, Ca + Cb, 3, 3, 3), device=dev) * 0.05
-wpk, NP = tc.pack_weights_t(w) if tc.use_t_kernel(Ca, Cb, Cout) else tc.pack_weights(w)
-fwd = tc.conv_fwd_t if isinstance(NP, tuple) else tc.conv_fwd
+wpk, cp = tc.pack_weights_t(w, variant="s")
 b = torch.zeros(Cout, device=dev)
 gz = torch.randn((1,) + shape + (Cout,), device=dev).to(torch.bfloat16)
 for _ in range(3):
-    fwd(xa, xb, wpk, NP, b, Cout, 3, up=up, slope=0.2)
+    tc.conv_fwd_t(xa, xb, wpk, cp, b, Cout, 3, up=up, slope=0.2)
     tc.conv_wgrad(xa, xb, gz, Ca + Cb, Cout, 3, up=up)
 torch.cuda.synchronize()

@@ -2,8 +2,9 @@
 import sys, os, statistics, json
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
-from voxelmorph_b200 import tc
+from voxelmorph_b200 import _lib, tc
 
+lib = _lib.load()
 dev = torch.device("cuda:0")
 FULL = (160, 192, 224)
 
@@ -34,7 +35,7 @@ def layer(name, shape, Ca, Cb, up, Cout):
     gz = torch.randn((1,) + shape + (max(8, Cout),), device=dev).to(torch.bfloat16)
     tw = timeit(lambda: tc.conv_wgrad(xa, xb, gz, Ca + Cb, Cout, 3, up=up))
     tt = ts = None
-    if tc.use_t_kernel(Ca, Cb, Cout):
+    if lib.vxm_conv3d_tct_supported(Ca, Cb, Cout) and lib.vxm_conv3d_tcs_supported(Ca, Cb, Cout):
         wt, cp = tc.pack_weights_t(w, variant="t")
         tt = timeit(lambda: tc.conv_fwd_t(xa, xb, wt, cp, b, Cout, 3, up=up, slope=0.2))
         ws_, cps = tc.pack_weights_t(w, variant="s")

@@ -1,6 +1,6 @@
 // Conv3d k=3 s=1 p=1 as an implicit GEMM on the Hopper tensor cores (wgmma.mma_async, accumulators in registers) —
 // the one-MMA-per-tap engine behind reference voxelmorph/torch/networks.py:299-304 (ConvBlock) and :211,257 (flow head),
-// kept as the tested baseline of the kw-stacked kernels (VXM_B200_TC_KERNEL=n).  Forward and dgrad share this kernel
+// kept as the tested baseline of the kw-stacked kernels (tc.conv_fwd).  Forward and dgrad share this kernel
 // (dgrad = same convolution with swapped channel roles and flipped taps, see vxm_conv3d_tc_pack).
 //
 // Formulation (per output d-slice of a 16 x 8 (h x w) tile):

@@ -20,159 +20,165 @@ def bump_weights_epoch():
     _weights_epoch += 1
 
 
-class _PackCache:
-    """Packed (bf16, MMA-ordered) copies of the convolution weights.  The copies live ON the parameter object
-    (attribute `_vxm_packs`), so they die with it: a table keyed by id()/data_ptr would hand a new model the packed
-    weights of a freed one whenever Python and the caching allocator both reuse the address."""
-
-    def get(self, w, key, fn):
-        packs = getattr(w, "_vxm_packs", None)
-        if packs is None:
-            packs = {}
-            w._vxm_packs = packs
-        stamp = (w.data_ptr(), w._version, _weights_epoch, tuple(w.shape), tc._variant())
-        hit = packs.get(key)
-        if hit is None or hit[0] != stamp:
-            hit = (stamp, fn())
-            packs[key] = hit
-        return hit[1]
+class _Layer:
+    """One convolution of a model's plan: its parameters, its inputs (tensor ids of the walk: 0 = the images, then every
+    convolution and pooling output in execution order) and how it runs.  `fwd` / `dgrad`: the execution form of the
+    forward and of the dgrad (see _run); `fwd_x3`: the block grid of the split-precision forward."""
+    __slots__ = ("w", "bias", "slope", "role", "a", "b", "out", "up", "ca", "cb", "cin", "cout", "fwd", "fwd_x3", "dgrad", "khm",
+                 "pk_fwd", "pk_dgrad", "pk_hi", "pk_lo", "w_hi", "w_lo")
 
 
-_cache = _PackCache()
+def _refuse(what):
+    raise _lib.VxmError("bf16 tensor-core engine: %s (use VXM_B200_CONV_ENGINE=f32 for other U-Net shapes)" % what)
 
 
-class _PackPlan:
-    """Every packed operand of a model (forward + transposed copy of each convolution, swizzled kw-stacked format) refreshed
-    by ONE kernel launch (tc.vxm_conv3d_tcs_pack_multi) instead of one launch per operand (23 per training step)."""
-
-    def __init__(self, model):
-        import ctypes
-        lib = _lib.load()
-        unet = model.unet_model
-        convs = [b.main for lvl in unet.encoder for b in lvl] + [b.main for lvl in unet.decoder for b in lvl] + \
-                [b.main for b in unet.remaining] + [model.flow]
-        self.params = [c.weight for c in convs]
-        dev = self.params[0].device
-        dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-        host = ctypes.create_string_buffer(dsz * (16 * len(convs) + 2))      # <= 2 K x 4 N blocks per operand
-        self.table = {}
-        self.keep = []
-        n, begin = 0, 0
-        # kd-folded 2-D operands (tc.planar_fold_kd): forward of the first convolution, dgrad of the flow head
-        for w, transposed in ((self.params[0], False), (self.params[-1], True)):
-            if w.dim() != 5 or w.shape[2] != 3:
-                continue
-            Cout, Cin = w.shape[0], w.shape[1]
-            real_in, nout = (Cout, Cin) if transposed else (Cin, Cout)
-            if 3 * real_in > (16 if transposed else 8) or nout not in (8, 16, 32):
-                continue
-            coutp = 16 if nout <= 16 else 32
-            out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(3 * real_in, coutp, 1)) // 2, dtype=torch.bfloat16, device=dev)
-            cnt = lib.vxm_conv3d_tcs_pack_desc_fold(ctypes.cast(ctypes.addressof(host) + n * dsz, ctypes.c_void_p), _lib.ptr(w), _lib.ptr(out),
-                                                    Cout, Cin, coutp, 1 if transposed else 0, begin)
-            if cnt <= 0:
-                continue
-            self.table[(id(w), transposed, "fold")] = (out, (coutp, "s"))
-            self.keep.append(out)
-            begin += cnt
-            n += 1
-        for li, w in enumerate(self.params):
-            w5 = w if w.dim() == 5 else w.unsqueeze(2)
-            Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
-            # a concatenating layer (decoder, after an upsample) reads the previous layer's output first, then the skip
-            ca = self.params[li - 1].shape[0] if li and Cin > self.params[li - 1].shape[0] else Cin
-            for transposed in (False, True):
-                if transposed and li == 0:
-                    continue                      # the images need no gradient: no dgrad of the first layer
-                cin_eff, nout = (Cout, Cin) if transposed else (Cin, Cout)
-                if li and Cout <= 64 and ca <= 64 and Cin - ca <= 64:
-                    blocks = tc.conv_blocks(Cout, 0, Cin, int(kd), ca if ca < Cin else None) if transposed else \
-                        tc.conv_blocks(ca, Cin - ca, Cout, int(kd))
-                    if blocks is not None:        # channel-blocked layer: one operand per (K block, N block)
-                        packs, n, begin = tc.block_descs(w, transposed, blocks, host, n, begin, dsz)
-                        self.table[(id(w), transposed, "blk")] = (blocks, packs)
-                        self.keep.extend(p[0] for p in packs.values())
-                        continue
-                if nout > 64 or cin_eff > 64:
-                    continue
-                coutp = 16 if nout <= 16 else (32 if nout <= 32 else (48 if nout <= 48 else 64))
-                nbytes = int(lib.vxm_conv3d_tcs_packed_bytes(cin_eff, coutp, kd))
-                out = torch.empty(nbytes // 2, dtype=torch.bfloat16, device=dev)
-                cnt = lib.vxm_conv3d_tcs_pack_desc(ctypes.cast(ctypes.addressof(host) + n * dsz, ctypes.c_void_p), _lib.ptr(w), _lib.ptr(out),
-                                                   Cout, Cin, kd, coutp, 1 if transposed else 0, begin)
-                if cnt <= 0:
-                    continue
-                self.table[(id(w), transposed)] = (out, (coutp, "s"))
-                self.keep.append(out)
-                begin += cnt
-                n += 1
-        self.ndesc, self.total = n, begin
-        self.descs = torch.frombuffer(bytearray(host.raw[:max(1, n) * dsz]), dtype=torch.uint8).to(dev)
-        self.ptrs = tuple(w.data_ptr() for w in self.params)
-        self.stamp = None
-
-    def valid_for(self, model):
-        return self.ptrs == tuple(w.data_ptr() for w in self.params)
-
-    def refresh(self):
-        stamp = (_weights_epoch, tuple(w._version for w in self.params))
-        if stamp != self.stamp and self.ndesc:
-            _lib.check(_lib.load().vxm_conv3d_tcs_pack_multi(_lib.ptr(self.descs), self.ndesc, self.total, _lib.stream_ptr()),
-                       "vxm_conv3d_tcs_pack_multi")
-            self.stamp = stamp
-
-    def lookup(self, w, transposed):
-        return self.table.get((id(w), transposed))
-
-    def lookup_blocks(self, w, transposed, blocks):
-        """Block operands of `w` packed for `blocks` (tc.conv_blocks), or None."""
-        hit = self.table.get((id(w), transposed, "blk"))
-        return hit[1] if hit is not None and hit[0] == blocks else None
-
-    def lookup_fold(self, w, transposed):
-        return self.table.get((id(w), transposed, "fold"))
+def _form(ca, cb, nout, kd, kw, split=None):
+    """Execution form of a convolution on the swizzled kw-stacked kernel: its channel blocks (tc.conv_blocks), or the 1 x 1
+    grid of one launch (kw: input channels of the weight operand).  Refuses a shape one of whose launches the kernel lacks."""
+    blocks = tc.conv_blocks(ca, cb, nout, kd, split)
+    launches = [(ca, cb, nout)] if blocks is None else \
+        [((ca, cb) if src == 2 else (kb, 0)) + (nb,) for src, _, kb in blocks[0] for _, nb, _, _ in blocks[1]]
+    for c0, c1, n in launches:
+        if not _lib.load().vxm_conv3d_tcs_supported(c0, c1, n):
+            _refuse("no tensor-core kernel takes a (%d + %d) -> %d convolution" % (c0, c1, n))
+    return blocks if blocks is not None else tc.one_block(kw, nout)
 
 
-def _plan_of(model):
-    """The model's pack plan (built lazily; rebuilt when the parameters moved, e.g. after .to(device) or FlatParams)."""
-    if tc._variant() not in ("auto", "s"):
-        return None
-    plan = model.__dict__.get("_vxm_pack_plan")
-    if plan is None or not plan.valid_for(model):
-        plan = _PackPlan(model)
-        object.__setattr__(model, "_vxm_pack_plan", plan)
-    plan.refresh()
-    return plan
+def _walk(model):
+    """The U-Net and flow head of `model` (a VxmDense) in execution order: _Layer and ("pool", in_id, out_id) entries with
+    shapes and execution forms only (allocates nothing).  Refuses a model some convolution of which no engine path runs."""
+    unet = model.unet_model
+    w0 = unet.encoder[0][0].main.weight
+    if w0.dim() not in (4, 5):
+        _refuse("2-D or 3-D convolutions only")
+    kd = 3 if w0.dim() == 5 else 1
+    fold = kd == 3 and tc.kdfold_enabled()
+    ops = []
+    chans = [8]           # channels of every tensor id: the images enter as one bf16 channels-last tensor of 8 channels
+    cur, pending_up, skips = 0, None, [None]
+
+    def conv(m, slope, role="inner"):
+        nonlocal cur, pending_up
+        L = _Layer()
+        L.w, L.bias, L.slope, L.role = m.weight, m.bias, slope, role
+        # a convolution after an upsample reads the upsampled previous output, then the skip (a fused upsample + concat)
+        L.a, L.b = pending_up if pending_up is not None else (cur, None)
+        L.up, pending_up = pending_up is not None, None
+        L.ca, L.cb = chans[L.a], (0 if L.b is None else chans[L.b])
+        L.cout, L.cin = m.weight.shape[0], m.weight.shape[1]
+        if m.weight.dim() != w0.dim():
+            _refuse("convolutions of different dimensionality")
+        if role == "first":
+            if L.cin > 8:
+                _refuse("the first convolution takes at most 8 input feature planes (src_feats + trg_feats)")
+        elif L.ca + L.cb != L.cin or L.cin % 16 or L.cin > (64 if role == "flow" else 128):
+            _refuse("unsupported convolution input channels %d (+%d); need a multiple of 16, at most 128 (64 into the flow "
+                    "head)" % (L.ca, L.cb))
+        if role == "flow" and L.cout > 8:
+            _refuse("the flow head has %d components" % L.cout)
+        if role != "flow" and L.cout not in (8, 16, 32, 64):
+            _refuse("a U-Net convolution has %d output channels; supported feature counts are 8, 16, 32 and 64" % L.cout)
+        L.fwd = L.fwd_x3 = _form(L.ca, L.cb, L.cout, kd, L.cin)
+        # kd folded into the channels of the layers with 2 / 3 real channels on one side (3 instead of 9 MMA steps per
+        # tile): the forward of the first convolution (bf16), the dgrad of the flow head
+        if role == "first" and fold and 3 * L.cin <= 8 and L.cout in (8, 16, 32):
+            L.fwd = "fold"
+        if role == "first":
+            L.dgrad = None                # the images need no gradient
+        elif role == "flow" and fold and L.b is None and L.cin in (8, 16) and 3 * L.cout <= 16:
+            L.dgrad = "fold"
+        else:                             # the flow gradient enters as 8 channels; a concatenation's dgrad splits its output
+            L.dgrad = _form(8 if role == "flow" else L.cout, 0, L.cin, kd, L.cout, L.ca if L.b is not None else None)
+        L.khm = L.cout <= 16              # weight gradient of the folded first layer: kh-in-M takes at most 16 outputs
+        L.out = cur = len(chans)
+        chans.append(L.cout)
+        ops.append(L)
+
+    def pool():
+        nonlocal cur
+        ops.append(("pool", cur, len(chans)))
+        cur = len(chans)
+        chans.append(chans[ops[-1][1]])
+
+    for convs in unet.encoder:
+        for blk in convs:
+            conv(blk.main, blk.activation.negative_slope, "first" if cur == 0 else "inner")
+        skips.append(cur)
+        pool()
+    for level, convs in enumerate(unet.decoder):
+        for blk in convs:
+            conv(blk.main, blk.activation.negative_slope)
+        if not unet.half_res or level < (unet.nb_levels - 2):
+            pending_up = (cur, skips.pop())
+    for blk in unet.remaining:
+        conv(blk.main, blk.activation.negative_slope)
+    conv(model.flow, None, "flow")        # no activation, fp32 planar output
+    return ops
 
 
 def supports(model):
-    """True when every convolution of `model` (a VxmDense) runs in one launch per layer on the tensor-core kernels: feature
-    counts in {8, 16, 32}, concatenated inputs a multiple of 16 and at most 64 channels, at most 8 image planes.  This is
-    what VXM_B200_CONV_ENGINE=tc selects the tensor cores for; VXM_B200_CONV_ENGINE=bf16 | bf16x3 also run U-Nets with
-    64-channel layers and concatenations of up to 128 channels, in channel blocks (tc.conv_blocks)."""
+    """True when the tensor-core engine runs every convolution of `model` (a VxmDense) in one launch per layer with feature
+    counts in {8, 16, 32} and inputs of at most 64 channels: what VXM_B200_CONV_ENGINE=tc selects the tensor cores for.
+    VXM_B200_CONV_ENGINE=bf16 | bf16x3 run every model _walk accepts, U-Nets with 64-channel layers and concatenations of
+    up to 128 channels included (in channel blocks)."""
     try:
-        unet = model.unet_model
-        convs = [b.main for lvl in unet.encoder for b in lvl] + [b.main for lvl in unet.decoder for b in lvl] + \
-                [b.main for b in unet.remaining]
-        first = convs[0]
-        if first.weight.shape[1] > 8 or first.weight.dim() not in (4, 5):
-            return False
-        for i, c in enumerate(convs):
-            co, ci = c.weight.shape[0], c.weight.shape[1]
-            if co not in (8, 16, 32):
-                return False
-            if i > 0 and (ci % 16 or ci > 64):
-                return False
-        fl = model.flow
-        return fl.weight.shape[1] % 16 == 0 and fl.weight.shape[1] <= 64 and fl.weight.shape[0] <= 8
-    except AttributeError:
+        ops = _walk(model)
+    except (AttributeError, _lib.VxmError):
         return False
+    return all(L.role == "flow" or (L.cout in (8, 16, 32) and L.ca + L.cb <= 64) for L in ops if isinstance(L, _Layer))
 
 
-def _check_cout(c, what):
-    if c not in (8, 16, 32, 64):
-        raise _lib.VxmError("bf16 tensor-core engine: %s has %d channels; supported feature counts are 8, 16, 32 and 64 "
-                            "(use VXM_B200_CONV_ENGINE=f32 for other U-Net shapes)" % (what, c))
+class _Plan:
+    """A model's walk (_walk) with every packed operand it runs on.  The bf16 operands (forward and transposed copy of
+    every convolution: whole, in channel blocks or kd-folded) are refreshed by ONE pack launch per step.  The bf16x3
+    forward operands, the bf16 hi and lo parts of every weight in the block grid of tc.conv_fwd_blocked, are packed from
+    persistent fp32 buffers by one more launch, so that their refresh stays graph-capturable."""
+
+    def __init__(self, model):
+        self.ops = _walk(model)
+        self.layers = [L for L in self.ops if isinstance(L, _Layer)]
+        self.nd = self.layers[0].w.dim() - 2
+        self.slope = {L.out: float(L.slope) for L in self.layers if L.slope is not None}     # convolution output id -> slope
+        bf16, x3 = [], []
+        for L in self.layers:
+            w = L.w.detach()
+            L.w_hi, L.w_lo = torch.empty_like(w), torch.empty_like(w)
+            bf16 += [(w, False, L.fwd)] + ([(w, True, L.dgrad)] if L.dgrad is not None else [])
+            x3 += [(L.w_hi, False, L.fwd_x3), (L.w_lo, False, L.fwd_x3)]
+        self.bf16, self.x3 = tc.PackTable(bf16), tc.PackTable(x3)
+        packs, packs3 = iter(self.bf16.packs), iter(self.x3.packs)
+        for L in self.layers:
+            L.pk_fwd, L.pk_dgrad = next(packs), (next(packs) if L.dgrad is not None else None)
+            L.pk_hi, L.pk_lo = next(packs3), next(packs3)
+        self.ptrs = self.weight_ptrs()
+        self.stamps = [None, None]
+
+    def weight_ptrs(self):
+        return tuple(L.w.data_ptr() for L in self.layers)
+
+    def refresh(self, split):
+        stamp = (_weights_epoch, tuple(L.w._version for L in self.layers))
+        if stamp != self.stamps[0]:
+            self.bf16.refresh()
+            self.stamps[0] = stamp
+        if split and stamp != self.stamps[1]:
+            for L in self.layers:         # hi = bf16(w), lo = w - hi
+                w = L.w.detach()
+                L.w_hi.copy_(w.to(torch.bfloat16))
+                torch.sub(w, L.w_hi, out=L.w_lo)
+            self.x3.refresh()
+            self.stamps[1] = stamp
+
+
+def _plan_of(model, split):
+    """The model's plan with its operands refreshed (built lazily; rebuilt when the parameters moved, e.g. after
+    .to(device) or FlatParams)."""
+    plan = model.__dict__.get("_vxm_pack_plan")
+    if plan is None or plan.ptrs != plan.weight_ptrs():
+        plan = _Plan(model)
+        object.__setattr__(model, "_vxm_pack_plan", plan)
+    plan.refresh(split)
+    return plan
 
 
 def _pool(x, nd):
@@ -205,310 +211,147 @@ def _unpool_combine(e_fine, g_skip, g_pool, nd, slope):
     return out
 
 
-class _Conv:
-    """One convolution of the tape: inputs, output, parameters."""
-    __slots__ = ("w", "b", "planar", "xa", "xb", "up", "out", "slope", "cin", "cout", "a_id", "b_id", "out_id", "planar_out",
-                 "xa_lo", "xb_lo", "fold")
+def _run(form, packs, xa, xb, nout, kd, bias=None, lo=None, **kw):
+    """The engine's one kernel selection: runs a convolution of the plan (a forward, or a dgrad on the transposed operand) in
+    its execution form.  "fold": one 2-D launch over kd-folded channels; a 1 x 1 grid: one launch of the swizzled
+    kw-stacked kernel (tc.conv_fwd_t); channel blocks, and every split-precision forward (lo): tc.conv_fwd_blocked."""
+    if form == "fold" or (lo is None and len(form[0]) == len(form[1]) == 1):
+        wpk, coutp = packs[0, 0]
+        return tc.conv_fwd_t(xa, xb, wpk, (coutp, "s"), bias, nout, 1 if form == "fold" else kd, **kw)
+    return tc.conv_fwd_blocked(xa, xb, form, packs, bias, nout, kd, lo=lo, **kw)
 
 
-def _run_conv_split(cv, kd):
-    """Forward of one tape entry in split precision (three tensor-core passes, see tc.conv_fwd_split).  Returns the
-    (hi, lo) output pair, or the fp32 planar flow."""
-    def packs():
-        wh, wl = tc.split_weights(cv.w)
-        return tc.pack_weights_t(wh, variant="s"), tc.pack_weights_t(wl, variant="s")
-    blocks = None if cv.planar_out else tc.conv_blocks(_width(cv.xa), _width(cv.xb), cv.cout, kd)
-    if blocks is not None:
-        def block_packs():
-            sp = getattr(cv.w, "_vxm_split_blocks", None)       # persistent buffers: the refresh stays graph-capturable
-            if sp is None or sp.blocks != blocks:
-                sp = tc.SplitBlockPacks(cv.w, blocks)
-                cv.w._vxm_split_blocks = sp
-            return sp.refresh(cv.w)
-        sp = _cache.get(cv.w, "fwd_split_blk", block_packs)
-        return tc.conv_fwd_blocked(cv.xa, cv.xb, blocks, sp.hi, cv.b.detach() if cv.b is not None else None, cv.cout, kd, up=cv.up,
-                                   slope=cv.slope, lo=(cv.xa_lo, cv.xb_lo, sp.lo))
-    pk = _cache.get(cv.w, "fwd_split", packs)
-    xa = None if cv.xa is None else (cv.xa, cv.xa_lo)
-    xb = None if cv.xb is None else (cv.xb, cv.xb_lo)
-    return tc.conv_fwd_split(xa, xb, pk, cv.b.detach() if cv.b is not None else None, cv.cout, kd, up=cv.up,
-                             out_fp32_planar=cv.planar_out, slope=cv.slope)
-
-
-def _width(x):
-    return 0 if x is None else x.shape[-1]
-
-
-def _block_packs(plan, cv, transposed, blocks):
-    packs = plan.lookup_blocks(cv.w, transposed, blocks) if plan is not None else None
-    if packs is None:
-        raise _lib.VxmError("bf16 engine: the %d -> %d convolution runs in channel blocks, which need the swizzled kw-stacked "
-                            "kernel (VXM_B200_TC_KERNEL=auto|s)" % (cv.cin, cv.cout))
-    return packs
-
-
-def _run_conv(cv, kd, plan=None):
-    """Forward of one tape entry."""
-    ca = 0 if cv.xa is None else cv.xa.shape[-1]
-    cb = 0 if cv.xb is None else cv.xb.shape[-1]
-    blocks = None if (cv.planar is not None or cv.fold == "x" or cv.planar_out) else tc.conv_blocks(ca, cb, cv.cout, kd)
-    if blocks is not None:
-        return tc.conv_fwd_blocked(cv.xa, cv.xb, blocks, _block_packs(plan, cv, False, blocks), cv.b.detach() if cv.b is not None else None,
-                                   cv.cout, kd, up=cv.up, slope=cv.slope)
-    if cv.fold == "x":
-        # kd folded into the input channels: a 2-D convolution per slice (3 instead of 9 MMA steps per tile)
-        wpk, cp = plan.lookup_fold(cv.w, False)
-        return tc.conv_fwd_t(cv.xa, None, wpk, cp, cv.b.detach() if cv.b is not None else None, cv.cout, 1, slope=cv.slope)
-    if cv.planar is None and tc.use_t_kernel(ca, cb, cv.cout):
-        hit = plan.lookup(cv.w, False) if (plan is not None and tc._use_s(ca, cb, cv.cout)) else None
-        wpk, cp = hit if hit is not None else _cache.get(cv.w, "fwd_t", lambda: tc.pack_weights_t(cv.w.detach()))
-        return tc.conv_fwd_t(cv.xa, cv.xb, wpk, cp, cv.b.detach() if cv.b is not None else None, cv.cout, kd, up=cv.up,
-                             out_fp32_planar=cv.planar_out, slope=cv.slope)
-    wpk, NP = _cache.get(cv.w, "fwd", lambda: tc.pack_weights(cv.w.detach()))
-    return tc.conv_fwd(cv.xa, cv.xb, wpk, NP, cv.b.detach() if cv.b is not None else None, cv.cout, kd, up=cv.up, planar=cv.planar,
-                       out_fp32_planar=cv.planar_out, slope=cv.slope)
+def _flat_grads(L):
+    """True when every parameter of L has a contiguous .grad view of FusedAdam's flat gradient buffer (optim.FlatParams
+    marks them): the weight gradients are then accumulated into it directly, and autograd receives none for them."""
+    return all(getattr(p, "_vxm_flat_grad", False) and p.grad is not None and p.grad.is_contiguous()
+               for p in (L.w, L.bias) if p is not None)
 
 
 def forward_tape(model, source, target, split=False):
     """Runs Unet + flow head, returns (flow fp32 (B,nd,*vol), tape).  `split`: split-precision (bf16x3) forward — every
     activation is a (hi, lo) bf16 pair and every layer three tensor-core passes; the tape keeps the hi parts, which is
     what the (bf16-operand) backward reads."""
-    unet = model.unet_model
     nd = source.dim() - 2
     kd = 3 if nd == 3 else 1
     _lib.require_cuda(source, target, what="VxmDense")
     source, target = _lib.contig(source), _lib.contig(target)
+    plan = _plan_of(model, split)
     planes = [source[:, i:i + 1] for i in range(source.shape[1])] + [target[:, i:i + 1] for i in range(target.shape[1])]
-    if len(planes) > 8:
-        raise _lib.VxmError("bf16 engine: at most 8 input feature planes (src_feats + trg_feats)")
-    tape = []            # list of ("conv", _Conv) / ("pool", in_id, out_id)
-    tensors = {}         # id -> bf16 NDHWC tensor
-    lows = {}            # id -> lo part (split precision only)
-    plan = None if split else _plan_of(model)
-    producer = {}        # id -> "conv" | "pool"
-    next_id = [0]
-
-    def new_id():
-        next_id[0] += 1
-        return next_id[0]
-
-    def conv(block_main, slope, planar=None, a_id=None, b_id=None, up=False, planar_out=False):
-        cv = _Conv()
-        cv.w, cv.b = block_main.weight, block_main.bias
-        cv.planar = planar
-        cv.xa = tensors[a_id] if a_id is not None else None
-        cv.xb = tensors[b_id] if b_id is not None else None
-        cv.up, cv.slope, cv.planar_out = up, slope, planar_out
-        cv.cout, cv.cin = cv.w.shape[0], cv.w.shape[1]
-        cv.a_id, cv.b_id = a_id, b_id
-        cv.xa_lo = lows.get(a_id) if split else None
-        cv.xb_lo = lows.get(b_id) if split else None
-        cv.fold = "x" if (a_id is not None and producer.get(a_id) == "input" and fold_first) else None
-        if not planar_out:
-            _check_cout(cv.cout, "a U-Net convolution output")
-        if planar is None:
-            ca = 0 if cv.xa is None else cv.xa.shape[-1]
-            cb = 0 if cv.xb is None else cv.xb.shape[-1]
-            first_layer = cv.xa is not None and producer.get(a_id) == "input"
-            if first_layer:
-                if ca != 8 or cb or cv.cin > 8 or (cv.fold == "x" and 3 * cv.cin > 8):
-                    raise _lib.VxmError("bf16 engine: the first convolution takes at most 8 input feature planes")
-            elif ca + cb != cv.cin or (ca + cb) % 16 or ca + cb > (64 if planar_out else 128):
-                raise _lib.VxmError("bf16 engine: unsupported convolution input channels %d (+%d); need a multiple of 16, at most 128 "
-                                    "(64 into the flow head) (use VXM_B200_CONV_ENGINE=f32 for other U-Net shapes)" % (ca, cb))
-        out = _run_conv_split(cv, kd) if split else _run_conv(cv, kd, plan)
-        cv.out_id = new_id()
-        if split and not planar_out:
-            out, lows[cv.out_id] = out
-        cv.out = out
-        cv.xa_lo = cv.xb_lo = None      # the backward reads the hi parts only
-        if not planar_out:
-            tensors[cv.out_id] = out
-            producer[cv.out_id] = "conv"
-        tape.append(("conv", cv))
-        return cv.out_id
-
-    def pool(in_id):
-        oid = new_id()
-        if split:
-            y, lows[oid] = tc.pool_split((tensors[in_id], lows[in_id]), nd)
-        else:
-            y = _pool(tensors[in_id], nd)
-        return _pool_done(y, in_id, oid)
-
-    def _pool_done(y, in_id, oid):
-        tensors[oid] = y
-        producer[oid] = "pool"
-        tape.append(("pool", in_id, oid))
-        return oid
-
-    # the fp32 images enter as one bf16 channels-last tensor with 8 channels (src planes, trg planes, zeros)
-    cur = new_id()
-    first_w = unet.encoder[0][0].main.weight
-    fold_first = (not split and nd == 3 and tc.kdfold_enabled() and plan is not None and plan.lookup_fold(first_w, False) is not None
-                  and first_w.shape[1] == len(planes) and tc._variant() in ("auto", "s"))
+    first = plan.layers[0]
+    if nd != plan.nd or len(planes) != first.cin:
+        raise _lib.VxmError("bf16 engine: the model takes %d %d-D image planes (src_feats + trg_feats), got %d %d-D"
+                            % (first.cin, plan.nd, len(planes), nd))
+    tensors = {}         # tensor id -> bf16 NDHWC tensor
+    lows = {}            # tensor id -> lo part (split precision only)
     if split:
-        tensors[cur], lows[cur] = tc.planar_to_ndhwc8_split(planes)
-    elif fold_first:
-        tensors[cur] = tc.planar_fold_kd(planes, 8)      # (kd, plane) channels: the first convolution runs as 2-D
+        tensors[0], lows[0] = tc.planar_to_ndhwc8_split(planes)
+    elif first.fwd == "fold":
+        tensors[0] = tc.planar_fold_kd(planes, 8)      # (kd, plane) channels: the first convolution runs as 2-D
     else:
-        tensors[cur] = tc.planar_to_ndhwc8(planes)
-    producer[cur] = "input"
-    skips = [None]
-    for level, convs in enumerate(unet.encoder):
-        for blk in convs:
-            slope = blk.activation.negative_slope
-            cur = conv(blk.main, slope, a_id=cur)
-        skips.append(cur)
-        cur = pool(cur)
-    pending_up = None    # (a_id, skip_id) to be consumed by the next convolution as a fused upsample+concat
-    for level, convs in enumerate(unet.decoder):
-        for blk in convs:
-            slope = blk.activation.negative_slope
-            if pending_up is not None:
-                cur = conv(blk.main, slope, a_id=pending_up[0], b_id=pending_up[1], up=True)
-                pending_up = None
+        tensors[0] = tc.planar_to_ndhwc8(planes)
+    for L in plan.ops:
+        if not isinstance(L, _Layer):
+            _, src, dst = L
+            if split:
+                tensors[dst], lows[dst] = tc.pool_split((tensors[src], lows[src]), nd)
             else:
-                cur = conv(blk.main, slope, a_id=cur)
-        if not unet.half_res or level < (unet.nb_levels - 2):
-            pending_up = (cur, skips.pop())
-    for blk in unet.remaining:
-        slope = blk.activation.negative_slope
-        if pending_up is not None:
-            cur = conv(blk.main, slope, a_id=pending_up[0], b_id=pending_up[1], up=True)
-            pending_up = None
+                tensors[dst] = _pool(tensors[src], nd)
+            continue
+        bias = None if L.bias is None else L.bias.detach()
+        kw = dict(up=L.up, slope=L.slope, out_fp32_planar=L.role == "flow")
+        if split:
+            out = _run(L.fwd_x3, L.pk_hi, tensors[L.a], tensors.get(L.b), L.cout, kd, bias, lo=(lows[L.a], lows.get(L.b), L.pk_lo), **kw)
         else:
-            cur = conv(blk.main, slope, a_id=cur)
-    # flow head (no activation, fp32 planar output)
-    if pending_up is not None:
-        fid = conv(model.flow, None, a_id=pending_up[0], b_id=pending_up[1], up=True, planar_out=True)
-    else:
-        fid = conv(model.flow, None, a_id=cur, planar_out=True)
-    flow = tape[-1][1].out
+            out = _run(L.fwd, L.pk_fwd, tensors[L.a], tensors.get(L.b), L.cout, kd, bias, **kw)
+        if L.role == "flow":
+            flow = out
+        elif split:
+            tensors[L.out], lows[L.out] = out
+        else:
+            tensors[L.out] = out
     if nd == 2:
         flow = flow.squeeze(2)
-    return flow, dict(tape=tape, tensors=tensors, producer=producer, nd=nd, kd=kd, plan=_plan_of(model) if split else plan)
+    return flow, dict(plan=plan, tensors=tensors, split=split)
 
 
 def backward_tape(ctx, g_flow):
-    """Hand-written backward over the tape.  Returns {param: grad}."""
-    lib = _lib.load()
-    tape, tensors, producer, nd, kd = ctx["tape"], ctx["tensors"], ctx["producer"], ctx["nd"], ctx["kd"]
-    plan = ctx.get("plan")
+    """Hand-written backward over the plan.  Returns {param: grad}."""
+    plan, tensors = ctx["plan"], ctx["tensors"]
+    nd = plan.nd
+    kd = 3 if nd == 3 else 1
     g_flow = _lib.contig(g_flow.float())
     if nd == 2:
         g_flow = g_flow.unsqueeze(2)
-    batch = tc.WgradBatch.get(g_flow.device)
+    dev = g_flow.device
+    batch = tc.WgradBatch.get(dev)
     batch.reset()
     gz = {}       # conv-output id -> masked gradient (bf16 NDHWC)
     graw = {}     # pool-output id -> raw gradient
     gskip = {}    # encoder-output id -> raw skip gradient
     grads = {}
-    dev = g_flow.device
-    folded = []   # (conv, gw2d, gb2d, kind): 2-D weight gradients of the kd-folded layers, mapped back after the flush
-    for entry in reversed(tape):
-        if entry[0] == "pool":
-            _, in_id, out_id = entry
-            e = tensors[in_id]
-            gz[in_id] = _unpool_combine(e, gskip.pop(in_id, None), graw.pop(out_id), nd, _slope_of(ctx, in_id))
+    folded = []   # (layer, gw2d, gb2d): 2-D weight gradients of the kd-folded layers, mapped back after the flush
+    for L in reversed(plan.ops):
+        if not isinstance(L, _Layer):
+            _, src, dst = L
+            gz[src] = _unpool_combine(tensors[src], gskip.pop(src, None), graw.pop(dst), nd, plan.slope[src])
             continue
-        cv = entry[1]
-        fold_g = (cv.planar_out and nd == 3 and tc.kdfold_enabled() and plan is not None and plan.lookup_fold(cv.w, True) is not None
-                  and cv.xb is None and not cv.up and cv.xa is not None and cv.xa.shape[-1] in (8, 16) and cv.xa.shape[-1] == cv.cin
-                  and producer.get(cv.a_id) == "conv" and tc._variant() in ("auto", "s"))
-        if fold_g:
-            # flow head, kd folded into the channels of the flow gradient: (kd', component) = 9 of 16 channels
-            g_in = tc.planar_fold_kd([g_flow[:, i:i + 1] for i in range(g_flow.shape[1])], 16)
-            gwf = torch.empty((3 * nd, cv.cin, 1, 3, 3), dtype=torch.float32, device=dev)
-            gbf = torch.empty(3 * nd, dtype=torch.float32, device=dev) if cv.b is not None else None
-            batch.add_khm(cv.xa, g_in, gwf, gbf, cv.cin, 3 * nd)
-            folded.append((cv, gwf, gbf, "g"))
-            t = cv.a_id
-            wpk, cp = plan.lookup_fold(cv.w, True)
-            gz[t] = tc.conv_fwd_t(g_in, None, wpk, cp, None, cv.cin, 1, slope=_slope_of(ctx, t), mask=tensors[t])
-            continue
-        if cv.planar_out:
-            # flow head: the fp32 planar flow gradient becomes an 8-channel bf16 channels-last tensor
-            g_in = tc.planar_to_ndhwc8([g_flow[:, i:i + 1] for i in range(g_flow.shape[1])])
+        xa, xb = tensors[L.a], tensors.get(L.b)
+        if L.role == "flow":
+            # the fp32 planar flow gradient becomes a bf16 channels-last tensor: 8 channels, or kd-folded (kd', component) =
+            # 9 of 16 channels
+            planes = [g_flow[:, i:i + 1] for i in range(g_flow.shape[1])]
+            g_in = tc.planar_fold_kd(planes, 16) if L.dgrad == "fold" else tc.planar_to_ndhwc8(planes)
         else:
-            g_in = gz.pop(cv.out_id)
-        if cv.fold == "x":
-            # first layer over the kd-folded images: 2-D weight gradient with kh in M, no dgrad
-            gwf = torch.empty((cv.cout, 3 * cv.cin, 1, 3, 3), dtype=torch.float32, device=dev)
-            gbf = torch.empty(cv.cout, dtype=torch.float32, device=dev) if cv.b is not None else None
-            if g_in.shape[-1] <= 16:
-                batch.add_khm(cv.xa, g_in, gwf, gbf, 3 * cv.cin, cv.cout)
-            else:      # kh-in-M takes at most 16 output channels: a wider first layer runs the plain 2-D kernel
-                batch.add(cv.xa, None, g_in, gwf, gbf, 3 * cv.cin, cv.cout, 1, False, False)
-            folded.append((cv, gwf, gbf, "x"))
-            continue
-        # parameters whose .grad is a view of FusedAdam's flat gradient buffer (optim.FlatParams marks them)
-        # are accumulated into directly by the reduce kernel; autograd then receives no gradient for them
-        direct = (getattr(cv.w, "_vxm_flat_grad", False) and cv.w.grad is not None and cv.w.grad.is_contiguous()
-                  and (cv.b is None or (getattr(cv.b, "_vxm_flat_grad", False) and cv.b.grad is not None)))
-        if direct:
-            tc.conv_wgrad(cv.xa, cv.xb, g_in, cv.cin, cv.cout, kd, up=cv.up, planar_x=cv.planar,
-                          out_w=cv.w.grad, out_b=None if cv.b is None else cv.b.grad, batch=batch)
+            g_in = gz.pop(L.out)
+        # ---- weight gradient ----
+        if L.dgrad == "fold":
+            gwf = torch.empty((3 * nd, L.cin, 1, 3, 3), dtype=torch.float32, device=dev)
+            gbf = torch.empty(3 * nd, dtype=torch.float32, device=dev) if L.bias is not None else None
+            batch.add_khm(xa, g_in, gwf, gbf, L.cin, 3 * nd)
+            folded.append((L, gwf, gbf))
+        elif L.fwd == "fold" and not ctx["split"]:
+            # first layer over the kd-folded images: a 2-D weight gradient
+            gwf = torch.empty((L.cout, 3 * L.cin, 1, 3, 3), dtype=torch.float32, device=dev)
+            gbf = torch.empty(L.cout, dtype=torch.float32, device=dev) if L.bias is not None else None
+            if L.khm:
+                batch.add_khm(xa, g_in, gwf, gbf, 3 * L.cin, L.cout)
+            else:
+                batch.add(xa, None, g_in, gwf, gbf, 3 * L.cin, L.cout, 1, False, False)
+            folded.append((L, gwf, gbf))
+        elif _flat_grads(L):
+            tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, out_w=L.w.grad, out_b=None if L.bias is None else L.bias.grad,
+                          batch=batch)
         else:
-            gw, gb = tc.conv_wgrad(cv.xa, cv.xb, g_in, cv.cin, cv.cout, kd, up=cv.up, planar_x=cv.planar, batch=batch)
-            grads[cv.w] = gw.squeeze(2) if nd == 2 else gw
-            if cv.b is not None:
-                grads[cv.b] = gb
-        g_in_planar = None
+            gw, gb = tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, batch=batch)
+            grads[L.w] = gw.squeeze(2) if nd == 2 else gw
+            if L.bias is not None:
+                grads[L.bias] = gb
         # ---- dgrad ----
-        if cv.planar is not None or producer.get(cv.a_id) == "input":
-            continue       # first layer: the images need no gradient
-        w = cv.w.detach()
-        if cv.b_id is None:
-            t = cv.a_id
-            msk = tensors[t] if producer[t] == "conv" else None
-            sl = _slope_of(ctx, t) if producer[t] == "conv" else None
-            blocks = tc.conv_blocks(g_in.shape[-1], 0, cv.cin, kd)
-            if blocks is not None:
-                res = tc.conv_fwd_blocked(g_in, None, blocks, _block_packs(plan, cv, True, blocks), None, cv.cin, kd, slope=sl, mask=msk)
-            elif tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
-                hit = plan.lookup(cv.w, True) if (plan is not None and tc._use_s(g_in.shape[-1], 0, cv.cin)) else None
-                wpk, cp = hit if hit is not None else _cache.get(cv.w, "dgrad_t", lambda: tc.pack_weights_t(w, transposed=True))
-                res = tc.conv_fwd_t(g_in, None, wpk, cp, None, cv.cin, kd, slope=sl, mask=msk)
-            else:
-                wpk, NP = _cache.get(cv.w, "dgrad", lambda: tc.pack_weights(w, transposed=True))
-                res = tc.conv_fwd(g_in, None, wpk, NP, None, cv.cin, kd, planar=g_in_planar, slope=sl, mask=msk)
-            if producer[t] == "conv":
-                gz[t] = res
-            else:
-                graw[t] = res
+        if L.dgrad is None:
+            continue
+        t = L.a
+        if L.b is None:
+            sl = plan.slope.get(t)         # None: a pooling output, no activation to differentiate
+            res = _run(L.dgrad, L.pk_dgrad, g_in, None, L.cin, kd, slope=sl, mask=None if sl is None else tensors[t])
+            (graw if sl is None else gz)[t] = res
         else:
-            ca = cv.xa.shape[-1]
             # single dgrad pass over the whole concat input: N = Ca + Cb output channels, split on store
-            blocks = tc.conv_blocks(g_in.shape[-1], 0, cv.cin, kd, ca)
-            if blocks is not None:
-                g_up, g_sk = tc.conv_fwd_blocked(g_in, None, blocks, _block_packs(plan, cv, True, blocks), None, cv.cin, kd, split=ca)
-            elif tc.use_t_kernel(g_in.shape[-1], 0, cv.cin):
-                hit = plan.lookup(cv.w, True) if (plan is not None and tc._use_s(g_in.shape[-1], 0, cv.cin)) else None
-                wpk, cp = hit if hit is not None else _cache.get(cv.w, "dgrad_t", lambda: tc.pack_weights_t(w, transposed=True))
-                g_up, g_sk = tc.conv_fwd_t(g_in, None, wpk, cp, None, cv.cin, kd, split=ca)
-            else:
-                wpk, NP = _cache.get(cv.w, "dgrad", lambda: tc.pack_weights(w, transposed=True))
-                g_up, g_sk = tc.conv_fwd(g_in, None, wpk, NP, None, cv.cin, kd, planar=g_in_planar, split=ca)
-            gz[cv.a_id] = _sumpool_mask(g_up, tensors[cv.a_id], nd, _slope_of(ctx, cv.a_id))   # grad wrt upsample(a): sum children
+            g_up, g_sk = _run(L.dgrad, L.pk_dgrad, g_in, None, L.cin, kd, split=L.ca)
+            gz[t] = _sumpool_mask(g_up, tensors[t], nd, plan.slope[t])   # grad wrt upsample(a): sum children
             del g_up
-            gskip[cv.b_id] = g_sk
+            gskip[L.b] = g_sk
     batch.flush()     # one launch reduces every layer's per-CTA partials (fixed order: deterministic)
-    for cv, gwf, gbf, kind in folded:
-        if kind == "x":
-            gw, gb = unfold_grad_first(gwf, cv.cout, cv.cin), gbf
+    for L, gwf, gbf in folded:
+        gw, gb = (unfold_grad_first(gwf, L.cout, L.cin), gbf) if L.role == "first" else unfold_grad_flow(gwf, gbf, nd, L.cin)
+        if _flat_grads(L):
+            L.w.grad.add_(gw)
+            if L.bias is not None:
+                L.bias.grad.add_(gb)
         else:
-            gw, gb = unfold_grad_flow(gwf, gbf, nd, cv.cin)
-        direct = (getattr(cv.w, "_vxm_flat_grad", False) and cv.w.grad is not None
-                  and (cv.b is None or (getattr(cv.b, "_vxm_flat_grad", False) and cv.b.grad is not None)))
-        if direct:
-            cv.w.grad.add_(gw)
-            if cv.b is not None:
-                cv.b.grad.add_(gb)
-        else:
-            grads[cv.w] = gw.contiguous()
-            if cv.b is not None:
-                grads[cv.b] = gb.contiguous()
+            grads[L.w] = gw.contiguous()
+            if L.bias is not None:
+                grads[L.bias] = gb.contiguous()
     return grads
 
 
@@ -550,14 +393,6 @@ def unfold_grad_flow(gwf, gbf, nd, cin):
     the gradient at v with x at v + 1 - kd').  The bias gradient is the channel sum of the unshifted copy (kd' = 1)."""
     gw = gwf.view(3, nd, cin, 3, 3).flip(0).permute(1, 2, 0, 3, 4)
     return gw, (None if gbf is None else gbf[nd:2 * nd])
-
-
-def _slope_of(ctx, tid):
-    for entry in ctx["tape"]:
-        if entry[0] == "conv" and entry[1].out_id == tid:
-            s = entry[1].slope
-            return -1.0 if s is None else float(s)
-    return -1.0
 
 
 class _UnetFlowFn(torch.autograd.Function):

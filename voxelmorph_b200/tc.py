@@ -102,18 +102,18 @@ _ws_lock = threading.Lock()      # workspace tables are shared by the per-GPU th
 
 def conv_wgrad(xa, xb, gz, cin, cout, kd, up=False, planar_x=None, planar_g=None, need_bias=True, out_w=None, out_b=None, batch=None):
     """fp32 grad_w (cout, cin, kd, 3, 3) and grad_b (cout) from the layer input (xa/xb or planar_x) and gz.
-    `batch` (a WgradBatch): only the wgmma partial-sum kernels are launched now, the reduction into gw / gb happens at
-    `batch.flush()` together with every other layer's."""
+    `batch` (a WgradBatch; channels-last sources only): only the wgmma partial-sum kernels are launched now, the reduction
+    into gw / gb happens at `batch.flush()` together with every other layer's."""
     lib = _lib.load()
-    if batch is not None and wgrad_deferrable(xa, xb, gz, planar_x, planar_g):
-        dev = gz.device
-        accumulate = out_w is not None
-        gw = out_w if accumulate else torch.empty((cout, cin, kd, 3, 3), dtype=torch.float32, device=dev)
-        gb = out_b if accumulate else (torch.empty(cout, dtype=torch.float32, device=dev) if need_bias else None)
-        batch.add(xa, xb, gz, gw, gb, cin, cout, kd, up, accumulate)
-        return gw, gb
     ref = gz if gz is not None else planar_g[0]
     dev = ref.device
+    # out_w / out_b: existing (contiguous fp32) gradient buffers to ACCUMULATE into instead of fresh tensors
+    accumulate = out_w is not None
+    gw = out_w if accumulate else torch.empty((cout, cin, kd, 3, 3), dtype=torch.float32, device=dev)
+    gb = out_b if accumulate else (torch.empty(cout, dtype=torch.float32, device=dev) if need_bias else None)
+    if batch is not None:
+        batch.add(xa, xb, gz, gw, gb, cin, cout, kd, up, accumulate)
+        return gw, gb
     if gz is not None:
         B, D, H, W, Cg = gz.shape
     else:
@@ -126,10 +126,6 @@ def conv_wgrad(xa, xb, gz, cin, cout, kd, up=False, planar_x=None, planar_g=None
             if work is None:
                 work = torch.empty(int(lib.vxm_conv3d_tc_wgrad_workspace_bytes(kd)), dtype=torch.uint8, device=dev)
                 _wgrad_ws[key] = work
-    # out_w / out_b: existing (contiguous fp32) gradient buffers to ACCUMULATE into instead of fresh tensors
-    accumulate = out_w is not None
-    gw = out_w if accumulate else torch.empty((cout, cin, kd, 3, 3), dtype=torch.float32, device=dev)
-    gb = out_b if accumulate else (torch.empty(cout, dtype=torch.float32, device=dev) if need_bias else None)
     xf, xs, npx = _planar_args(planar_x)
     gf, gs, npg = _planar_args(planar_g)
     Ca = 0 if xa is None else xa.shape[-1]
@@ -177,49 +173,17 @@ def planar_fold_kd(planes, cout):
 
 def pack_weights_fold(w, transposed=False):
     """Packed kd-folded 2-D operand of the 3-D weight w (Cout, Cin, 3, 3, 3) (see vxm_conv3d_tcs_pack_desc_fold).
-    Returns (tensor, (coutp, "s")).  Stand-alone helper (tests / tools); the engine packs through its _PackPlan."""
-    lib = _lib.load()
-    w = w.contiguous()
-    Cout, Cin = w.shape[0], w.shape[1]
-    real_in, nout = (Cout, Cin) if transposed else (Cin, Cout)
-    coutp = 16 if nout <= 16 else 32
-    nbytes = int(lib.vxm_conv3d_tcs_packed_bytes(3 * real_in, coutp, 1))
-    out = torch.empty(nbytes // 2, dtype=torch.bfloat16, device=w.device)
-    dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-    host = ctypes.create_string_buffer(dsz)
-    cnt = lib.vxm_conv3d_tcs_pack_desc_fold(ctypes.cast(host, ctypes.c_void_p), _lib.ptr(w), _lib.ptr(out), Cout, Cin, coutp, 1 if transposed else 0, 0)
-    if cnt <= 0:
-        raise _lib.VxmError("vxm_conv3d_tcs_pack_desc_fold: %s" % _lib.last_error())
-    descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(w.device)
-    _lib.check(lib.vxm_conv3d_tcs_pack_multi(_lib.ptr(descs), 1, cnt, _lib.stream_ptr()), "vxm_conv3d_tcs_pack_multi")
-    torch.cuda.current_stream(w.device).synchronize()       # `descs` must outlive the launch
+    Returns (tensor, (coutp, "s")).  Stand-alone helper (tests / tools); the engine packs through its model plan."""
+    table = PackTable([(w.contiguous(), transposed, "fold")])
+    table.refresh()
+    torch.cuda.current_stream(w.device).synchronize()       # the descriptor table must outlive the launch
+    out, coutp = table.packs[0][0, 0]
     return out, (coutp, "s")
 
 
-# ---- weights-stationary ("transposed") kernel: Cin in {8,16,32,48}, Cout <= 32 -------------------------------------
+# ---- kw-stacked kernels: variant "s" (swizzled operands; what the engine runs) and "t" (SWIZZLE_NONE operands) ----------
 
-def _variant():
-    """'s' = kw-stacked kernel with swizzled operands, 't' = kw-stacked with SWIZZLE_NONE operands, 'n' = one MMA per tap."""
-    import os
-    return os.environ.get("VXM_B200_TC_KERNEL", "auto")
-
-
-def use_t_kernel(ca, cb, cout):
-    """True when this convolution runs on a kw-stacked kernel (VXM_B200_TC_KERNEL = auto | s | t | n)."""
-    mode = _variant()
-    if mode == "n":
-        return False
-    lib = _lib.load()
-    if mode in ("auto", "s") and lib.vxm_conv3d_tcs_supported(ca, cb, cout):
-        return True
-    return bool(lib.vxm_conv3d_tct_supported(ca, cb, cout))
-
-
-def _use_s(ca, cb, cout):
-    return _variant() in ("auto", "s") and bool(_lib.load().vxm_conv3d_tcs_supported(ca, cb, cout))
-
-
-def pack_weights_t(w, transposed=False, variant=None):
+def pack_weights_t(w, transposed=False, variant="s"):
     """Packed weights for a kw-stacked kernel.  Returns (tensor, (coutp, variant))."""
     lib = _lib.load()
     if w.dim() == 4:
@@ -228,8 +192,6 @@ def pack_weights_t(w, transposed=False, variant=None):
     Cout, Cin, kd = w.shape[0], w.shape[1], w.shape[2]
     cin_eff, nout = (Cout, Cin) if transposed else (Cin, Cout)
     coutp = 16 if nout <= 16 else (32 if nout <= 32 else (48 if nout <= 48 else 64))
-    if variant is None:
-        variant = "s" if _variant() in ("auto", "s") else "t"
     fb, fp = (lib.vxm_conv3d_tcs_packed_bytes, lib.vxm_conv3d_tcs_pack) if variant == "s" else \
              (lib.vxm_conv3d_tct_packed_bytes, lib.vxm_conv3d_tct_pack)
     nbytes = int(fb(cin_eff, coutp, kd))
@@ -290,75 +252,81 @@ def conv_blocks(ca, cb, nout, kd, split=None):
     return ks, tuple((p0 + j, min(nbmax, pn - j), dst, j) for p0, pn, dst in pieces for j in range(0, pn, nbmax))
 
 
-def block_descs(w, transposed, blocks, host, n, begin, dsz):
-    """Appends the pack descriptors of every (K block, N block) operand of `w` to the host array `host` (n filled so far,
-    element offset `begin`).  Returns ({(ki, ni): (tensor, coutp)}, n, begin)."""
-    lib = _lib.load()
-    w5 = w if w.dim() == 5 else w.unsqueeze(2)
-    Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
-    ks, ns = blocks
-    packs = {}
-    for ki, (_, k0, kb) in enumerate(ks):
-        for ni, (n0, nb, _, _) in enumerate(ns):
-            coutp = np_for(nb)
-            out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(kb, coutp, kd)) // 2, dtype=torch.bfloat16, device=w.device)
-            cnt = lib.vxm_conv3d_tcs_pack_desc_blk(ctypes.cast(ctypes.addressof(host) + n * dsz, ctypes.c_void_p), _lib.ptr(w5), _lib.ptr(out),
-                                                   Cout, Cin, kd, coutp, 1 if transposed else 0, n0, nb, k0, kb, begin)
-            if cnt <= 0:
-                raise _lib.VxmError("vxm_conv3d_tcs_pack_desc_blk: %s" % _lib.last_error())
-            packs[(ki, ni)] = (out, coutp)
-            n, begin = n + 1, begin + cnt
-    return packs, n, begin
+def one_block(cin, nout):
+    """The 1 x 1 block grid (see conv_blocks) of a convolution that runs as one launch per pass: `cin` input channels of
+    the weight operand (the input tensor may pad them), `nout` outputs."""
+    return ((2, 0, cin),), ((0, nout, 0, 0),)
+
+
+class PackTable:
+    """Packed bf16 operands of several weights, all refreshed by ONE vxm_conv3d_tcs_pack_multi launch.  `operands`:
+    [(w, transposed, form)] with form "fold" (the kd-folded 2-D operand of a 3-D weight, see vxm_conv3d_tcs_pack_desc_fold)
+    or channel blocks (conv_blocks, one_block).  packs[i] = {(ki, ni): (tensor, coutp)} of operand i ((0, 0) for a folded
+    one).  The descriptor table is uploaded once and points at the (contiguous fp32) weights themselves, so `refresh`
+    repacks their current values and can be captured in a CUDA graph."""
+
+    def __init__(self, operands):
+        lib = _lib.load()
+        dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
+        host = ctypes.create_string_buffer(dsz * sum(1 if f == "fold" else len(f[0]) * len(f[1]) for _, _, f in operands))
+        self.packs, self.n, self.total = [], 0, 0
+        for w, transposed, form in operands:
+            w5 = w if w.dim() == 5 else w.unsqueeze(2)
+            Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
+            t = 1 if transposed else 0
+            packs = {}
+            if form == "fold":
+                real_in, nout = (Cout, Cin) if transposed else (Cin, Cout)
+                coutp = 16 if nout <= 16 else 32
+                out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(3 * real_in, coutp, 1)) // 2, dtype=torch.bfloat16, device=w.device)
+                cnt = lib.vxm_conv3d_tcs_pack_desc_fold(self._slot(host, dsz), _lib.ptr(w5), _lib.ptr(out), Cout, Cin, coutp, t, self.total)
+                self._add(packs, (0, 0), out, coutp, cnt)
+            else:
+                for ki, (_, k0, kb) in enumerate(form[0]):
+                    for ni, (n0, nb, _, _) in enumerate(form[1]):
+                        coutp = np_for(nb)
+                        out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(kb, coutp, kd)) // 2, dtype=torch.bfloat16, device=w.device)
+                        cnt = lib.vxm_conv3d_tcs_pack_desc_blk(self._slot(host, dsz), _lib.ptr(w5), _lib.ptr(out), Cout, Cin, kd, coutp, t,
+                                                               n0, nb, k0, kb, self.total)
+                        self._add(packs, (ki, ni), out, coutp, cnt)
+            self.packs.append(packs)
+        self.descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(operands[0][0].device)
+
+    def _slot(self, host, dsz):
+        return ctypes.cast(ctypes.addressof(host) + self.n * dsz, ctypes.c_void_p)
+
+    def _add(self, packs, key, out, coutp, cnt):
+        if cnt <= 0:
+            raise _lib.VxmError("vxm_conv3d_tcs_pack_desc: %s" % _lib.last_error())
+        packs[key] = (out, coutp)
+        self.n, self.total = self.n + 1, self.total + cnt
+
+    def refresh(self):
+        _lib.check(_lib.load().vxm_conv3d_tcs_pack_multi(_lib.ptr(self.descs), self.n, self.total, _lib.stream_ptr()),
+                   "vxm_conv3d_tcs_pack_multi")
 
 
 def pack_weights_blocks(w, transposed, blocks):
     """Packed block operands of one weight (one launch).  Returns {(ki, ni): (tensor, coutp)}; the descriptor table stays
     referenced by the result (key None) until the launch has read it."""
-    lib = _lib.load()
-    w = w.contiguous()
-    dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-    host = ctypes.create_string_buffer(dsz * len(blocks[0]) * len(blocks[1]))
-    packs, n, total = block_descs(w, transposed, blocks, host, 0, 0, dsz)
-    descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(w.device)
-    _lib.check(lib.vxm_conv3d_tcs_pack_multi(_lib.ptr(descs), n, total, _lib.stream_ptr()), "vxm_conv3d_tcs_pack_multi")
-    packs[None] = (descs, w)
+    table = PackTable([(w.contiguous(), transposed, blocks)])
+    table.refresh()
+    packs = table.packs[0]
+    packs[None] = table
     return packs
-
-
-class SplitBlockPacks:
-    """Split-precision (bf16x3) operands of a channel-blocked layer: the bf16 hi and lo parts of the weights (see
-    split_weights), packed per block into `hi` / `lo` ({(ki, ni): (tensor, coutp)}).  The descriptor table is uploaded once
-    and points at persistent fp32 buffers, so `refresh` (two elementwise kernels and one pack launch) can be captured in a
-    CUDA graph."""
-
-    def __init__(self, w, blocks):
-        lib = _lib.load()
-        self.blocks = blocks
-        self.w_hi, self.w_lo = torch.empty_like(w.detach()), torch.empty_like(w.detach())
-        dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-        host = ctypes.create_string_buffer(dsz * 2 * len(blocks[0]) * len(blocks[1]))
-        self.hi, n, begin = block_descs(self.w_hi, False, blocks, host, 0, 0, dsz)
-        self.lo, self.n, self.total = block_descs(self.w_lo, False, blocks, host, n, begin, dsz)
-        self.descs = torch.frombuffer(bytearray(host.raw), dtype=torch.uint8).to(w.device)
-
-    def refresh(self, w):
-        w = w.detach()
-        self.w_hi.copy_(w.to(torch.bfloat16))
-        torch.sub(w, self.w_hi, out=self.w_lo)
-        _lib.check(_lib.load().vxm_conv3d_tcs_pack_multi(_lib.ptr(self.descs), self.n, self.total, _lib.stream_ptr()),
-                   "vxm_conv3d_tcs_pack_multi")
-        return self
 
 
 def _ptr_at(t, off):
     return None if t is None else ctypes.c_void_p(t.data_ptr() + off * t.element_size())
 
 
-def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None, mask=None, split=None, lo=None):
+def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None, mask=None, split=None, lo=None, out_fp32_planar=False):
     """One convolution in channel blocks (see conv_blocks); packs[(ki, ni)] = (operand, coutp) of K block ki, N block ni.
     Every N block accumulates its K blocks in an fp32 channels-last buffer (out_mode 2) and the last launch adds bias and
     activation (or the LeakyReLU-derivative mask) and stores its channels into the full-width bf16 output.
-    lo = (xa_lo, xb_lo, packs_lo): split precision, three passes per K block; returns the (hi, lo) pair.
+    lo = (xa_lo, xb_lo, packs_lo): split precision (bf16x3), three passes per K block, x_lo * w_hi + x_hi * w_lo +
+    x_hi * w_hi (smallest terms first); returns the (hi, lo) pair, or with out_fp32_planar (one N block) the fp32 planar
+    (B, nout, D, H, W) output.  A 1 x 1 grid (one_block) is the split-precision form of a layer that runs in one launch.
     split: returns the outputs [0, split) and [split, nout) as two tensors (dgrad of a concatenation)."""
     lib = _lib.load()
     ks, ns = blocks
@@ -368,10 +336,16 @@ def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None
         D, H, W = (D * 2 if kd == 3 else D), H * 2, W * 2
     if mask is not None and split:
         raise _lib.VxmError("conv_fwd_blocked: a mask with a split output is not implemented")
-    outs = [torch.empty((B, D, H, W, c), dtype=torch.bfloat16, device=full.device) for c in ([split, nout - split] if split else [nout])]
-    outs_lo = [torch.empty_like(o) for o in outs] if lo is not None else [None] * len(outs)
+    if out_fp32_planar and (split or len(ns) != 1):
+        raise _lib.VxmError("conv_fwd_blocked: the fp32 planar output takes one N block")
+    if out_fp32_planar:
+        outs = [torch.empty((B, nout, D, H, W), dtype=torch.float32, device=full.device)]
+    else:
+        outs = [torch.empty((B, D, H, W, c), dtype=torch.bfloat16, device=full.device) for c in ([split, nout - split] if split else [nout])]
+    outs_lo = [torch.empty_like(o) for o in outs] if lo is not None and not out_fp32_planar else [None] * len(outs)
     s = -1.0 if slope is None else float(slope)
     ca = 0 if xa is None else xa.shape[-1]
+    cb = 0 if xb is None else xb.shape[-1]
     for ni, (n0, nb, dst, doff) in enumerate(ns):
         out, pitch = outs[dst], outs[dst].shape[-1]
         passes = [(ki, 0, False) for ki in range(len(ks))] if lo is None else \
@@ -386,13 +360,18 @@ def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None
             elif src == 1:
                 x0, x1, c0, c1, u = pb, None, kb, 0, False
             else:
-                x0, x1, c0, c1, u = pa, pb, ca, kb - ca, up
+                x0, x1, c0, c1, u = pa, pb, ca, cb, up
             wpk, coutp = (lo[2] if wlo else packs)[(ki, ni)]
             if pi + 1 < len(passes):
                 ain = acc
                 if acc is None:
                     acc = torch.empty((B, D, H, W, coutp), dtype=torch.float32, device=full.device)
                 o, olo, m, mode, op, bptr = _lib.ptr(acc), None, None, 2, 0, None
+            elif out_fp32_planar:        # + bias -> fp32 planar (the flow head), an entry point without an output pitch
+                _lib.check(lib.vxm_conv3d_tcs_fwd_acc(_lib.ptr(x0), _lib.ptr(x1), _lib.ptr(wpk), _lib.ptr(bias), _lib.ptr(out), None,
+                                                      _lib.ptr(acc), B, D, H, W, c0, c1, 1 if u else 0, nb, coutp, kd, 1, s,
+                                                      _lib.stream_ptr()), "vxm_conv3d_tcs_fwd_acc")
+                continue
             else:
                 ain = acc
                 o, olo, m = _ptr_at(out, doff), _ptr_at(outs_lo[dst], doff), _ptr_at(mask, n0)
@@ -400,18 +379,14 @@ def conv_fwd_blocked(xa, xb, blocks, packs, bias, nout, kd, up=False, slope=None
             _lib.check(lib.vxm_conv3d_tcs_fwd_blk(_lib.ptr(x0), _lib.ptr(x1), _lib.ptr(wpk), bptr, o, olo, m, _lib.ptr(ain),
                                                   B, D, H, W, c0, c1, 1 if u else 0, nb, coutp, kd, mode, s, op, _lib.stream_ptr()),
                        "vxm_conv3d_tcs_fwd_blk")
+    if out_fp32_planar:
+        return outs[0]
     if lo is not None:
         return outs[0], outs_lo[0]
     return tuple(outs) if split else outs[0]
 
 
-# ---- split-precision (bf16x3) passes ----------------------------------------------------------------------------------
-
-def split_weights(w):
-    """fp32 weights -> (hi, lo) fp32 tensors with hi = bf16(w), lo = w - hi (packed as bf16 by the weight packer)."""
-    hi = w.detach().to(torch.bfloat16).float()
-    return hi, w.detach() - hi
-
+# ---- split-precision (bf16x3) glue ------------------------------------------------------------------------------------
 
 def planar_to_ndhwc8_split(planes):
     """<= 8 planar fp32 volumes -> (hi, lo) bf16 (B,D,H,W,8) tensors with hi + lo = x to 16 mantissa bits."""
@@ -426,47 +401,6 @@ def planar_to_ndhwc8_split(planes):
     lo = torch.empty_like(hi)
     _lib.check(lib.vxm_planar_to_ndhwc8_split_bf16(arr_p, arr_s, n, _lib.ptr(hi), _lib.ptr(lo), B, D * H * W, _lib.stream_ptr()),
                "vxm_planar_to_ndhwc8_split_bf16")
-    return hi, lo
-
-
-def conv_fwd_split(xa, xb, packs, bias, cout, kd, up=False, out_fp32_planar=False, slope=None):
-    """One convolution layer in split precision: three passes of the kw-stacked wgmma kernel accumulating
-    x_lo*w_hi + x_hi*w_lo + x_hi*w_hi in an fp32 channels-last buffer.  xa / xb: (hi, lo) pairs (or None);
-    packs: ((wpk_hi, meta), (wpk_lo, meta)) from pack_weights_t.  Returns a (hi, lo) pair of bf16 NDHWC tensors, or the
-    fp32 planar tensor when out_fp32_planar."""
-    lib = _lib.load()
-    (wh, (coutp, variant)), (wl, _) = packs
-    if variant != "s":
-        raise _lib.VxmError("split-precision convolution needs the swizzled kw-stacked kernel (VXM_B200_TC_KERNEL=auto|s)")
-    full = xb if xb is not None else xa
-    fh = full[0]
-    B, D, H, W = fh.shape[0], fh.shape[1], fh.shape[2], fh.shape[3]
-    if xb is None and up:
-        D, H, W = (D * 2 if kd == 3 else D), H * 2, W * 2
-    Ca = 0 if xa is None else xa[0].shape[-1]
-    Cb = 0 if xb is None else xb[0].shape[-1]
-    dev = fh.device
-    acc = torch.empty((B, D, H, W, coutp), dtype=torch.float32, device=dev)
-    s = -1.0 if slope is None else float(slope)
-
-    def part(x, k):
-        return None if x is None else x[k]
-
-    def launch(k_x, wpk, out, out_lo, acc_in, mode):
-        _lib.check(lib.vxm_conv3d_tcs_fwd_acc(_lib.ptr(part(xa, k_x)), _lib.ptr(part(xb, k_x)), _lib.ptr(wpk), _lib.ptr(bias),
-                                              _lib.ptr(out), _lib.ptr(out_lo), _lib.ptr(acc_in), B, D, H, W, Ca, Cb,
-                                              1 if up else 0, cout, coutp, kd, mode, s, _lib.stream_ptr()),
-                   "vxm_conv3d_tcs_fwd_acc")
-
-    launch(1, wh, acc, None, None, 2)          # x_lo * w_hi   (smallest terms first)
-    launch(0, wl, acc, None, acc, 2)           # + x_hi * w_lo
-    if out_fp32_planar:
-        out = torch.empty((B, cout, D, H, W), dtype=torch.float32, device=dev)
-        launch(0, wh, out, None, acc, 1)       # + x_hi * w_hi + bias -> fp32 planar
-        return out
-    hi = torch.empty((B, D, H, W, cout), dtype=torch.bfloat16, device=dev)
-    lo = torch.empty_like(hi)
-    launch(0, wh, hi, lo, acc, 3)              # + x_hi * w_hi + bias, activation -> (hi, lo)
     return hi, lo
 
 
@@ -557,15 +491,3 @@ class WgradBatch:
                        "vxm_conv3d_tc_wgrad2_flush")
         self.n.value = 0
         self.off = 0
-
-
-def wgrad_deferrable(xa, xb, gz, planar_x=None, planar_g=None):
-    import os
-    if os.environ.get("VXM_B200_WGRAD_DEFER", "1") != "1" or os.environ.get("VXM_B200_WGRAD", "")[:1] == "o":
-        return False
-    if gz is None or planar_x is not None or planar_g is not None:
-        return False
-    ok = lambda c: c in (8, 16, 32, 64)  # noqa: E731
-    ca = 0 if xa is None else xa.shape[-1]
-    cb = 0 if xb is None else xb.shape[-1]
-    return (ca == 0 or ok(ca)) and (cb == 0 or ok(cb)) and ca + cb > 0 and ok(gz.shape[-1])
