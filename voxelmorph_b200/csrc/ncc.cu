@@ -223,16 +223,19 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
 // The generic kernel above spends ~290 instructions per voxel (direct 9-tap sums in all three passes, a 16x32 tile
 // whose 24x40 halo'd slab is re-staged and re-filtered for every one of its zchunk + 8 slices) and two-plus
 // barriers per slice on 252 CTAs: 0.04 of the HBM roofline.  This kernel
-//   * runs the D pass FIRST, as a sliding window kept in shared memory: per halo'd column  S += P(z+4) - P(z-5)
-//     (P = the 5 product fields of the new slice; the leaving slice is re-read from L2), so the z halo slices cost a
-//     load and 10 adds per column, not a W and an H pass;
-//   * runs the W and H passes on the D-summed slice as register sliding windows (8 / 4 outputs per thread:
-//     9-term seed + 2 adds per further output instead of 9 adds each);
+//   * runs the D pass FIRST, so the z halo slices cost loads, not a W and an H pass.  The forward sums every halo'd
+//     column directly over the window's slices, re-read from L1 / L2: a running sum's rounding residue would be as
+//     large as the true sums in background and rim windows, and the pointwise stage divides by den ~ 1e-5 there.
+//     The backward's box sums of A, Bq, T feed no division; there the window slides, S += P(z+4) - P(z-5) in shared
+//     memory, and the leading halo slices cost a load and 3 adds per column;
+//   * runs the W and H passes on the D-summed slice in registers, 8 / 4 outputs per thread, each window the sum of
+//     a suffix sum of the first half and a prefix sum of the second (22 / 14 adds instead of 72 / 36, no subtraction),
+//     so every box sum is a sum of the window's own values and a window of zeros sums to exactly 0, as in the reference;
 //   * uses a 32 x 56 tile (halo overhead 1.43x instead of 1.88x; 224 = 4 x 56), 512 threads, 2 CTAs per SM,
 //     bank-conflict-free pitches (68 / 60 floats) for the 16-byte shared-memory accesses of the W pass;
 //   * is persistent over (tile, depth-chunk) items, so any volume fits the reduction workspace.
-// A sliding window of at most zchunk + 8 updates accumulates less rounding than the 729-term direct sum it
-// replaces; tests/test_gpu_ops.py holds the loss to 1e-4 and the gradient to 1e-3 of the reference.
+// tests/test_gpu_fp32_step_kernels.py holds the loss and the gradient to twice the fp64 distance of the
+// reference's own fp32 arithmetic (+1e-6), on smooth, skull-stripped and offset images.
 // ------------------------------------------------------------------------------------------------------------
 namespace ncc9 {
 constexpr int TH = 32, TW = 56, HR = TH + 8, HC = TW + 8, PD = 68, PW = 60, NT = 512;
@@ -269,7 +272,6 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
     const float* f0 = (MODE == 0 ? a.I : a.saved_in) + (size_t)b * (MODE == 0 ? 1 : 3) * DHW;
     const float* f1 = MODE == 0 ? a.J + (size_t)b * DHW : f0 + DHW;
     const float* f2 = MODE == 0 ? nullptr : f0 + 2 * DHW;
-    for (int i = tid; i < NS * HR * PD; i += NT) s_d[i] = 0.f;
     int goff[KC], soff[KC];
 #pragma unroll
     for (int k = 0; k < KC; ++k) {
@@ -278,10 +280,45 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
       goff[k] = (h >= 0 && h < a.H && w >= 0 && w < a.W) ? h * a.W + w : -1;
       soff[k] = r * PD + c;
     }
-    __syncthreads();
-    for (int zi = z0 - PDZ; zi < z1 + PDZ; ++zi) {
-      // ---------------- D pass: slide the window of every halo'd column by one slice ----------------
-      {
+    if (MODE == 1) {
+      for (int i = tid; i < NS * HR * PD; i += NT) s_d[i] = 0.f;
+      __syncthreads();
+    }
+    // forward: one iteration per output slice; backward: the window's leading halo slices first (running sum)
+    for (int zi = MODE == 0 ? z0 + PDZ : z0 - PDZ; zi < z1 + PDZ; ++zi) {
+      const int zo = zi - PDZ;
+      if (MODE == 0) {
+        // ---------------- D pass (forward): every halo'd column summed directly over the WD slices of the window ----
+        // (zero padded).  A running sum (S += new - old) keeps the rounding of the larger values it slid past: where a
+        // window then holds only zeros or faint values (the background and rims of skull-stripped images) that residue
+        // is as large as the true sums, and den = Ivar * Jvar + 1e-5 turns it into large errors in cc, A and Bq.
+#pragma unroll
+        for (int k = 0; k < KC; ++k) {
+          float acc[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
+          if (goff[k] >= 0) {
+            float u[WD], v[WD];
+#pragma unroll
+            for (int j = 0; j < WD; ++j) {
+              const int zj = zo - PDZ + j;
+              u[j] = v[j] = 0.f;
+              if (zj >= 0 && zj < a.D) {
+                const size_t o = (size_t)zj * HW + goff[k];
+                u[j] = __ldg(f0 + o); v[j] = __ldg(f1 + o);
+              }
+            }
+#pragma unroll
+            for (int j = 0; j < WD; ++j) {
+              acc[0] += u[j]; acc[1] += v[j]; acc[2] += u[j] * u[j]; acc[3] += v[j] * v[j]; acc[4] += u[j] * v[j];
+            }
+          }
+          float* d = s_d + soff[k];
+#pragma unroll
+          for (int f = 0; f < 5; ++f) d[f * HR * PD] = acc[f];
+        }
+      } else {
+        // ---------------- D pass (backward): slide the window of every halo'd column by one slice ----------------
+        // S += P(zi) - P(zi - WD) over the saved A, Bq, T.  No division follows, so the residue of this running sum stays
+        // at the rounding level of the values it slid past (the test suite checks d/dJ on skull-stripped images).
         const int zold = zi - WD;
         const bool has_new = zi >= 0 && zi < a.D;
         const bool has_old = WD > 1 && zold >= z0 - PDZ && zold >= 0;   // it was added earlier in this chunk
@@ -292,13 +329,11 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
           if (goff[k] >= 0) {
             if (has_new) {
               const size_t o = (size_t)zi * HW + goff[k];
-              un[k] = __ldg(f0 + o); vn[k] = __ldg(f1 + o);
-              if (MODE == 1) tn[k] = __ldg(f2 + o);
+              un[k] = __ldg(f0 + o); vn[k] = __ldg(f1 + o); tn[k] = __ldg(f2 + o);
             }
             if (has_old) {
               const size_t o = (size_t)zold * HW + goff[k];
-              uo[k] = __ldg(f0 + o); vo[k] = __ldg(f1 + o);
-              if (MODE == 1) to[k] = __ldg(f2 + o);
+              uo[k] = __ldg(f0 + o); vo[k] = __ldg(f1 + o); to[k] = __ldg(f2 + o);
             }
           }
         }
@@ -306,25 +341,15 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
         for (int k = 0; k < KC; ++k) {
           if (goff[k] >= 0) {
             float* d = s_d + soff[k];
-            if (MODE == 0) {
-              const float dl[5] = {un[k] - uo[k], vn[k] - vo[k], un[k] * un[k] - uo[k] * uo[k], vn[k] * vn[k] - vo[k] * vo[k],
-                                   un[k] * vn[k] - uo[k] * vo[k]};
+            const float dl[3] = {un[k] - uo[k], vn[k] - vo[k], tn[k] - to[k]};
 #pragma unroll
-              for (int f = 0; f < 5; ++f) {
-                if (WD > 1) d[f * HR * PD] += dl[f]; else d[f * HR * PD] = dl[f];
-              }
-            } else {
-              const float dl[3] = {un[k] - uo[k], vn[k] - vo[k], tn[k] - to[k]};
-#pragma unroll
-              for (int f = 0; f < 3; ++f) {
-                if (WD > 1) d[f * HR * PD] += dl[f]; else d[f * HR * PD] = dl[f];
-              }
+            for (int f = 0; f < 3; ++f) {
+              if (WD > 1) d[f * HR * PD] += dl[f]; else d[f * HR * PD] = dl[f];
             }
           }
         }
       }
       __syncthreads();
-      const int zo = zi - PDZ;
       if (zo >= z0) {   // block-uniform
         // ---------------- W pass: 8 adjacent window sums per work item from 16 staged values ----------------
         for (int it = tid; it < NS * 7 * HR; it += NT) {
@@ -332,10 +357,17 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
           const float4* src = reinterpret_cast<const float4*>(s_d + (f * HR + r) * PD + seg * 8);
           const float4 x0 = src[0], x1 = src[1], x2 = src[2], x3 = src[3];
           const float x[16] = {x0.x, x0.y, x0.z, x0.w, x1.x, x1.y, x1.z, x1.w, x2.x, x2.y, x2.z, x2.w, x3.x, x3.y, x3.z, x3.w};
-          float o[8];
-          o[0] = (((x[0] + x[1]) + (x[2] + x[3])) + ((x[4] + x[5]) + (x[6] + x[7]))) + x[8];
+          // o[j] = x[j..j+8] = (x[j] + .. + x[7]) + (x[8] + .. + x[8+j]): suffix sums of the first half plus prefix sums
+          // of the second, no subtraction, so a window of zeros sums to exactly 0
+          float sfx[8], pfx[8], o[8];
+          sfx[7] = x[7];
+          pfx[0] = x[8];
 #pragma unroll
-          for (int j = 1; j < 8; ++j) o[j] = o[j - 1] + (x[j + 8] - x[j - 1]);
+          for (int j = 6; j >= 0; --j) sfx[j] = x[j] + sfx[j + 1];
+#pragma unroll
+          for (int j = 1; j < 8; ++j) pfx[j] = pfx[j - 1] + x[j + 8];
+#pragma unroll
+          for (int j = 0; j < 8; ++j) o[j] = sfx[j] + pfx[j];
           float4* dst = reinterpret_cast<float4*>(s_w + (f * HR + r) * PW + seg * 8);
           dst[0] = make_float4(o[0], o[1], o[2], o[3]);
           dst[1] = make_float4(o[4], o[5], o[6], o[7]);
@@ -351,9 +383,14 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
             float col[12];
 #pragma unroll
             for (int j = 0; j < 12; ++j) col[j] = colp[j * PW];
-            S[f][0] = (((col[0] + col[1]) + (col[2] + col[3])) + ((col[4] + col[5]) + (col[6] + col[7]))) + col[8];
+            // S[j] = col[j..j+8] = (col[j] + .. + col[7]) + (col[8] + .. + col[8+j]), as in the W pass
+            float sfx = col[3] + ((col[4] + col[5]) + (col[6] + col[7])), pfx = col[8];
+            S[f][3] = sfx;
 #pragma unroll
-            for (int j = 1; j < 4; ++j) S[f][j] = S[f][j - 1] + (col[j + 8] - col[j - 1]);
+            for (int j = 2; j >= 0; --j) { sfx = col[j] + sfx; S[f][j] = sfx; }
+            S[f][0] += pfx;
+#pragma unroll
+            for (int j = 1; j < 4; ++j) { pfx += col[j + 8]; S[f][j] += pfx; }
           }
           const int w = wt * TW + wl;
           if (w < a.W) {
@@ -392,7 +429,7 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
         }
       }
     }
-    __syncthreads();   // every thread is done with s_w / s_d before the next item clears s_d
+    __syncthreads();   // every thread is done with s_w / s_d before the next item writes them
   }
   if (MODE == 0) {
     double tot = block_sum<double>(local, s_red);
