@@ -1,11 +1,17 @@
-// Trilinear / nearest gather primitives shared by the warp and VecInt kernels.
+// Trilinear / nearest sampling shared by the warp and VecInt kernels, written once per arithmetic mode.
 //
-// Reference semantics: voxelmorph/torch/layers.py:30-48 -> F.grid_sample(align_corners=True,
-// padding_mode='zeros').  Corner weights and accumulation order follow ATen's
-// grid_sampler_3d (weights are products (x1-x)(y1-y)(z1-z) ...; corners outside the volume
-// contribute nothing).  Products and sums use explicit _rn intrinsics so the result does not
-// depend on FMA contraction: the linear path reproduces the torch CPU reference to the bit on
-// every input we have tried, and the nearest path is bit-exact by construction.
+// Reference semantics: voxelmorph/torch/layers.py:30-48 -> F.grid_sample(align_corners=True, padding_mode='zeros').
+// Corners are numbered in ATen's order: bit0 = x+1, bit1 = y+1, bit2 = z+1; a corner outside the volume reads as 0
+// and receives no gradient.
+//
+// * Exact mode (VXM_ARITH_TRUE_DIV / VXM_ARITH_RECIPROCAL): the reference's coordinate replay (`exact_coords`),
+//   ATen grid_sampler_3d's corner weights (products (x1-x)(y1-y)(z1-z) ...) and accumulation order, every product
+//   and sum an explicit _rn intrinsic so that the result does not depend on FMA contraction.  The linear path
+//   reproduces the torch CPU reference to the bit on every input we have tried; the nearest path is bit-exact by
+//   construction.  This is the reference mode the bit-exact tests compare against.
+// * Fast mode (VXM_ARITH_FAST): coordinates (p + v)·r computed by the caller, the blend and its gradient as lerp
+//   trees, and cells that lie inside the volume (all but a one-voxel shell for registration flows) read their
+//   corners without per-corner predicates.
 #pragma once
 #include "common.cuh"
 
@@ -23,131 +29,111 @@ __host__ __device__ inline Vol make_vol(int D, int H, int W) {
   return v;
 }
 
-// Corner stencil of one sampling position: base index (may be out of range), per-corner
-// weights and validity mask, in ATen corner order: bit2 = z+1, bit1 = y+1, bit0 = x+1.
-struct Stencil {
-  int x0, y0, z0;
-  float wx0, wx1, wy0, wy1, wz0, wz1;
-  unsigned mask;  // bit k set <=> corner k inside the volume
-};
+// ------------------------------------------------------------------------------------------------------------
+// Exact mode
+// ------------------------------------------------------------------------------------------------------------
 
-template <bool IS3D>
-__device__ __forceinline__ Stencil make_stencil(float cx, float cy, float cz, const Vol& s) {
-  Stencil st;
-  float fx = floorf(cx), fy = floorf(cy);
-  st.x0 = f2i(fx);
-  st.y0 = f2i(fy);
-  st.wx0 = __fsub_rn(__fadd_rn(fx, 1.0f), cx);
-  st.wx1 = __fsub_rn(cx, fx);
-  st.wy0 = __fsub_rn(__fadd_rn(fy, 1.0f), cy);
-  st.wy1 = __fsub_rn(cy, fy);
-  bool x0ok = (unsigned)st.x0 < (unsigned)s.W, x1ok = (unsigned)(st.x0 + 1) < (unsigned)s.W;
-  bool y0ok = (unsigned)st.y0 < (unsigned)s.H, y1ok = (unsigned)(st.y0 + 1) < (unsigned)s.H;
-  bool z0ok = true, z1ok = false;
+// Replays the reference's sampling coordinates of voxel (z, y, x).  f points at the voxel's first field channel,
+// cs is the channel stride (channel order D, H, W for 3-D; H, W for 2-D); fv receives the field's own values.
+// G is any geometry with the AxisNorms ax, ay, az.  Plain loads: VecInt reads fields written earlier in its launch.
+template <bool IS3D, int ARITH, class G>
+__device__ __forceinline__ void exact_coords(const float* f, size_t cs, int z, int y, int x, const G& g, float fv[3],
+                                             float& cz, float& cy, float& cx) {
   if (IS3D) {
-    float fz = floorf(cz);
-    st.z0 = f2i(fz);
-    st.wz0 = __fsub_rn(__fadd_rn(fz, 1.0f), cz);
-    st.wz1 = __fsub_rn(cz, fz);
-    z0ok = (unsigned)st.z0 < (unsigned)s.D;
-    z1ok = (unsigned)(st.z0 + 1) < (unsigned)s.D;
+    fv[0] = f[0]; fv[1] = f[cs]; fv[2] = f[2 * cs];
+    cz = sample_coord<ARITH>((float)z, fv[0], g.az);
+    cy = sample_coord<ARITH>((float)y, fv[1], g.ay);
+    cx = sample_coord<ARITH>((float)x, fv[2], g.ax);
   } else {
-    st.z0 = 0; st.wz0 = 1.0f; st.wz1 = 0.0f;
+    fv[0] = f[0]; fv[1] = f[cs]; fv[2] = 0.f;
+    cz = 0.f;
+    cy = sample_coord<ARITH>((float)y, fv[0], g.ay);
+    cx = sample_coord<ARITH>((float)x, fv[1], g.ax);
   }
-  unsigned m = 0;
-  m |= (z0ok && y0ok && x0ok) ? 1u : 0u;
-  m |= (z0ok && y0ok && x1ok) ? 2u : 0u;
-  m |= (z0ok && y1ok && x0ok) ? 4u : 0u;
-  m |= (z0ok && y1ok && x1ok) ? 8u : 0u;
-  m |= (z1ok && y0ok && x0ok) ? 16u : 0u;
-  m |= (z1ok && y0ok && x1ok) ? 32u : 0u;
-  m |= (z1ok && y1ok && x0ok) ? 64u : 0u;
-  m |= (z1ok && y1ok && x1ok) ? 128u : 0u;
-  st.mask = m;
-  return st;
 }
 
-// weight of corner k: (x-term * y-term) * z-term, each product rounded (ATen order)
+// The trilinear cell of one exact-mode sample point: per corner a clamped offset (always loadable) and a weight, per
+// axis the two tap weights, and the mask of the corners inside the volume.  A tap outside the volume has weight 0.
 template <bool IS3D>
-__device__ __forceinline__ float corner_weight(const Stencil& st, int k) {
-  float wx = (k & 1) ? st.wx1 : st.wx0;
-  float wy = (k & 2) ? st.wy1 : st.wy0;
-  float w = __fmul_rn(wx, wy);
-  if (IS3D) {
-    float wz = (k & 4) ? st.wz1 : st.wz0;
-    w = __fmul_rn(w, wz);
-  }
-  return w;
-}
-
-__device__ __forceinline__ ptrdiff_t corner_offset(const Stencil& st, int k, const Vol& s) {
-  return ((ptrdiff_t)(st.z0 + ((k >> 2) & 1)) * s.H + (st.y0 + ((k >> 1) & 1))) * (ptrdiff_t)s.W +
-         (st.x0 + (k & 1));
-}
-
-// value of one channel plane at the stencil
-template <bool IS3D>
-__device__ __forceinline__ float sample_linear(const float* __restrict__ plane, const Stencil& st,
-                                               const Vol& s) {
-  constexpr int NC = IS3D ? 8 : 4;
-  float acc = 0.0f;
-  ptrdiff_t base = corner_offset(st, 0, s);
-#pragma unroll
-  for (int k = 0; k < NC; ++k) {
-    if (st.mask & (1u << k)) {
-      ptrdiff_t off = base + ((k >> 2) & 1) * (ptrdiff_t)s.HW + ((k >> 1) & 1) * (ptrdiff_t)s.W + (k & 1);
-      float v = __ldg(plane + off);
-      acc = __fadd_rn(acc, __fmul_rn(v, corner_weight<IS3D>(st, k)));
-    }
-  }
-  return acc;
-}
-
-// Branch-free form of the same stencil for the hot forward kernels: 32-bit clamped offsets and weights that are
-// exactly 0 for out-of-volume corners.  acc + v*0 leaves acc unchanged, so the result equals the predicated form
-// (for finite inputs) bit for bit, with ~3x fewer instructions.
-struct Stencil8 {
+struct ExactCell {
   int off[8];
-  float w[8];
+  float w[8];      // (x-weight * y-weight) * z-weight, each product rounded (ATen order)
+  float wx[2], wy[2], wz[2];
+  unsigned mask;   // bit k set <=> corner k inside the volume
 };
+
 template <bool IS3D>
-__device__ __forceinline__ void make_stencil8(float cx, float cy, float cz, int D, int H, int W, Stencil8& s) {
+__device__ __forceinline__ ExactCell<IS3D> exact_cell(float cz, float cy, float cx, int D, int H, int W) {
+  ExactCell<IS3D> c;
   const float fx = floorf(cx), fy = floorf(cy);
   const int x0 = f2i(fx), y0 = f2i(fy);
-  float wx0 = __fsub_rn(__fadd_rn(fx, 1.0f), cx), wx1 = __fsub_rn(cx, fx);
-  float wy0 = __fsub_rn(__fadd_rn(fy, 1.0f), cy), wy1 = __fsub_rn(cy, fy);
-  wx0 = (unsigned)x0 < (unsigned)W ? wx0 : 0.f;
-  wx1 = (unsigned)(x0 + 1) < (unsigned)W ? wx1 : 0.f;
-  wy0 = (unsigned)y0 < (unsigned)H ? wy0 : 0.f;
-  wy1 = (unsigned)(y0 + 1) < (unsigned)H ? wy1 : 0.f;
-  const int xa = min(max(x0, 0), W - 1), xb = min(max(x0, -1) + 1, W - 1);
-  const int ya = min(max(y0, 0), H - 1) * W, yb = (min(max(y0, -1) + 1, H - 1)) * W;
-  const float w00 = __fmul_rn(wx0, wy0), w10 = __fmul_rn(wx1, wy0), w01 = __fmul_rn(wx0, wy1), w11 = __fmul_rn(wx1, wy1);
+  const bool xok[2] = {(unsigned)x0 < (unsigned)W, (unsigned)(x0 + 1) < (unsigned)W};
+  const bool yok[2] = {(unsigned)y0 < (unsigned)H, (unsigned)(y0 + 1) < (unsigned)H};
+  bool zok[2] = {true, false};
+  c.wx[0] = xok[0] ? __fsub_rn(__fadd_rn(fx, 1.0f), cx) : 0.f;
+  c.wx[1] = xok[1] ? __fsub_rn(cx, fx) : 0.f;
+  c.wy[0] = yok[0] ? __fsub_rn(__fadd_rn(fy, 1.0f), cy) : 0.f;
+  c.wy[1] = yok[1] ? __fsub_rn(cy, fy) : 0.f;
+  const int ox[2] = {min(max(x0, 0), W - 1), min(max(x0, -1) + 1, W - 1)};
+  const int oy[2] = {min(max(y0, 0), H - 1) * W, min(max(y0, -1) + 1, H - 1) * W};
+  int oz[2] = {0, 0};
+  c.wz[0] = 1.0f; c.wz[1] = 0.0f;
   if (IS3D) {
     const float fz = floorf(cz);
     const int z0 = f2i(fz);
-    float wz0 = __fsub_rn(__fadd_rn(fz, 1.0f), cz), wz1 = __fsub_rn(cz, fz);
-    wz0 = (unsigned)z0 < (unsigned)D ? wz0 : 0.f;
-    wz1 = (unsigned)(z0 + 1) < (unsigned)D ? wz1 : 0.f;
-    const int za = min(max(z0, 0), D - 1) * (H * W), zb = (min(max(z0, -1) + 1, D - 1)) * (H * W);
-    s.off[0] = za + ya + xa; s.off[1] = za + ya + xb; s.off[2] = za + yb + xa; s.off[3] = za + yb + xb;
-    s.off[4] = zb + ya + xa; s.off[5] = zb + ya + xb; s.off[6] = zb + yb + xa; s.off[7] = zb + yb + xb;
-    s.w[0] = __fmul_rn(w00, wz0); s.w[1] = __fmul_rn(w10, wz0); s.w[2] = __fmul_rn(w01, wz0); s.w[3] = __fmul_rn(w11, wz0);
-    s.w[4] = __fmul_rn(w00, wz1); s.w[5] = __fmul_rn(w10, wz1); s.w[6] = __fmul_rn(w01, wz1); s.w[7] = __fmul_rn(w11, wz1);
-  } else {
-    s.off[0] = ya + xa; s.off[1] = ya + xb; s.off[2] = yb + xa; s.off[3] = yb + xb;
-    s.w[0] = w00; s.w[1] = w10; s.w[2] = w01; s.w[3] = w11;
+    zok[0] = (unsigned)z0 < (unsigned)D;
+    zok[1] = (unsigned)(z0 + 1) < (unsigned)D;
+    c.wz[0] = zok[0] ? __fsub_rn(__fadd_rn(fz, 1.0f), cz) : 0.f;
+    c.wz[1] = zok[1] ? __fsub_rn(cz, fz) : 0.f;
+    oz[0] = min(max(z0, 0), D - 1) * (H * W); oz[1] = min(max(z0, -1) + 1, D - 1) * (H * W);
   }
+  c.mask = 0;
+#pragma unroll
+  for (int k = 0; k < 8; ++k) {
+    c.off[k] = oz[k >> 2] + oy[(k >> 1) & 1] + ox[k & 1];
+    const float w = __fmul_rn(c.wx[k & 1], c.wy[(k >> 1) & 1]);
+    c.w[k] = IS3D ? __fmul_rn(w, c.wz[k >> 2]) : w;
+    c.mask |= (zok[k >> 2] && yok[(k >> 1) & 1] && xok[k & 1]) ? (1u << k) : 0u;
+  }
+  return c;
 }
+
+// Value of one channel plane at the cell, branch free: a corner outside the volume has weight 0 and acc + v*0 leaves
+// acc unchanged, so this equals the masked sum bit for bit (for finite inputs).  READONLY: the plane is not written
+// during the launch, so it may go through the read-only path.
 template <bool IS3D, bool READONLY>
-__device__ __forceinline__ float sample8(const float* __restrict__ plane, const Stencil8& s) {
+__device__ __forceinline__ float exact_sample(const float* __restrict__ plane, const ExactCell<IS3D>& c) {
   float acc = 0.0f;
 #pragma unroll
   for (int k = 0; k < (IS3D ? 8 : 4); ++k) {
-    const float v = READONLY ? __ldg(plane + s.off[k]) : plane[s.off[k]];
-    acc = __fadd_rn(acc, __fmul_rn(v, s.w[k]));
+    const float v = READONLY ? __ldg(plane + c.off[k]) : plane[c.off[k]];
+    acc = __fadd_rn(acc, __fmul_rn(v, c.w[k]));
   }
   return acc;
+}
+
+// d(value)/d(coordinate) in signed-sum form, added to (gz, gy, gx).  s(off) is the scalar corner k carries: its value
+// times an adjoint, or its channels dotted with one.
+template <bool IS3D, class S>
+__device__ __forceinline__ void exact_grad(const ExactCell<IS3D>& c, S s, float& gz, float& gy, float& gx) {
+#pragma unroll
+  for (int k = 0; k < (IS3D ? 8 : 4); ++k) {
+    if (c.mask & (1u << k)) {
+      const float v = s(c.off[k]);
+      const float wx = c.wx[k & 1], wy = c.wy[(k >> 1) & 1], wz = IS3D ? c.wz[k >> 2] : 1.0f;
+      gx += ((k & 1) ? v : -v) * wy * wz;
+      gy += ((k & 2) ? v : -v) * wx * wz;
+      if (IS3D) gz += ((k & 4) ? v : -v) * wx * wy;
+    }
+  }
+}
+
+// d(value)/d(plane): adds weight(k) * go to every corner inside the volume (fp32 atomics)
+template <bool IS3D>
+__device__ __forceinline__ void exact_scatter(const ExactCell<IS3D>& c, float* plane, float go) {
+#pragma unroll
+  for (int k = 0; k < (IS3D ? 8 : 4); ++k)
+    if (c.mask & (1u << k)) atomicAdd(plane + c.off[k], c.w[k] * go);
 }
 
 // nearest index (round half to even) or -1 when outside the volume
@@ -157,6 +143,135 @@ __device__ __forceinline__ ptrdiff_t nearest_index(float cx, float cy, float cz,
   int z = IS3D ? f2i(rintf(cz)) : 0;
   bool ok = (unsigned)x < (unsigned)s.W && (unsigned)y < (unsigned)s.H && (unsigned)z < (unsigned)s.D;
   return ok ? ((ptrdiff_t)z * s.H + y) * (ptrdiff_t)s.W + x : (ptrdiff_t)-1;
+}
+
+// ------------------------------------------------------------------------------------------------------------
+// Fast mode
+// ------------------------------------------------------------------------------------------------------------
+
+__device__ __forceinline__ float scaled(float g, float w) { return w * g; }
+__device__ __forceinline__ float4 scaled(const float4& g, float w) { return make_float4(w * g.x, w * g.y, w * g.z, 0.f); }
+
+// The trilinear cell of one fast-mode sample point.  Corner values are per channel plane (float) or per voxel of an
+// interleaved field (float4); the blend and gradient take scalars.
+template <bool IS3D>
+struct FastCell {
+  int x0, y0, z0;                // integer corner
+  float tx, ty, tz;              // fractions
+  bool inx[2], iny[2], inz[2];   // is the lower / upper tap of each axis inside the volume
+  int ox[2], oy[2], oz[2];       // clamped per-axis offsets (always loadable; rows and planes pre-multiplied)
+  bool interior;                 // all 8 corners inside: they lie at base + step(k)
+  int base, W, HW;
+
+  __device__ __forceinline__ int off(int k) const { return oz[k >> 2] + oy[(k >> 1) & 1] + ox[k & 1]; }
+  __device__ __forceinline__ int step(int k) const { return (k & 1) + ((k >> 1) & 1) * W + (k >> 2) * HW; }
+  __device__ __forceinline__ bool inside(int k) const { return inz[k >> 2] && iny[(k >> 1) & 1] && inx[k & 1]; }
+  __device__ __forceinline__ float weight(int k) const {
+    const float wx = (k & 1) ? tx : 1.f - tx, wy = (k & 2) ? ty : 1.f - ty;
+    return IS3D ? ((k & 4) ? tz : 1.f - tz) * wy * wx : wy * wx;
+  }
+
+  // the corner values of a plane that is not written during the launch, 0 outside the volume
+  template <class T>
+  __device__ __forceinline__ void fetch(const T* __restrict__ plane, T (&u)[8]) const {
+    if (interior) {
+      const T* s = plane + base;
+#pragma unroll
+      for (int k = 0; k < (IS3D ? 8 : 4); ++k) u[k] = __ldg(s + step(k));
+    } else {
+#pragma unroll
+      for (int k = 0; k < (IS3D ? 8 : 4); ++k) u[k] = inside(k) ? __ldg(plane + off(k)) : T();
+    }
+  }
+
+  // three nested lerps: along x, then y, then z
+  __device__ __forceinline__ float blend(const float (&u)[8]) const {
+    const float r0 = fmaf(tx, u[1] - u[0], u[0]), r1 = fmaf(tx, u[3] - u[2], u[2]);
+    float v = fmaf(ty, r1 - r0, r0);
+    if (IS3D) {
+      const float q0 = fmaf(tx, u[5] - u[4], u[4]), q1 = fmaf(tx, u[7] - u[6], u[6]);
+      const float v1 = fmaf(ty, q1 - q0, q0);
+      v = fmaf(tz, v1 - v, v);
+    }
+    return v;
+  }
+
+  // d(blend)/d(coordinate) from the same lerp tree; d/dx is lerp_z(lerp_y(upper - lower along x)), d/dy and d/dz alike
+  __device__ __forceinline__ void grad(const float (&u)[8], float& dz, float& dy, float& dx) const {
+    const float ex0 = u[1] - u[0], ex1 = u[3] - u[2];
+    const float dxa = fmaf(ty, ex1 - ex0, ex0);
+    const float ra0 = fmaf(tx, ex0, u[0]), ra1 = fmaf(tx, ex1, u[2]);
+    const float dya = ra1 - ra0;
+    if (IS3D) {
+      const float fx0 = u[5] - u[4], fx1 = u[7] - u[6];
+      const float dxb = fmaf(ty, fx1 - fx0, fx0);
+      const float rb0 = fmaf(tx, fx0, u[4]), rb1 = fmaf(tx, fx1, u[6]);
+      const float dyb = rb1 - rb0;
+      dx = fmaf(tz, dxb - dxa, dxa);
+      dy = fmaf(tz, dyb - dya, dya);
+      dz = fmaf(ty, rb1 - rb0, rb0) - fmaf(ty, ra1 - ra0, ra0);
+    } else {
+      dx = dxa;
+      dy = dya;
+      dz = 0.f;
+    }
+  }
+
+  // d(blend)/d(plane): adds weight(k) * go to every corner inside the volume (fp32 atomics; a float4 adjoint is one
+  // red.global.add.v4.f32 per corner)
+  template <class T>
+  __device__ __forceinline__ void scatter(T* plane, const T& go) const {
+    if (interior) {
+      T* s = plane + base;
+#pragma unroll
+      for (int k = 0; k < (IS3D ? 8 : 4); ++k) atomicAdd(s + step(k), scaled(go, weight(k)));
+    } else {
+#pragma unroll
+      for (int k = 0; k < (IS3D ? 8 : 4); ++k)
+        if (inside(k)) atomicAdd(plane + off(k), scaled(go, weight(k)));
+    }
+  }
+
+  // VecInt's branch-free blend of the float4 values at the clamped offsets off(k): every tap is weighted by (1 - t, t),
+  // or 0 outside the volume, so interior and border voxels run the same code and the gathers of several voxels can be
+  // in flight together
+  __device__ __forceinline__ float4 weighted_blend(const float4 (&u)[8]) const {
+    const float wx[2] = {inx[0] ? 1.f - tx : 0.f, inx[1] ? tx : 0.f};
+    const float wy[2] = {iny[0] ? 1.f - ty : 0.f, iny[1] ? ty : 0.f};
+    const float wz[2] = {inz[0] ? 1.f - tz : 0.f, inz[1] ? tz : 0.f};
+    float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int zz = 0; zz < 2; ++zz) {
+      float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int yy = 0; yy < 2; ++yy) {
+        const float4& a = u[zz * 4 + yy * 2], & b = u[zz * 4 + yy * 2 + 1];
+        const float qx = fmaf(wx[1], b.x, wx[0] * a.x), qy = fmaf(wx[1], b.y, wx[0] * a.y), qz = fmaf(wx[1], b.z, wx[0] * a.z);
+        p.x = fmaf(wy[yy], qx, p.x); p.y = fmaf(wy[yy], qy, p.y); p.z = fmaf(wy[yy], qz, p.z);
+      }
+      r.x = fmaf(wz[zz], p.x, r.x); r.y = fmaf(wz[zz], p.y, r.y); r.z = fmaf(wz[zz], p.z, r.z);
+    }
+    return r;
+  }
+};
+
+template <bool IS3D>
+__device__ __forceinline__ FastCell<IS3D> fast_cell(float cz, float cy, float cx, int D, int H, int W) {
+  FastCell<IS3D> c;
+  const float fx = floorf(cx), fy = floorf(cy), fz = IS3D ? floorf(cz) : 0.f;
+  c.x0 = f2i(fx); c.y0 = f2i(fy); c.z0 = IS3D ? f2i(fz) : 0;
+  c.tx = cx - fx; c.ty = cy - fy; c.tz = IS3D ? cz - fz : 0.f;
+  c.inx[0] = (unsigned)c.x0 < (unsigned)W; c.inx[1] = (unsigned)(c.x0 + 1) < (unsigned)W;
+  c.iny[0] = (unsigned)c.y0 < (unsigned)H; c.iny[1] = (unsigned)(c.y0 + 1) < (unsigned)H;
+  c.inz[0] = !IS3D || (unsigned)c.z0 < (unsigned)D; c.inz[1] = IS3D && (unsigned)(c.z0 + 1) < (unsigned)D;
+  c.W = W; c.HW = H * W;
+  c.ox[0] = min(max(c.x0, 0), W - 1); c.ox[1] = min(max(c.x0, -1) + 1, W - 1);
+  c.oy[0] = min(max(c.y0, 0), H - 1) * W; c.oy[1] = min(max(c.y0, -1) + 1, H - 1) * W;
+  c.oz[0] = IS3D ? min(max(c.z0, 0), D - 1) * c.HW : 0; c.oz[1] = IS3D ? min(max(c.z0, -1) + 1, D - 1) * c.HW : 0;
+  c.interior = (unsigned)c.x0 < (unsigned)(W - 1) && (unsigned)c.y0 < (unsigned)(H - 1) &&
+               (!IS3D || (unsigned)c.z0 < (unsigned)(D - 1));
+  c.base = (c.z0 * H + c.y0) * W + c.x0;
+  return c;
 }
 
 }  // namespace vxm

@@ -4,12 +4,11 @@
 // grid_sample, add).  Here ALL nsteps squarings run in ONE cooperative launch: a persistent grid
 // walks the field, `grid.sync()` separates the steps, and the (B,nd,D,H,W) field (10.3 MB at
 // 80x96x112) stays L2-resident between steps.  The backward runs the reversed chain in one
-// cooperative launch as well.
+// cooperative launch as well.  The trilinear arithmetic of both paths lives in sampler.cuh.
 //
 // Algorithmic bytes (fp32) per voxel per step: forward 4*nd read + 4*nd write;
 // backward 4*nd (v_k) + 4*nd (g_{k+1}) read + 4*nd (g_k) write.
 #include <cooperative_groups.h>
-#include <stdlib.h>
 
 #include "sampler.cuh"
 
@@ -24,29 +23,11 @@ struct VecGeom {
   size_t N;  // B * nd * DHW
 };
 
-template <bool IS3D, int ARITH>
-__device__ __forceinline__ void field_coords(const float* __restrict__ fb, size_t p, int x, int y, int z,
-                                             const VecGeom& g, float fv[3], float& cx, float& cy, float& cz) {
-  // fv[i]: the field's own value at p (channel order: D,H,W for 3-D; H,W for 2-D)
-  if (IS3D) {
-    fv[0] = fb[p]; fv[1] = fb[p + g.vol.DHW]; fv[2] = fb[p + 2 * g.vol.DHW];
-    cz = sample_coord<ARITH>((float)z, fv[0], g.az);
-    cy = sample_coord<ARITH>((float)y, fv[1], g.ay);
-    cx = sample_coord<ARITH>((float)x, fv[2], g.ax);
-  } else {
-    fv[0] = fb[p]; fv[1] = fb[p + g.vol.DHW]; fv[2] = 0.f;
-    cz = 0.f;
-    cy = sample_coord<ARITH>((float)y, fv[0], g.ay);
-    cx = sample_coord<ARITH>((float)x, fv[1], g.ax);
-  }
-}
-
 // step == -1: scaling pass; 0 <= step < nsteps: one squaring
 template <bool IS3D, int ARITH>
 __global__ void __launch_bounds__(256) vecint_fwd_kernel(const float* __restrict__ vel, float* out,
                                                          float* states, float* work, VecGeom g,
-                                                         int nsteps, int step_begin, int step_end,
-                                                         float scale, int coop) {
+                                                         int nsteps, float scale) {
   cg::grid_group grid = cg::this_grid();
   const size_t tid0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
@@ -56,7 +37,7 @@ __global__ void __launch_bounds__(256) vecint_fwd_kernel(const float* __restrict
     if (states) return states + (size_t)k * g.N;
     return ((nsteps - k) & 1) ? work : out;
   };
-  for (int s = step_begin; s < step_end; ++s) {
+  for (int s = -1; s < nsteps; ++s) {
     if (s < 0) {
       float* dst = buf(0);
       for (size_t i = tid0; i < g.N; i += stride) dst[i] = __fmul_rn(vel[i], scale);
@@ -70,19 +51,18 @@ __global__ void __launch_bounds__(256) vecint_fwd_kernel(const float* __restrict
         int r = (int)(p - (size_t)z * g.vol.HW);
         int y = r / g.vol.W, x = r - y * g.vol.W;
         const float* fb = cur + (size_t)b * g.nd * g.vol.DHW;
-        float fv[3], cx, cy, cz;
-        field_coords<IS3D, ARITH>(fb, p, x, y, z, g, fv, cx, cy, cz);
-        Stencil8 st;
-        make_stencil8<IS3D>(cx, cy, cz, g.vol.D, g.vol.H, g.vol.W, st);
+        float fv[3], cz, cy, cx;
+        exact_coords<IS3D, ARITH>(fb + p, g.vol.DHW, z, y, x, g, fv, cz, cy, cx);
+        const ExactCell<IS3D> cell = exact_cell<IS3D>(cz, cy, cx, g.vol.D, g.vol.H, g.vol.W);
         float* ob = nxt + (size_t)b * g.nd * g.vol.DHW + p;
 #pragma unroll
         for (int c = 0; c < (IS3D ? 3 : 2); ++c) {
           // plain (coherent) loads: `cur` was written earlier in this same launch
-          ob[(size_t)c * g.vol.DHW] = __fadd_rn(fv[c], sample8<IS3D, false>(fb + (size_t)c * g.vol.DHW, st));
+          ob[(size_t)c * g.vol.DHW] = __fadd_rn(fv[c], exact_sample<IS3D, false>(fb + (size_t)c * g.vol.DHW, cell));
         }
       }
     }
-    if (coop && s + 1 < step_end) grid.sync();
+    if (s + 1 < nsteps) grid.sync();
   }
 }
 
@@ -93,17 +73,15 @@ template <bool IS3D, int ARITH>
 __global__ void __launch_bounds__(256) vecint_bwd_kernel(const float* __restrict__ gout,
                                                          const float* __restrict__ states,
                                                          float* grad_vel, float* work, VecGeom g,
-                                                         int nsteps, int item_begin, int item_end,
-                                                         float scale, float mz, float my, float mx, int coop) {
+                                                         int nsteps, float scale, float mz, float my, float mx) {
   cg::grid_group grid = cg::this_grid();
   const size_t tid0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t nvox = (size_t)g.B * g.vol.DHW;
   constexpr int NCH = IS3D ? 3 : 2;
-  constexpr int NC = IS3D ? 8 : 4;
   // work items: for k = nsteps-1 .. 0: (phase 0, phase 1); then the final scaling pass
   // item index it = 2*(nsteps-1-k) + phase, final = 2*nsteps
-  for (int it = item_begin; it < item_end; ++it) {
+  for (int it = 0; it <= 2 * nsteps; ++it) {
     if (it == 2 * nsteps) {
       const float* G0 = nsteps == 0 ? gout : (((nsteps - 1) & 1) ? work + g.N : work);
       for (size_t i = tid0; i < g.N; i += stride) grad_vel[i] = G0[i] * scale;
@@ -120,30 +98,21 @@ __global__ void __launch_bounds__(256) vecint_bwd_kernel(const float* __restrict
         int r = (int)(p - (size_t)z * g.vol.HW);
         int y = r / g.vol.W, x = r - y * g.vol.W;
         const float* fb = v + (size_t)b * g.nd * g.vol.DHW;
-        float fv[3], cx, cy, cz;
-        field_coords<IS3D, ARITH>(fb, p, x, y, z, g, fv, cx, cy, cz);
-        Stencil st = make_stencil<IS3D>(cx, cy, cz, g.vol);
-        ptrdiff_t base = corner_offset(st, 0, g.vol);
+        float fv[3], cz, cy, cx;
+        exact_coords<IS3D, ARITH>(fb + p, g.vol.DHW, z, y, x, g, fv, cz, cy, cx);
+        const ExactCell<IS3D> cell = exact_cell<IS3D>(cz, cy, cx, g.vol.D, g.vol.H, g.vol.W);
         const float* gnb = gn + (size_t)b * g.nd * g.vol.DHW + p;
         float go[NCH];
 #pragma unroll
         for (int c = 0; c < NCH; ++c) go[c] = gnb[(size_t)c * g.vol.DHW];
         if (phase == 0) {
           float gx = 0.f, gy = 0.f, gz = 0.f;
+          exact_grad(cell, [&](int off) {
+            float vg = 0.f;
 #pragma unroll
-          for (int kk = 0; kk < NC; ++kk) {
-            if (st.mask & (1u << kk)) {
-              ptrdiff_t off = base + ((kk >> 2) & 1) * (ptrdiff_t)g.vol.HW + ((kk >> 1) & 1) * (ptrdiff_t)g.vol.W + (kk & 1);
-              float wx = (kk & 1) ? st.wx1 : st.wx0, wy = (kk & 2) ? st.wy1 : st.wy0;
-              float wz = IS3D ? ((kk & 4) ? st.wz1 : st.wz0) : 1.0f;
-              float vg = 0.f;
-#pragma unroll
-              for (int c = 0; c < NCH; ++c) vg += __ldg(fb + (size_t)c * g.vol.DHW + off) * go[c];
-              gx += ((kk & 1) ? vg : -vg) * wy * wz;
-              gy += ((kk & 2) ? vg : -vg) * wx * wz;
-              if (IS3D) gz += ((kk & 4) ? vg : -vg) * wx * wy;
-            }
-          }
+            for (int c = 0; c < NCH; ++c) vg += __ldg(fb + (size_t)c * g.vol.DHW + off) * go[c];
+            return vg;
+          }, gz, gy, gx);
           float* gcb = gc + (size_t)b * g.nd * g.vol.DHW + p;
           if (IS3D) {
             gcb[0] = go[0] + gz * mz;
@@ -156,18 +125,11 @@ __global__ void __launch_bounds__(256) vecint_bwd_kernel(const float* __restrict
         } else {
           float* gcb = gc + (size_t)b * g.nd * g.vol.DHW;
 #pragma unroll
-          for (int kk = 0; kk < NC; ++kk) {
-            if (st.mask & (1u << kk)) {
-              ptrdiff_t off = base + ((kk >> 2) & 1) * (ptrdiff_t)g.vol.HW + ((kk >> 1) & 1) * (ptrdiff_t)g.vol.W + (kk & 1);
-              float w = corner_weight<IS3D>(st, kk);
-#pragma unroll
-              for (int c = 0; c < NCH; ++c) atomicAdd(gcb + (size_t)c * g.vol.DHW + off, w * go[c]);
-            }
-          }
+          for (int c = 0; c < NCH; ++c) exact_scatter(cell, gcb + (size_t)c * g.vol.DHW, go[c]);
         }
       }
     }
-    if (coop && it + 1 < item_end) grid.sync();
+    if (it < 2 * nsteps) grid.sync();
   }
 }
 
@@ -176,8 +138,8 @@ __global__ void __launch_bounds__(256) vecint_bwd_kernel(const float* __restrict
 //  * the field lives in an INTERLEAVED float4 (z, y, x, 0) layout inside the launch: a squaring step is one
 //    16-byte own load, eight 16-byte gathers and one 16-byte store per voxel instead of 3 + 24 + 3 four-byte
 //    accesses (the planar layout is only read in the scaling pass and written by the last step);
-//  * coordinates are p + v directly (no replay of the reference's normalise / un-normalise round trip), the blend
-//    is a lerp tree, interior voxels take a predicate-free branch (see warp.cu);
+//  * coordinates are p + v directly (no replay of the reference's normalise / un-normalise round trip), and the cell
+//    is sampler.cuh's FastCell, as in the fast warp;
 //  * the backward scatters d/d(src) with ONE red.global.add.v4.f32 per corner (8 + 1 vector reductions per voxel
 //    and step instead of 24 scalar atomics), rotating three float4 gradient buffers so that every step is one
 //    phase (one grid.sync) instead of two.
@@ -205,92 +167,11 @@ struct VecFast {
   FastDiv dW, dH, dD;
 };
 
-struct Corner8 {
-  bool interior;
-  int base;            // interior: offset of corner (z0,y0,x0)
-  int off[8];          // border: clamped offsets
-  float w[8];          // border: weights (0 outside the volume)
-  unsigned ok;         // border: bit k set <=> corner k inside the volume
-  float tx, ty, tz;
-};
-
-__device__ __forceinline__ void corners_fast(float cz, float cy, float cx, const VecFast& g, Corner8& c) {
-  const float fx = floorf(cx), fy = floorf(cy), fz = floorf(cz);
-  const int x0 = f2i(fx), y0 = f2i(fy), z0 = f2i(fz);
-  c.tx = cx - fx; c.ty = cy - fy; c.tz = cz - fz;
-  c.interior = (unsigned)x0 < (unsigned)(g.W - 1) && (unsigned)y0 < (unsigned)(g.H - 1) && (unsigned)z0 < (unsigned)(g.D - 1);
-  c.base = (z0 * g.H + y0) * g.W + x0;
-  if (!c.interior) {
-    const float wx[2] = {(unsigned)x0 < (unsigned)g.W ? 1.f - c.tx : 0.f, (unsigned)(x0 + 1) < (unsigned)g.W ? c.tx : 0.f};
-    const float wy[2] = {(unsigned)y0 < (unsigned)g.H ? 1.f - c.ty : 0.f, (unsigned)(y0 + 1) < (unsigned)g.H ? c.ty : 0.f};
-    const float wz[2] = {(unsigned)z0 < (unsigned)g.D ? 1.f - c.tz : 0.f, (unsigned)(z0 + 1) < (unsigned)g.D ? c.tz : 0.f};
-    const int xo[2] = {min(max(x0, 0), g.W - 1), min(max(x0 + 1, 0), g.W - 1)};
-    const int yo[2] = {min(max(y0, 0), g.H - 1) * g.W, min(max(y0 + 1, 0), g.H - 1) * g.W};
-    const int zo[2] = {min(max(z0, 0), g.D - 1) * g.HW, min(max(z0 + 1, 0), g.D - 1) * g.HW};
-    const bool vx[2] = {(unsigned)x0 < (unsigned)g.W, (unsigned)(x0 + 1) < (unsigned)g.W};
-    const bool vy[2] = {(unsigned)y0 < (unsigned)g.H, (unsigned)(y0 + 1) < (unsigned)g.H};
-    const bool vz[2] = {(unsigned)z0 < (unsigned)g.D, (unsigned)(z0 + 1) < (unsigned)g.D};
-    c.ok = 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      c.off[k] = zo[k >> 2] + yo[(k >> 1) & 1] + xo[k & 1];
-      c.w[k] = wz[k >> 2] * wy[(k >> 1) & 1] * wx[k & 1];
-      c.ok |= (vz[k >> 2] && vy[(k >> 1) & 1] && vx[k & 1]) ? (1u << k) : 0u;
-    }
-  }
-}
-
-// Branch-free trilinear footprint of one sample point: clamped corner offsets (always loadable) and per-axis weights with
-// the zeros padding folded in (a corner outside the volume has weight 0), so interior and border voxels run the same code
-// and the gathers of several voxels can be in flight together.
-struct Foot {
-  int oz[2], oy[2], ox[2];     // clamped offsets of the two planes / rows / columns
-  float wz[2], wy[2], wx[2];   // (1 - t, t) or 0 where the plane / row / column lies outside the volume
-  float vz[2], vy[2], vx[2];   // 1 / 0 validity (the derivative of w with respect to the coordinate is -v[0], +v[1])
-  int key;                     // (z0 * H + y0) * W + x0 when all 8 corners are inside, else -1
-};
-__device__ __forceinline__ void footprint(float cz, float cy, float cx, const VecFast& g, Foot& f) {
-  const float fx = floorf(cx), fy = floorf(cy), fz = floorf(cz);
-  const int x0 = f2i(fx), y0 = f2i(fy), z0 = f2i(fz);
-  const float tx = cx - fx, ty = cy - fy, tz = cz - fz;
-  const bool bx0 = (unsigned)x0 < (unsigned)g.W, bx1 = (unsigned)(x0 + 1) < (unsigned)g.W;
-  const bool by0 = (unsigned)y0 < (unsigned)g.H, by1 = (unsigned)(y0 + 1) < (unsigned)g.H;
-  const bool bz0 = (unsigned)z0 < (unsigned)g.D, bz1 = (unsigned)(z0 + 1) < (unsigned)g.D;
-  f.vx[0] = bx0 ? 1.f : 0.f; f.vx[1] = bx1 ? 1.f : 0.f;
-  f.vy[0] = by0 ? 1.f : 0.f; f.vy[1] = by1 ? 1.f : 0.f;
-  f.vz[0] = bz0 ? 1.f : 0.f; f.vz[1] = bz1 ? 1.f : 0.f;
-  f.wx[0] = bx0 ? 1.f - tx : 0.f; f.wx[1] = bx1 ? tx : 0.f;
-  f.wy[0] = by0 ? 1.f - ty : 0.f; f.wy[1] = by1 ? ty : 0.f;
-  f.wz[0] = bz0 ? 1.f - tz : 0.f; f.wz[1] = bz1 ? tz : 0.f;
-  f.ox[0] = min(max(x0, 0), g.W - 1); f.ox[1] = min(max(x0 + 1, 0), g.W - 1);
-  f.oy[0] = min(max(y0, 0), g.H - 1) * g.W; f.oy[1] = min(max(y0 + 1, 0), g.H - 1) * g.W;
-  f.oz[0] = min(max(z0, 0), g.D - 1) * g.HW; f.oz[1] = min(max(z0 + 1, 0), g.D - 1) * g.HW;
-  f.key = (bx0 && bx1 && by0 && by1 && bz0 && bz1) ? (z0 * g.H + y0) * g.W + x0 : -1;
-}
-__device__ __forceinline__ void gather8(const float4* __restrict__ cb, const Foot& f, float4 (&u)[8]) {
-#pragma unroll
-  for (int k = 0; k < 8; ++k) u[k] = cb[f.oz[k >> 2] + f.oy[(k >> 1) & 1] + f.ox[k & 1]];
-}
-__device__ __forceinline__ float4 blend8(const Foot& f, const float4 (&u)[8]) {
-  float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-  for (int zz = 0; zz < 2; ++zz) {
-    float4 p = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int yy = 0; yy < 2; ++yy) {
-      const float4& a = u[zz * 4 + yy * 2], & b = u[zz * 4 + yy * 2 + 1];
-      const float qx = fmaf(f.wx[1], b.x, f.wx[0] * a.x), qy = fmaf(f.wx[1], b.y, f.wx[0] * a.y), qz = fmaf(f.wx[1], b.z, f.wx[0] * a.z);
-      p.x = fmaf(f.wy[yy], qx, p.x); p.y = fmaf(f.wy[yy], qy, p.y); p.z = fmaf(f.wy[yy], qz, p.z);
-    }
-    r.x = fmaf(f.wz[zz], p.x, r.x); r.y = fmaf(f.wz[zz], p.y, r.y); r.z = fmaf(f.wz[zz], p.z, r.z);
-  }
-  return r;
-}
-
-// Work decomposition of both fast kernels: the field is cut into 512-voxel blocks; CTA c owns the contiguous run of blocks
+// Work decomposition of the forward: the field is cut into 512-voxel blocks; CTA c owns the contiguous run of blocks
 // [c * nblk / grid, (c + 1) * nblk / grid) (so consecutive iterations of a CTA touch neighbouring rows: L1 reuse), and a thread
 // carries TWO voxels (blocks blk, blk + 1) per iteration with all 16 gathers in flight — at 16 warps per SM the kernel is bound by
-// the L2 round trip of its gathers otherwise.
+// the L2 round trip of its gathers otherwise.  The gathers read the clamped corners of FastCell and blend them with its
+// branch-free weighted_blend, so interior and border voxels issue the same loads.
 // SAVE: every intermediate field v_0 .. v_{n-1} is kept (states, for the backward); otherwise two buffers ping-pong
 template <bool SAVE>
 __global__ void __launch_bounds__(512) vecint_fwd_fast_kernel(const float* __restrict__ vel, float* __restrict__ out, float4* buf,
@@ -320,9 +201,8 @@ __global__ void __launch_bounds__(512) vecint_fwd_fast_kernel(const float* __res
       int q[2];
       bool has[2];
       float4 v[2];
-      Foot f[2];
+      FastCell<true> f[2];
       float4 u[2][8];
-      const float4* cb[2];
       int bb[2];
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
@@ -337,13 +217,14 @@ __global__ void __launch_bounds__(512) vecint_fwd_fast_kernel(const float* __res
         const int t2 = fdiv(t1, g.dH), y = t1 - t2 * g.H;
         const int b = fdiv(t2, g.dD), z = t2 - b * g.D;
         bb[e] = b;
-        cb[e] = cur + (size_t)b * g.DHW;
-        footprint((float)z + v[e].x, (float)y + v[e].y, (float)x + v[e].z, g, f[e]);
-        gather8(cb[e], f[e], u[e]);
+        const float4* cb = cur + (size_t)b * g.DHW;
+        f[e] = fast_cell<true>((float)z + v[e].x, (float)y + v[e].y, (float)x + v[e].z, g.D, g.H, g.W);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) u[e][k] = cb[f[e].off(k)];
       }
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const float4 r = blend8(f[e], u[e]);
+        const float4 r = f[e].weighted_blend(u[e]);
         const float4 o = make_float4(v[e].x + r.x, v[e].y + r.y, v[e].z + r.z, 0.f);
         if (has[e]) {
           if (last) {
@@ -360,21 +241,18 @@ __global__ void __launch_bounds__(512) vecint_fwd_fast_kernel(const float* __res
   }
 }
 
-// three rotating float4 gradient buffers G[0..2] (work): step j reads G[j%3], reduces into G[(j+1)%3] (zero on entry)
-// and zeroes G[(j+2)%3] for the step after.
+// The backward walks the field grid-stride, loading the next voxel's own data ahead of this one's gathers.  Three rotating
+// float4 gradient buffers G[0..2] (work): step j reads G[j%3], reduces into G[(j+1)%3] (zero on entry) and zeroes G[(j+2)%3]
+// for the step after.
 __global__ void __launch_bounds__(512) vecint_bwd_fast_kernel(const float* __restrict__ gout, const float4* __restrict__ states,
-                                                              float* __restrict__ grad_vel, float4* G, VecFast g, int nsteps, float scale, int dbg) {
+                                                              float* __restrict__ grad_vel, float4* G, VecFast g, int nsteps, float scale) {
   cg::grid_group grid = cg::this_grid();
-  // voxel walk: grid-stride (default), or — dbg & 2, profiling A/B — a contiguous run of 512-voxel blocks per CTA
-  const int nblk = (g.nvox + 511) >> 9;
-  const bool contig = dbg & 2;
-  const int tid0 = contig ? (((int)((long long)blockIdx.x * nblk / gridDim.x)) << 9) + (int)threadIdx.x : (int)(blockIdx.x * blockDim.x + threadIdx.x);
-  const int stride = contig ? 512 : (int)(gridDim.x * blockDim.x);
-  const int qend = contig ? min(g.nvox, ((int)((long long)(blockIdx.x + 1) * nblk / gridDim.x)) << 9) : g.nvox;
+  const int tid0 = (int)(blockIdx.x * blockDim.x + threadIdx.x);
+  const int stride = (int)(gridDim.x * blockDim.x);
   float4* G0 = G;
   float4* G1 = G + (size_t)g.nvox;
   float4* G2 = G + 2 * (size_t)g.nvox;
-  for (int q = tid0; q < qend; q += stride) {
+  for (int q = tid0; q < g.nvox; q += stride) {
     const int b = q / g.DHW, p = q - b * g.DHW;
     const float* gb = gout + (size_t)b * 3 * g.DHW + p;
     G0[q] = make_float4(__ldg(gb), __ldg(gb + g.DHW), __ldg(gb + 2 * g.DHW), 0.f);
@@ -388,65 +266,31 @@ __global__ void __launch_bounds__(512) vecint_bwd_fast_kernel(const float* __res
     float4* gc = j % 3 == 0 ? G1 : (j % 3 == 1 ? G2 : G0);
     float4* __restrict__ gz = j % 3 == 0 ? G2 : (j % 3 == 1 ? G0 : G1);
     float4 own_next = make_float4(0.f, 0.f, 0.f, 0.f), go_next = own_next;
-    if (tid0 < qend) { own_next = v[tid0]; go_next = gn[tid0]; }
-    for (int q = tid0; q < qend; q += stride) {
+    if (tid0 < g.nvox) { own_next = v[tid0]; go_next = gn[tid0]; }
+    for (int q = tid0; q < g.nvox; q += stride) {
       const int t1 = fdiv(q, g.dW), x = q - t1 * g.W;
       const int t2 = fdiv(t1, g.dH), y = t1 - t2 * g.H;
       const int b = fdiv(t2, g.dD), z = t2 - b * g.D;
-      const float4* vb = v + (size_t)b * g.DHW;
-      float4* gcb = gc + (size_t)b * g.DHW;
       const float4 own = own_next;
       const float4 go = go_next;
-      if (q + stride < qend) { own_next = v[q + stride]; go_next = gn[q + stride]; }   // next iteration's own data, ahead of this one's gathers
+      if (q + stride < g.nvox) { own_next = v[q + stride]; go_next = gn[q + stride]; }   // next iteration's own data, ahead of this one's gathers
       gz[q] = make_float4(0.f, 0.f, 0.f, 0.f);
-      Corner8 c;
-      corners_fast((float)z + own.x, (float)y + own.y, (float)x + own.z, g, c);
-      float dz, dy, dx;
-      if (c.interior) {
-        const float4* s0 = vb + c.base;
-        float4* t0 = gcb + c.base;
-        const float4 a00 = s0[0], a01 = s0[1], a10 = s0[g.W], a11 = s0[g.W + 1];
-        const float4 b00 = s0[g.HW], b01 = s0[g.HW + 1], b10 = s0[g.HW + g.W], b11 = s0[g.HW + g.W + 1];
-        // <corner, go>: the scalar field whose position-gradient is the flow gradient of this voxel
-        auto dot = [&](const float4& u) { return fmaf(u.x, go.x, fmaf(u.y, go.y, u.z * go.z)); };
-        const float s000 = dot(a00), s001 = dot(a01), s010 = dot(a10), s011 = dot(a11);
-        const float s100 = dot(b00), s101 = dot(b01), s110 = dot(b10), s111 = dot(b11);
-        const float ra0 = fmaf(c.tx, s001 - s000, s000), ra1 = fmaf(c.tx, s011 - s010, s010);
-        const float rb0 = fmaf(c.tx, s101 - s100, s100), rb1 = fmaf(c.tx, s111 - s110, s110);
-        const float dxa = fmaf(c.ty, (s011 - s010) - (s001 - s000), s001 - s000), dxb = fmaf(c.ty, (s111 - s110) - (s101 - s100), s101 - s100);
-        dx = fmaf(c.tz, dxb - dxa, dxa);
-        const float dya = ra1 - ra0, dyb = rb1 - rb0;
-        dy = fmaf(c.tz, dyb - dya, dya);
-        dz = fmaf(c.ty, rb1 - rb0, rb0) - fmaf(c.ty, ra1 - ra0, ra0);
-        const float wx0 = 1.f - c.tx, wy0 = 1.f - c.ty, wz0 = 1.f - c.tz;
-        auto red = [&](float4* t, float w) { atomicAdd(t, make_float4(w * go.x, w * go.y, w * go.z, 0.f)); };
-        red(t0, wz0 * wy0 * wx0); red(t0 + 1, wz0 * wy0 * c.tx);
-        red(t0 + g.W, wz0 * c.ty * wx0); red(t0 + g.W + 1, wz0 * c.ty * c.tx);
-        red(t0 + g.HW, c.tz * wy0 * wx0); red(t0 + g.HW + 1, c.tz * wy0 * c.tx);
-        red(t0 + g.HW + g.W, c.tz * c.ty * wx0); red(t0 + g.HW + g.W + 1, c.tz * c.ty * c.tx);
-      } else {
-        // border: only in-volume corners carry a value (zeros padding) and receive gradient
-        const float fx = c.tx, fy = c.ty, fz = c.tz;
-        dz = dy = dx = 0.f;
+      const FastCell<true> cell = fast_cell<true>((float)z + own.x, (float)y + own.y, (float)x + own.z, g.D, g.H, g.W);
+      float4 u[8];
+      cell.fetch(v + (size_t)b * g.DHW, u);
+      // <corner, go>: the scalar field whose position-gradient is the flow gradient of this voxel
+      float s[8];
 #pragma unroll
-        for (int k = 0; k < 8; ++k) {
-          if (c.ok & (1u << k)) {
-            const float4 u = vb[c.off[k]];
-            const float sk = fmaf(u.x, go.x, fmaf(u.y, go.y, u.z * go.z));
-            const float wx = (k & 1) ? fx : 1.f - fx, wy = (k & 2) ? fy : 1.f - fy, wz = (k & 4) ? fz : 1.f - fz;
-            dx += ((k & 1) ? sk : -sk) * wy * wz;
-            dy += ((k & 2) ? sk : -sk) * wx * wz;
-            dz += ((k & 4) ? sk : -sk) * wx * wy;
-            atomicAdd(gcb + c.off[k], make_float4(c.w[k] * go.x, c.w[k] * go.y, c.w[k] * go.z, 0.f));
-          }
-        }
-      }
+      for (int c = 0; c < 8; ++c) s[c] = fmaf(u[c].x, go.x, fmaf(u[c].y, go.y, u[c].z * go.z));
+      float dz, dy, dx;
+      cell.grad(s, dz, dy, dx);
+      cell.scatter(gc + (size_t)b * g.DHW, go);
       atomicAdd(gc + q, make_float4(go.x + dz, go.y + dy, go.z + dx, 0.f));
     }
     grid.sync();
   }
   const float4* Gf = nsteps % 3 == 0 ? G0 : (nsteps % 3 == 1 ? G1 : G2);
-  for (int q = tid0; q < qend; q += stride) {
+  for (int q = tid0; q < g.nvox; q += stride) {
     const int b = q / g.DHW, p = q - b * g.DHW;
     const float4 r = Gf[q];
     float* o = grad_vel + (size_t)b * 3 * g.DHW + p;
@@ -479,8 +323,9 @@ static VecGeom make_vgeom(int B, int D, int H, int W, int nd) {
   return g;
 }
 
+// grid of a cooperative launch: as many CTAs as fit on the device at once, but no more than max_ctas
 template <typename K>
-static int coop_grid(K kernel, int threads, size_t work_items, int* grid_out) {
+static int coop_grid(K kernel, int threads, size_t max_ctas, int* grid_out) {
   int dev = 0, nsm = 0, coop = 0, per_sm = 0;
   VXM_CUDA(cudaGetDevice(&dev));
   VXM_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
@@ -490,9 +335,8 @@ static int coop_grid(K kernel, int threads, size_t work_items, int* grid_out) {
     set_error("vecint: cooperative launch unavailable on this device");
     return VXM_ERR_UNSUPPORTED;
   }
-  size_t need = (work_items + threads - 1) / threads;
-  size_t cap = (size_t)nsm * per_sm;
-  *grid_out = (int)(need < cap ? (need ? need : 1) : cap);
+  const size_t cap = (size_t)nsm * per_sm;
+  *grid_out = (int)(max_ctas < cap ? max_ctas : cap);
   return VXM_OK;
 }
 
@@ -512,24 +356,9 @@ extern "C" size_t vxm_vecint_fast_work_bytes(int B, int D, int H, int W, int bac
   return (size_t)(backward ? 3 : 2) * B * D * H * W * sizeof(float4);
 }
 
-template <typename K>
-static int coop_grid_fast(K kernel, int threads, int* grid_out) {
-  int dev = 0, nsm = 0, coop = 0, per_sm = 0;
-  VXM_CUDA(cudaGetDevice(&dev));
-  VXM_CUDA(cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev));
-  VXM_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  VXM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, 0));
-  if (!coop || per_sm < 1) {
-    set_error("vecint: cooperative launch unavailable on this device");
-    return VXM_ERR_UNSUPPORTED;
-  }
-  *grid_out = nsm * per_sm;
-  return VXM_OK;
-}
-
 extern "C" int vxm_debug_gridsync(int nsync, int ctas_per_sm, void* stream) {
   int grid = 0;
-  int rc = coop_grid_fast(gridsync_probe_kernel, 512, &grid);
+  int rc = coop_grid(gridsync_probe_kernel, 512, SIZE_MAX, &grid);
   if (rc) return rc;
   if (ctas_per_sm > 0 && ctas_per_sm * sm_count() < grid) grid = ctas_per_sm * sm_count();
   unsigned* sink = nullptr;
@@ -553,17 +382,12 @@ static int vecint_fwd_fast(const float* vel, float* out, void* states, void* wor
   VecFast g = make_vfast(B, D, H, W);
   float scale = 1.0f / (float)(1u << nsteps);
   float4* buf = (float4*)(states ? states : work);
+  auto kern = states ? vecint_fwd_fast_kernel<true> : vecint_fwd_fast_kernel<false>;
   int grid = 0;
+  rc = coop_grid(kern, 512, SIZE_MAX, &grid);
+  if (rc) return rc;
   void* args[] = {(void*)&vel, (void*)&out, (void*)&buf, (void*)&g, (void*)&nsteps, (void*)&scale};
-  if (states) {
-    rc = coop_grid_fast(vecint_fwd_fast_kernel<true>, 512, &grid);
-    if (rc) return rc;
-    VXM_CUDA(cudaLaunchCooperativeKernel((void*)vecint_fwd_fast_kernel<true>, dim3(grid), dim3(512), args, 0, st));
-  } else {
-    rc = coop_grid_fast(vecint_fwd_fast_kernel<false>, 512, &grid);
-    if (rc) return rc;
-    VXM_CUDA(cudaLaunchCooperativeKernel((void*)vecint_fwd_fast_kernel<false>, dim3(grid), dim3(512), args, 0, st));
-  }
+  VXM_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(512), args, 0, st));
   return check_launch("vecint_fwd");
 }
 
@@ -576,11 +400,9 @@ static int vecint_bwd_fast(const float* gout, const void* states, float* grad_ve
   const float4* sp = (const float4*)states;
   float4* G = (float4*)work;
   int grid = 0;
-  rc = coop_grid_fast(vecint_bwd_fast_kernel, 512, &grid);
+  rc = coop_grid(vecint_bwd_fast_kernel, 512, SIZE_MAX, &grid);
   if (rc) return rc;
-  const char* de = getenv("VXM_B200_VECINT_DBG");
-  int dbg = de ? atoi(de) : 0;
-  void* args[] = {(void*)&gout, (void*)&sp, (void*)&grad_vel, (void*)&G, (void*)&g, (void*)&nsteps, (void*)&scale, (void*)&dbg};
+  void* args[] = {(void*)&gout, (void*)&sp, (void*)&grad_vel, (void*)&G, (void*)&g, (void*)&nsteps, (void*)&scale};
   VXM_CUDA(cudaLaunchCooperativeKernel((void*)vecint_bwd_fast_kernel, dim3(grid), dim3(512), args, 0, st));
   return check_launch("vecint_bwd");
 }
@@ -590,11 +412,9 @@ static int vecint_fwd_launch(const float* vel, float* out, float* states, float*
                              int nsteps, float scale, cudaStream_t st) {
   auto kern = vecint_fwd_kernel<IS3D, ARITH>;
   int grid = 0;
-  int rc = coop_grid(kern, 256, (size_t)g.B * g.vol.DHW, &grid);
+  int rc = coop_grid(kern, 256, ((size_t)g.B * g.vol.DHW + 255) / 256, &grid);
   if (rc) return rc;
-  int sb = -1, se = nsteps, coop = 1;
-  void* args[] = {(void*)&vel, (void*)&out, (void*)&states, (void*)&work, (void*)&g,
-                  (void*)&nsteps, (void*)&sb, (void*)&se, (void*)&scale, (void*)&coop};
+  void* args[] = {(void*)&vel, (void*)&out, (void*)&states, (void*)&work, (void*)&g, (void*)&nsteps, (void*)&scale};
   VXM_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(256), args, 0, st));
   return check_launch("vecint_fwd");
 }
@@ -623,14 +443,13 @@ static int vecint_bwd_launch(const float* gout, const float* states, float* grad
                              VecGeom g, int nsteps, float scale, cudaStream_t st) {
   auto kern = vecint_bwd_kernel<IS3D, ARITH>;
   int grid = 0;
-  int rc = coop_grid(kern, 256, (size_t)g.B * g.vol.DHW, &grid);
+  int rc = coop_grid(kern, 256, ((size_t)g.B * g.vol.DHW + 255) / 256, &grid);
   if (rc) return rc;
   float mx = (g.ax.src_sm1 * 0.5f) * 2.0f / g.ax.sm1;
   float my = (g.ay.src_sm1 * 0.5f) * 2.0f / g.ay.sm1;
   float mz = IS3D ? (g.az.src_sm1 * 0.5f) * 2.0f / g.az.sm1 : 0.f;
-  int ib = 0, ie = 2 * nsteps + 1, coop = 1;
   void* args[] = {(void*)&gout, (void*)&states, (void*)&grad_vel, (void*)&work, (void*)&g, (void*)&nsteps,
-                  (void*)&ib, (void*)&ie, (void*)&scale, (void*)&mz, (void*)&my, (void*)&mx, (void*)&coop};
+                  (void*)&scale, (void*)&mz, (void*)&my, (void*)&mx};
   VXM_CUDA(cudaLaunchCooperativeKernel((void*)kern, dim3(grid), dim3(256), args, 0, st));
   return check_launch("vecint_bwd");
 }

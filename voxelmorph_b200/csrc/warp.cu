@@ -4,7 +4,7 @@
 // gather goes through the read-only path and is served by L1/L2 (neighbouring threads touch
 // neighbouring source lines because registration flows are smooth).  The identity grid the
 // reference materialises as a buffer (layers.py:17-28, 82.6 MB at 160x192x224) is never built:
-// p is the thread's own index.
+// p is the thread's own index.  The trilinear arithmetic of both paths lives in sampler.cuh.
 //
 // Algorithmic HBM bytes per output voxel (fp32): 4*C (src) + 4*nd (flow) + 4*C (out).
 #include "sampler.cuh"
@@ -19,6 +19,7 @@ struct WarpGeom {
   int B, C, nd;
 };
 
+// exact (and nearest) path: the reference's coordinate replay and ATen's corner arithmetic
 template <bool IS3D, int MODE, int ARITH>
 __global__ void __launch_bounds__(TX* TY) warp_fwd_kernel(const float* __restrict__ src,
                                                           const float* __restrict__ flow,
@@ -29,26 +30,17 @@ __global__ void __launch_bounds__(TX* TY) warp_fwd_kernel(const float* __restric
   int z = zb % g.dst.D, b = zb / g.dst.D;
   if (x >= g.dst.W || y >= g.dst.H) return;
   size_t p = ((size_t)z * g.dst.H + y) * g.dst.W + x;
-  const float* fb = flow + (size_t)b * g.nd * g.dst.DHW + p;
-  float cz = 0.f, cy, cx;
-  if (IS3D) {
-    cz = sample_coord<ARITH>((float)z, __ldg(fb), g.az);
-    cy = sample_coord<ARITH>((float)y, __ldg(fb + g.dst.DHW), g.ay);
-    cx = sample_coord<ARITH>((float)x, __ldg(fb + 2 * g.dst.DHW), g.ax);
-  } else {
-    cy = sample_coord<ARITH>((float)y, __ldg(fb), g.ay);
-    cx = sample_coord<ARITH>((float)x, __ldg(fb + g.dst.DHW), g.ax);
-  }
+  float fv[3], cz, cy, cx;
+  exact_coords<IS3D, ARITH>(flow + (size_t)b * g.nd * g.dst.DHW + p, g.dst.DHW, z, y, x, g, fv, cz, cy, cx);
   const float* sb = src + (size_t)b * g.C * g.src.DHW;
   float* ob = out + (size_t)b * g.C * g.dst.DHW + p;
   if (MODE == VXM_MODE_NEAREST) {
     ptrdiff_t idx = nearest_index<IS3D>(cx, cy, cz, g.src);
     for (int c = 0; c < g.C; ++c) ob[(size_t)c * g.dst.DHW] = idx >= 0 ? __ldg(sb + (size_t)c * g.src.DHW + idx) : 0.0f;
   } else {
-    Stencil8 st;
-    make_stencil8<IS3D>(cx, cy, cz, g.src.D, g.src.H, g.src.W, st);
+    const ExactCell<IS3D> cell = exact_cell<IS3D>(cz, cy, cx, g.src.D, g.src.H, g.src.W);
     for (int c = 0; c < g.C; ++c)
-      ob[(size_t)c * g.dst.DHW] = sample8<IS3D, true>(sb + (size_t)c * g.src.DHW, st);
+      ob[(size_t)c * g.dst.DHW] = exact_sample<IS3D, true>(sb + (size_t)c * g.src.DHW, cell);
   }
 }
 
@@ -65,16 +57,8 @@ __global__ void __launch_bounds__(TX* TY) warp_bwd_kernel(const float* __restric
   int z = zb % g.dst.D, b = zb / g.dst.D;
   if (x >= g.dst.W || y >= g.dst.H) return;
   size_t p = ((size_t)z * g.dst.H + y) * g.dst.W + x;
-  const float* fb = flow + (size_t)b * g.nd * g.dst.DHW + p;
-  float cz = 0.f, cy, cx;
-  if (IS3D) {
-    cz = sample_coord<ARITH>((float)z, __ldg(fb), g.az);
-    cy = sample_coord<ARITH>((float)y, __ldg(fb + g.dst.DHW), g.ay);
-    cx = sample_coord<ARITH>((float)x, __ldg(fb + 2 * g.dst.DHW), g.ax);
-  } else {
-    cy = sample_coord<ARITH>((float)y, __ldg(fb), g.ay);
-    cx = sample_coord<ARITH>((float)x, __ldg(fb + g.dst.DHW), g.ax);
-  }
+  float fv[3], cz, cy, cx;
+  exact_coords<IS3D, ARITH>(flow + (size_t)b * g.nd * g.dst.DHW + p, g.dst.DHW, z, y, x, g, fv, cz, cy, cx);
   const float* sb = src + (size_t)b * g.C * g.src.DHW;
   float* gsb = gsrc ? gsrc + (size_t)b * g.C * g.src.DHW : nullptr;
   const float* gob = gout + (size_t)b * g.C * g.dst.DHW + p;
@@ -84,27 +68,12 @@ __global__ void __launch_bounds__(TX* TY) warp_bwd_kernel(const float* __restric
     if (gsb && idx >= 0)
       for (int c = 0; c < g.C; ++c) atomicAdd(gsb + (size_t)c * g.src.DHW + idx, __ldg(gob + (size_t)c * g.dst.DHW));
   } else {
-    constexpr int NC = IS3D ? 8 : 4;
-    Stencil st = make_stencil<IS3D>(cx, cy, cz, g.src);
-    ptrdiff_t base = corner_offset(st, 0, g.src);
+    const ExactCell<IS3D> cell = exact_cell<IS3D>(cz, cy, cx, g.src.D, g.src.H, g.src.W);
     for (int c = 0; c < g.C; ++c) {
-      float go = __ldg(gob + (size_t)c * g.dst.DHW);
+      const float go = __ldg(gob + (size_t)c * g.dst.DHW);
       const float* plane = sb + (size_t)c * g.src.DHW;
-#pragma unroll
-      for (int k = 0; k < NC; ++k) {
-        if (st.mask & (1u << k)) {
-          ptrdiff_t off = base + ((k >> 2) & 1) * (ptrdiff_t)g.src.HW + ((k >> 1) & 1) * (ptrdiff_t)g.src.W + (k & 1);
-          float wx = (k & 1) ? st.wx1 : st.wx0, wy = (k & 2) ? st.wy1 : st.wy0;
-          float wz = IS3D ? ((k & 4) ? st.wz1 : st.wz0) : 1.0f;
-          if (gsb) atomicAdd(gsb + (size_t)c * g.src.DHW + off, corner_weight<IS3D>(st, k) * go);
-          if (gflow) {
-            float v = __ldg(plane + off) * go;
-            gx += ((k & 1) ? v : -v) * wy * wz;
-            gy += ((k & 2) ? v : -v) * wx * wz;
-            if (IS3D) gz += ((k & 4) ? v : -v) * wx * wy;
-          }
-        }
-      }
+      if (gflow) exact_grad(cell, [&](int off) { return __ldg(plane + off) * go; }, gz, gy, gx);
+      if (gsb) exact_scatter(cell, gsb + (size_t)c * g.src.DHW, go);
     }
   }
   if (gflow) {
@@ -125,10 +94,10 @@ __global__ void __launch_bounds__(TX* TY) warp_bwd_kernel(const float* __restric
 // not for a replay of torch's coordinate round trip (layers.py:37 + GridSampler.h:27-31), which costs a true
 // fp32 division and ~10 dependent roundings per axis and made the exact kernel instruction bound (336 executed
 // instructions per voxel, 15 % of HBM peak).  Here  coord = (p + flow) * (Ssrc-1)/(S-1)  (the same map in exact
-// arithmetic; identity scale when src and flow grids agree, which is the only case the reference uses), the
-// 8-corner blend is three nested lerps, and voxels whose stencil lies inside the volume (all but a one-voxel
-// shell for registration flows) take a branch with no per-corner predicates.  Each thread walks ZU consecutive
-// slices and issues all of their flow loads before the first gather so that enough bytes are in flight.
+// arithmetic; identity scale when src and flow grids agree, which is the only case the reference uses), and the
+// cell is sampler.cuh's FastCell: a lerp-tree blend of zero-padded corners, read without per-corner predicates
+// when the cell lies inside the volume.  Each thread walks ZU consecutive slices and issues all of their flow
+// loads before the first gather so that enough bytes are in flight.
 // Deviation from the exact path: <= a few 1e-6 of the value range (tests/test_gpu_ops.py).
 // ------------------------------------------------------------------------------------------------------------
 constexpr int ZU = 4;
@@ -138,25 +107,6 @@ struct FastGeom {
   float rz, ry, rx;
 };
 
-template <bool IS3D>
-__device__ __forceinline__ float blend_fast(const float* __restrict__ plane, bool interior, int base, int sW, int sHW,
-                                            float tx, float ty, float tz, const Stencil8& st) {
-  if (interior) {
-    const float* s = plane + base;
-    const float a00 = __ldg(s), a01 = __ldg(s + 1), a10 = __ldg(s + sW), a11 = __ldg(s + sW + 1);
-    const float r0 = fmaf(tx, a01 - a00, a00), r1 = fmaf(tx, a11 - a10, a10);
-    float v0 = fmaf(ty, r1 - r0, r0);
-    if (IS3D) {
-      const float b00 = __ldg(s + sHW), b01 = __ldg(s + sHW + 1), b10 = __ldg(s + sHW + sW), b11 = __ldg(s + sHW + sW + 1);
-      const float q0 = fmaf(tx, b01 - b00, b00), q1 = fmaf(tx, b11 - b10, b10);
-      const float v1 = fmaf(ty, q1 - q0, q0);
-      v0 = fmaf(tz, v1 - v0, v0);
-    }
-    return v0;
-  }
-  return sample8<IS3D, true>(plane, st);
-}
-
 template <bool IS3D, bool C1>
 __global__ void __launch_bounds__(TX* TY) warp_fwd_fast_kernel(const float* __restrict__ src, const float* __restrict__ flow,
                                                                float* __restrict__ out, FastGeom g) {
@@ -165,10 +115,11 @@ __global__ void __launch_bounds__(TX* TY) warp_fwd_fast_kernel(const float* __re
   const int zc = blockIdx.z % g.nzc, b = blockIdx.z / g.nzc;
   if (x >= g.W || y >= g.H) return;
   const int HW = g.H * g.W, DHW = g.D * HW;
-  const int sW = g.Ws, sHW = g.Hs * g.Ws, sDHW = g.Ds * sHW;
+  const int sDHW = g.Ds * g.Hs * g.Ws;
+  const int C = C1 ? 1 : g.C;
   const float* fb = flow + (size_t)b * g.nd * DHW + y * g.W + x;
-  const float* sb = src + (size_t)b * g.C * sDHW;
-  float* ob = out + (size_t)b * g.C * DHW + y * g.W + x;
+  const float* sb = src + (size_t)b * C * sDHW;
+  float* ob = out + (size_t)b * C * DHW + y * g.W + x;
   const int z0c = zc * ZU;
   float f[ZU][3];
 #pragma unroll
@@ -187,40 +138,18 @@ __global__ void __launch_bounds__(TX* TY) warp_fwd_fast_kernel(const float* __re
     const float cz = IS3D ? ((float)z + f[u][0]) * g.rz : 0.f;
     const float cy = ((float)y + f[u][1]) * g.ry;
     const float cx = ((float)x + f[u][2]) * g.rx;
-    const float fx = floorf(cx), fy = floorf(cy), fz = floorf(cz);
-    const int x0 = f2i(fx), y0 = f2i(fy), zz0 = f2i(fz);
-    const bool interior = (unsigned)x0 < (unsigned)(g.Ws - 1) && (unsigned)y0 < (unsigned)(g.Hs - 1) &&
-                          (!IS3D || (unsigned)zz0 < (unsigned)(g.Ds - 1));
-    Stencil8 st;
-    if (!interior) make_stencil8<IS3D>(cx, cy, cz, g.Ds, g.Hs, g.Ws, st);
-    const int base = (zz0 * g.Hs + y0) * g.Ws + x0;
-    const float tx = cx - fx, ty = cy - fy, tz = cz - fz;
-    if (C1) {
-      ob[z * HW] = blend_fast<IS3D>(sb, interior, base, sW, sHW, tx, ty, tz, st);
-    } else {
-      for (int c = 0; c < g.C; ++c)
-        ob[(size_t)c * DHW + z * HW] = blend_fast<IS3D>(sb + (size_t)c * sDHW, interior, base, sW, sHW, tx, ty, tz, st);
+    const FastCell<IS3D> cell = fast_cell<IS3D>(cz, cy, cx, g.Ds, g.Hs, g.Ws);
+    for (int c = 0; c < C; ++c) {
+      float v[8];
+      cell.fetch(sb + (size_t)c * sDHW, v);
+      ob[(size_t)c * DHW + z * HW] = cell.blend(v);
     }
   }
 }
 
-// backward of the fast path: d out / d flow from the same lerp tree (needs the 8 corner values once per channel),
-// d out / d src as a scatter (red.global.add) only when the caller asks for it.  NOSRC: no gradient w.r.t. the source
-// (the moving image of the training step) — with interior voxels on a predicate-free branch this is the variant the
-// step runs; the general form handles borders, source gradients and several channels.
-template <bool IS3D>
-__device__ __forceinline__ void dflow_from_corners(float a00, float a01, float a10, float a11, float b00, float b01, float b10, float b11,
-                                                   float tx, float ty, float tz, float go, float& gx, float& gy, float& gz) {
-  // d/dx: lerp_z(lerp_y(b - a along x));  d/dy, d/dz alike
-  const float dxa = fmaf(ty, (a11 - a10) - (a01 - a00), a01 - a00), dxb = fmaf(ty, (b11 - b10) - (b01 - b00), b01 - b00);
-  const float ra0 = fmaf(tx, a01 - a00, a00), ra1 = fmaf(tx, a11 - a10, a10);
-  const float rb0 = fmaf(tx, b01 - b00, b00), rb1 = fmaf(tx, b11 - b10, b10);
-  const float dya = ra1 - ra0, dyb = rb1 - rb0;
-  gx = fmaf(go, IS3D ? fmaf(tz, dxb - dxa, dxa) : dxa, gx);
-  gy = fmaf(go, IS3D ? fmaf(tz, dyb - dya, dya) : dya, gy);
-  if (IS3D) gz = fmaf(go, fmaf(ty, rb1 - rb0, rb0) - fmaf(ty, ra1 - ra0, ra0), gz);
-}
-
+// backward of the fast path: d out / d flow from the lerp tree of the same corners, d out / d src as a scatter
+// (red.global.add) only when the caller asks for it.  NOSRC: no gradient w.r.t. the source (the moving image of the
+// training step), the variant the step runs.
 template <bool IS3D, bool NOSRC>
 __global__ void __launch_bounds__(TX* TY, NOSRC ? 3 : 2) warp_bwd_fast_kernel(const float* __restrict__ gout, const float* __restrict__ src,
                                                                const float* __restrict__ flow, float* __restrict__ gsrc,
@@ -230,7 +159,7 @@ __global__ void __launch_bounds__(TX* TY, NOSRC ? 3 : 2) warp_bwd_fast_kernel(co
   const int zc = blockIdx.z % g.nzc, b = blockIdx.z / g.nzc;
   if (x >= g.W || y >= g.H) return;
   const int HW = g.H * g.W, DHW = g.D * HW;
-  const int sW = g.Ws, sHW = g.Hs * g.Ws, sDHW = g.Ds * sHW;
+  const int sDHW = g.Ds * g.Hs * g.Ws;
   const float* fb = flow + (size_t)b * g.nd * DHW + y * g.W + x;
   const float* sb = src + (size_t)b * g.C * sDHW;
   float* gsb = (!NOSRC && gsrc) ? gsrc + (size_t)b * g.C * sDHW : nullptr;
@@ -253,56 +182,19 @@ __global__ void __launch_bounds__(TX* TY, NOSRC ? 3 : 2) warp_bwd_fast_kernel(co
     const float cz = IS3D ? ((float)z + f[u][0]) * g.rz : 0.f;
     const float cy = ((float)y + f[u][1]) * g.ry;
     const float cx = ((float)x + f[u][2]) * g.rx;
-    const float fx = floorf(cx), fy = floorf(cy), fz = floorf(cz);
-    const int x0 = f2i(fx), y0 = f2i(fy), zz0 = f2i(fz);
-    const float tx = cx - fx, ty = cy - fy, tz = IS3D ? cz - fz : 0.f;
+    const FastCell<IS3D> cell = fast_cell<IS3D>(cz, cy, cx, g.Ds, g.Hs, g.Ws);
     float gx = 0.f, gy = 0.f, gz = 0.f;
-    const bool interior = (unsigned)x0 < (unsigned)(g.Ws - 1) && (unsigned)y0 < (unsigned)(g.Hs - 1) &&
-                          (!IS3D || (unsigned)zz0 < (unsigned)(g.Ds - 1));
-    if (NOSRC && interior) {
-      const int base = (zz0 * g.Hs + y0) * g.Ws + x0;
-      for (int c = 0; c < g.C; ++c) {
-        const float go = __ldg(gob + (size_t)c * DHW + z * HW);
-        const float* s = sb + (size_t)c * sDHW + base;
-        const float a00 = __ldg(s), a01 = __ldg(s + 1), a10 = __ldg(s + sW), a11 = __ldg(s + sW + 1);
-        float b00 = 0.f, b01 = 0.f, b10 = 0.f, b11 = 0.f;
-        if (IS3D) { b00 = __ldg(s + sHW); b01 = __ldg(s + sHW + 1); b10 = __ldg(s + sHW + sW); b11 = __ldg(s + sHW + sW + 1); }
-        dflow_from_corners<IS3D>(a00, a01, a10, a11, b00, b01, b10, b11, tx, ty, tz, go, gx, gy, gz);
+    for (int c = 0; c < g.C; ++c) {
+      const float go = __ldg(gob + (size_t)c * DHW + z * HW);
+      if (NOSRC || gflow) {
+        float v[8], dz, dy, dx;
+        cell.fetch(sb + (size_t)c * sDHW, v);
+        cell.grad(v, dz, dy, dx);
+        gx = fmaf(go, dx, gx);
+        gy = fmaf(go, dy, gy);
+        if (IS3D) gz = fmaf(go, dz, gz);
       }
-    } else {
-      // per-axis validity of the two taps (zeros padding): out-of-volume taps read as 0 and receive no gradient
-      const bool xa = (unsigned)x0 < (unsigned)g.Ws, xb = (unsigned)(x0 + 1) < (unsigned)g.Ws;
-      const bool ya = (unsigned)y0 < (unsigned)g.Hs, yb = (unsigned)(y0 + 1) < (unsigned)g.Hs;
-      const bool za = !IS3D || (unsigned)zz0 < (unsigned)g.Ds, zb = IS3D && (unsigned)(zz0 + 1) < (unsigned)g.Ds;
-      const int xo0 = min(max(x0, 0), g.Ws - 1), xo1 = min(max(x0 + 1, 0), g.Ws - 1);
-      const int yo0 = min(max(y0, 0), g.Hs - 1) * sW, yo1 = min(max(y0 + 1, 0), g.Hs - 1) * sW;
-      const int zo0 = IS3D ? min(max(zz0, 0), g.Ds - 1) * sHW : 0, zo1 = IS3D ? min(max(zz0 + 1, 0), g.Ds - 1) * sHW : 0;
-      for (int c = 0; c < g.C; ++c) {
-        const float go = __ldg(gob + (size_t)c * DHW + z * HW);
-        const float* s = sb + (size_t)c * sDHW;
-        const float a00 = (za && ya && xa) ? __ldg(s + zo0 + yo0 + xo0) : 0.f, a01 = (za && ya && xb) ? __ldg(s + zo0 + yo0 + xo1) : 0.f;
-        const float a10 = (za && yb && xa) ? __ldg(s + zo0 + yo1 + xo0) : 0.f, a11 = (za && yb && xb) ? __ldg(s + zo0 + yo1 + xo1) : 0.f;
-        float b00 = 0.f, b01 = 0.f, b10 = 0.f, b11 = 0.f;
-        if (IS3D) {
-          b00 = (zb && ya && xa) ? __ldg(s + zo1 + yo0 + xo0) : 0.f; b01 = (zb && ya && xb) ? __ldg(s + zo1 + yo0 + xo1) : 0.f;
-          b10 = (zb && yb && xa) ? __ldg(s + zo1 + yo1 + xo0) : 0.f; b11 = (zb && yb && xb) ? __ldg(s + zo1 + yo1 + xo1) : 0.f;
-        }
-        if (gflow) dflow_from_corners<IS3D>(a00, a01, a10, a11, b00, b01, b10, b11, tx, ty, tz, go, gx, gy, gz);
-        if (!NOSRC && gsb) {
-          float* t = gsb + (size_t)c * sDHW;
-          const float wx0 = 1.f - tx, wy0 = 1.f - ty, wz0 = IS3D ? 1.f - tz : 1.f;
-          if (za && ya && xa) atomicAdd(t + zo0 + yo0 + xo0, go * wx0 * wy0 * wz0);
-          if (za && ya && xb) atomicAdd(t + zo0 + yo0 + xo1, go * tx * wy0 * wz0);
-          if (za && yb && xa) atomicAdd(t + zo0 + yo1 + xo0, go * wx0 * ty * wz0);
-          if (za && yb && xb) atomicAdd(t + zo0 + yo1 + xo1, go * tx * ty * wz0);
-          if (IS3D) {
-            if (zb && ya && xa) atomicAdd(t + zo1 + yo0 + xo0, go * wx0 * wy0 * tz);
-            if (zb && ya && xb) atomicAdd(t + zo1 + yo0 + xo1, go * tx * wy0 * tz);
-            if (zb && yb && xa) atomicAdd(t + zo1 + yo1 + xo0, go * wx0 * ty * tz);
-            if (zb && yb && xb) atomicAdd(t + zo1 + yo1 + xo1, go * tx * ty * tz);
-          }
-        }
-      }
+      if (gsb) cell.scatter(gsb + (size_t)c * sDHW, go);
     }
     if (gflow) {
       float* gf = gflow + (size_t)b * g.nd * DHW + z * HW + y * g.W + x;
