@@ -1,5 +1,6 @@
-"""Median CUDA-event time of every full-resolution convolution launch of the benchmark step (forward, dgrad, wgrad), under the
-environment switches given as KEY=VALUE,... sets on the command line (profiling aid; A/B of kernel variants)."""
+"""Median CUDA-event time and rate of every full-resolution convolution launch of the benchmark step (forward, dgrad,
+wgrad), under the environment switches given as KEY=VALUE,... sets on the command line (profiling aid; A/B of kernel
+variants). The rate is the layer's useful work, 2*27*Cin*Cout*V FLOPs over its real (unpadded) channels, over the time."""
 import sys, os, json, statistics
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -8,6 +9,12 @@ from voxelmorph_b200 import tc
 dev = torch.device("cuda:0")
 FULL = (160, 192, 224)
 HALF = tuple(s // 2 for s in FULL)
+V = FULL[0] * FULL[1] * FULL[2]
+FLOPS = {}          # layer name -> useful FLOPs of the launch (none for the layout kernels)
+
+
+def flops(name, cin, cout):
+    FLOPS[name] = 2 * 27 * cin * cout * V
 
 
 def timeit(fn, n=7):
@@ -40,9 +47,11 @@ def build():
         pk, cp = tc.pack_weights_t(W, variant="s")
         b = torch.zeros(co, device=dev)
         L[name] = (lambda xa=xa, xb=xb, pk=pk, cp=cp, b=b, co=co, up=up: tc.conv_fwd_t(xa, xb, pk, cp, b, co, 3, up=up, slope=0.2))
+        flops(name, 2 if ca + cb == 8 else ca + cb, co)
     # flow head: 16 -> 3, fp32 planar out
     x = rnd(FULL, 16); W = w(3, 16); pk, cp = tc.pack_weights_t(W, variant="s"); b3 = torch.zeros(3, device=dev)
     L["flow_fwd 16->3 planar"] = lambda: tc.conv_fwd_t(x, None, pk, cp, b3, 3, 3, out_fp32_planar=True)
+    flops("flow_fwd 16->3 planar", 16, 3)
     # dgrads (transposed weights): g (Cout ch) -> Cin ch
     for name, cg, cin, mask, split in (("flow_dgrad 8->16 mask", 8, 16, True, None), ("rem2_dgrad 16->16 mask", 16, 16, True, None),
                                        ("rem1_dgrad 16->32 mask", 16, 32, True, None), ("rem0_dgrad 32->48 split", 32, 48, False, 32)):
@@ -51,6 +60,7 @@ def build():
         pk, cp = tc.pack_weights_t(W, transposed=True, variant="s")
         m = rnd(FULL, cin) if mask else None
         L[name] = (lambda g=g, pk=pk, cp=cp, cin=cin, m=m, split=split: tc.conv_fwd_t(g, None, pk, cp, None, cin, 3, slope=0.2 if m is not None else None, mask=m, split=split))
+        flops(name, cg if cg != 8 else 3, cin)
     # wgrads
     for name, cx, up, cg in (("flow_wgrad x16 g8", 16, False, 8), ("rem2_wgrad x16 g16", 16, False, 16), ("rem1_wgrad x32 g16", 32, False, 16),
                              ("rem0_wgrad_a x32^ g32", 32, True, 32), ("rem0_wgrad_b x16 g32", 16, False, 32), ("enc0_wgrad x8 g16", 8, False, 16)):
@@ -59,6 +69,7 @@ def build():
         cout = 3 if cg == 8 else cg
         cin = 2 if cx == 8 else cx
         L[name] = (lambda xx=xx, g=g, cin=cin, cout=cout, up=up: tc.conv_wgrad(xx, None, g, cin, cout, 3, up=up))
+        flops(name, cin, cout)
     # kd-folded variants of the two layers with 2 / 3 real channels on one side
     planes2 = [torch.rand((1, 1) + FULL, device=dev) for _ in range(2)]
     planes3 = [torch.randn((1, 1) + FULL, device=dev) for _ in range(3)]
@@ -68,9 +79,11 @@ def build():
     x3 = tc.planar_fold_kd(planes2, 8)
     W0 = w(16, 2); pk0, cp0 = tc.pack_weights_fold(W0); b16 = torch.zeros(16, device=dev)
     L["fold: enc0_fwd 2D (6 of 8)->16"] = lambda: tc.conv_fwd_t(x3, None, pk0, cp0, b16, 16, 1, slope=0.2)
+    flops("fold: enc0_fwd 2D (6 of 8)->16", 2, 16)
     g3 = tc.planar_fold_kd(planes3, 16)
     Wf = w(3, 16); pkf, cpf = tc.pack_weights_fold(Wf, transposed=True); m16 = rnd(FULL, 16)
     L["fold: flow_dgrad 2D (9 of 16)->16 mask"] = lambda: tc.conv_fwd_t(g3, None, pkf, cpf, None, 16, 1, slope=0.2, mask=m16)
+    flops("fold: flow_dgrad 2D (9 of 16)->16 mask", 3, 16)
     batch = tc.WgradBatch.get(dev)
     gw0 = torch.empty((16, 6, 1, 3, 3), device=dev); gb0 = torch.empty(16, device=dev); gz16 = rnd(FULL, 16)
     gwf = torch.empty((9, 16, 1, 3, 3), device=dev); gbf = torch.empty(9, device=dev); x16 = rnd(FULL, 16)
@@ -80,6 +93,8 @@ def build():
         batch.flush()
     L["fold: enc0_wgrad khm"] = lambda: khm(x3, gz16, gw0, gb0, 6, 16)
     L["fold: flow_wgrad khm"] = lambda: khm(x16, g3, gwf, gbf, 16, 9)
+    flops("fold: enc0_wgrad khm", 2, 16)
+    flops("fold: flow_wgrad khm", 16, 3)
     return L
 
 
@@ -102,8 +117,14 @@ for s in sets:
     for k in kv:
         os.environ.pop(k, None)
 names = list(L)
-print("%-28s" % "layer" + "".join("%22s" % (s or "default")[-22:] for s in sets))
+
+
+def rate(n, us):
+    return "%8.1f TF/s" % (FLOPS[n] / (us * 1e-6) / 1e12) if n in FLOPS else " " * 13
+
+
+print("%-40s" % "layer" + "".join("%26s" % (s or "default")[-26:] for s in sets))
 for n in names:
-    print("%-28s" % n + "".join("%22.1f" % res[s or "default"][n] for s in sets))
-print("%-28s" % "sum" + "".join("%22.1f" % sum(res[s or "default"].values()) for s in sets))
+    print("%-40s" % n + "".join("%10.1f us %s" % (res[s or "default"][n], rate(n, res[s or "default"][n])) for s in sets))
+print("%-40s" % "sum" + "".join("%10.1f us %13s" % (sum(res[s or "default"].values()), "") for s in sets))
 print(json.dumps(res))

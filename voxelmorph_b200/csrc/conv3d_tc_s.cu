@@ -185,13 +185,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     const int wq = warp & 3;
     float* stage = s_stage + grp * ACC_STAGE_FLOATS;
     const int nbar = 1 + grp;
-    // MMA N per wgmma: the three kw taps stacked (N = 3 * COUT) up to COUT = 32; wider layers run in passes of 16
-    // output channels with one wgmma per kw (the accumulators of a pass stay within the register budget)
-    constexpr bool STACK = COUT <= 32;
-    constexpr int CW = STACK ? COUT : 16;            // output channels per pass
-    constexpr int NPASS = COUT / CW;
-    constexpr int NA = STACK ? NN : CW;              // N of one wgmma
-    constexpr int NW = STACK ? 1 : 3;                // wgmmas per K step and tile half
+    // Every wgmma stacks the three kw taps (N = 3 * COUT).  Up to COUT = 32 one chain covers the 128-row tile half in
+    // two m64 accumulators and thread t drains row t.  Wider layers run one chain per m64 half (`sub`: tile rows
+    // 2 sub, 2 sub + 1) so that its single accumulator stays at 72 / 96 floats per thread; all 128 threads drain it, two
+    // per voxel row, the warp pair wq >> 1 taking every other 16-channel chunk.
+    constexpr int NSUB = NN > 96 ? 2 : 1;            // chains per tile half
+    constexpr int NF = 2 / NSUB;                     // m64 accumulators per chain
+    constexpr int NCH = NSUB == 1 ? COUT / 16 : (COUT + 31) / 32;   // 16-channel chunks per thread and chain
+    const int trow0 = NSUB == 1 ? wq : (wq & 1);     // tile row of this thread in sub-tile `sub`: trow0 + 2 * sub
+    auto chan = [&](int i) { return NSUB == 1 ? 16 * i : 32 * i + 16 * (wq >> 1); };   // first channel of chunk i
     const uint32_t slab_u32 = smem_u32(s_slab), w_u32 = smem_u32(s_w);
     constexpr uint32_t WSTEP = (uint32_t)NN * (W0 + W1);          // bytes of packed weights per (kd, kh) step
     mbar_wait(wbar, 0);
@@ -201,8 +203,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     auto observe = [&](uint32_t upto) {              // wait for every slab up to global index `upto`, in order
       for (; wcur <= upto; ++wcur) mbar_wait(&full[wcur % NSLOT], (wcur / NSLOT) & 1);
     };
-    // wgmma chain of tile half hb of the step whose kd window starts at ring slot `hslot`, output channels of `pass`
-    auto mma = [&](uint32_t hslot, int hb, int pass, float (&acc)[2][NW][NA / 2]) {
+    // wgmma chain of sub-tile `sub` of tile half hb of the step whose kd window starts at ring slot `hslot`
+    auto mma = [&](uint32_t hslot, int hb, int sub, float (&acc)[NF][NN / 2]) {
       uint64_t adesc0_kd[KD], adesc1_kd[KD];
       uint32_t sl = hslot;
 #pragma unroll
@@ -225,29 +227,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
             const uint64_t adesc = (g0 ? adesc0_kd[kd] : adesc1_kd[kd]) + (uint64_t)(((hb * 4 + kh) * WT * wr + kk * 32) >> 4);
             const uint64_t bdesc = (g0 ? bdesc0 : bdesc1) + (uint64_t)((st * WSTEP + kk * 32) >> 4);
 #pragma unroll
-            for (int g = 0; g < NW; ++g) {
-              // non-stacked: weight rows kw * COUT + pass * 16 (whole 8-row swizzle atoms)
-              const uint64_t bd = STACK ? bdesc : bdesc + (uint64_t)(((g * COUT + pass * CW) * wr) >> 4);
-#pragma unroll
-              for (int hf = 0; hf < 2; ++hf)            // rows 64-127 of the tile: two slab rows further
-                Wgmma<NA, 0, 0>::mma(acc[hf][g], adesc + (uint64_t)((hf * 2 * WT * wr) >> 4), bd, (st | k) ? 1u : 0u);
-            }
+            for (int f = 0; f < NF; ++f)                // m64 half sub + f of the tile half: two slab rows per half
+              Wgmma<NN, 0, 0>::mma(acc[f], adesc + (uint64_t)(((sub + f) * 2 * WT * wr) >> 4), bdesc, (st | k) ? 1u : 0u);
           }
         }
       }
       wg_commit();
       wg_wait<0>();
     };
-    // v[c] = out[w'][pass * CW + cc + c] = P0[w'-1] + P1[w'] + P2[w'+1] (kw partial sums, shuffled across lanes)
-    auto combine = [&](float (&acc)[2][NW][NA / 2], int cc, float (&v)[16]) {
+    // columns [c, c + 16) of the chain's accumulators in row form (see chan for the 16 this thread receives)
+    auto readout = [&](float (&acc)[NF][NN / 2], int c, uint32_t (&r)[16]) {
+      if constexpr (NSUB == 1) acc_row16(acc[0], acc[NF - 1], c, stage, nbar, r);
+      else acc_half_row16(acc[0], c, COUT - (c % COUT) < 32 ? 16 : 32, stage, nbar, r);
+    };
+    // v[c] = out[w'][chan(i) + c] = P0[w'-1] + P1[w'] + P2[w'+1] (kw partial sums, shuffled across lanes)
+    auto combine = [&](float (&acc)[NF][NN / 2], int i, float (&v)[16]) {
+      const int cb = NSUB == 1 ? 16 * i : 32 * i;
       uint32_t r[16];
-      acc_row16(acc[0][0], acc[1][0], STACK ? cc : 0, stage, nbar, r);
+      readout(acc, cb, r);
 #pragma unroll
       for (int c = 0; c < 16; ++c) v[c] = __shfl_up_sync(0xffffffffu, __uint_as_float(r[c]), 1);
-      acc_row16(acc[0][NW > 1 ? 1 : 0], acc[1][NW > 1 ? 1 : 0], STACK ? COUT + cc : 0, stage, nbar, r);
+      readout(acc, COUT + cb, r);
 #pragma unroll
       for (int c = 0; c < 16; ++c) v[c] += __uint_as_float(r[c]);
-      acc_row16(acc[0][NW - 1], acc[1][NW - 1], STACK ? 2 * COUT + cc : 0, stage, nbar, r);
+      readout(acc, 2 * COUT + cb, r);
 #pragma unroll
       for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, __uint_as_float(r[c]), 1);
     };
@@ -273,13 +276,16 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
         const int nd = d1 - d0;
         const bool wok = lane >= 1 && lane <= WUSE && w < a.W;
-        bool ok[NH];
-        size_t vx[NH];                                           // voxel index of this lane in slice d0
+        bool ok[NH][NSUB];
+        size_t vx[NH][NSUB];                                     // voxel index of this lane in slice d0
 #pragma unroll
         for (int hb = 0; hb < NH; ++hb) {
-          const int h = ht * HT + hb * 4 + wq;
-          ok[hb] = wok && h < a.H;
-          vx[hb] = (((size_t)b * a.D + d0) * a.H + h) * a.W + w;
+#pragma unroll
+          for (int sub = 0; sub < NSUB; ++sub) {
+            const int h = ht * HT + hb * 4 + trow0 + 2 * sub;
+            ok[hb][sub] = wok && h < a.H;
+            vx[hb][sub] = (((size_t)b * a.D + d0) * a.H + h) * a.W + w;
+          }
         }
         for (int j = 0; j < nd; ++j) {
           observe(cnt_base + (uint32_t)j + (KD == 3 ? 2u : 0u));
@@ -287,26 +293,31 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
 #pragma unroll
           for (int hb = 0; hb < NH; ++hb) {
             const bool mine = (int)(ecnt++ % NGRP) == grp;
-            const size_t vox = vx[hb];
-            vx[hb] += HWp;
-            if (!mine) continue;
-            const bool valid = ok[hb];
-            [[maybe_unused]] uint32_t mreg[EPI == 2 ? COUT / 16 : 1][8];
-            if constexpr (EPI == 2) {
-              if (valid) {
+            size_t voxs[NSUB];
 #pragma unroll
-                for (int q = 0; q < COUT / 16; ++q) ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + q * 16, mreg[q]);
-              }
+            for (int sub = 0; sub < NSUB; ++sub) {
+              voxs[sub] = vx[hb][sub];
+              vx[hb][sub] += HWp;
             }
+            if (!mine) continue;
 #pragma unroll
-            for (int pass = 0; pass < NPASS; ++pass) {
-              float acc[2][NW][NA / 2];
-              mma(hslot, hb, pass, acc);
+            for (int sub = 0; sub < NSUB; ++sub) {
+              const size_t vox = voxs[sub];
+              const bool valid = ok[hb][sub];
+              [[maybe_unused]] uint32_t mreg[EPI == 2 ? NCH : 1][8];
+              if constexpr (EPI == 2) {
 #pragma unroll
-              for (int cc = 0; cc < CW; cc += 16) {
-                const int c0 = pass * CW + cc;
+                for (int i = 0; i < NCH; ++i)
+                  if (valid && chan(i) < COUT) ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + chan(i), mreg[i]);
+              }
+              float acc[NF][NN / 2];
+              mma(hslot, hb, sub, acc);
+#pragma unroll
+              for (int i = 0; i < NCH; ++i) {
+                const int c0 = chan(i);
                 float v[16];
-                combine(acc, cc, v);
+                combine(acc, i, v);
+                if (NSUB > 1 && c0 >= COUT) continue;            // (48 channels: the second warp pair has one chunk less)
                 if constexpr (EPI == 1) {
 #pragma unroll
                   for (int c = 0; c < 16; ++c) {
@@ -316,7 +327,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                 } else if constexpr (EPI == 2) {
 #pragma unroll
                   for (int e = 0; e < 8; ++e) {                    // sign bits of the saved bf16 activations
-                    const uint32_t mw = mreg[c0 / 16][e];
+                    const uint32_t mw = mreg[i][e];
                     if (mw & 0x8000u) v[2 * e] *= slope;
                     if (mw & 0x80000000u) v[2 * e + 1] *= slope;
                   }
@@ -349,39 +360,45 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
 #pragma unroll
         for (int hb = 0; hb < NH; ++hb) {
         if ((int)(ecnt++ % NGRP) != grp) continue;
-        const int h = ht * HT + hb * 4 + wq;
+#pragma unroll
+        for (int sub = 0; sub < NSUB; ++sub) {
+        const int h = ht * HT + hb * 4 + trow0 + 2 * sub;
         const bool valid = lane >= 1 && lane <= WUSE && h < a.H && w < a.W;
         const size_t vox = (((size_t)b * a.D + d) * a.H + h) * a.W + w;
-        // prefetch the LeakyReLU-derivative mask of this voxel before the MMAs
-        uint4 mreg[COUT / 8];
-        if (a.mask && valid) {
+        // prefetch the LeakyReLU-derivative mask of this voxel before the MMAs (one chain per m64 half: read after the
+        // combine instead, the prefetch would spill next to the wider accumulator)
+        constexpr bool PREF = NSUB == 1;
+        [[maybe_unused]] uint4 mreg[PREF ? NCH : 1][2];
+        if (PREF && a.mask && valid) {
 #pragma unroll
-          for (int q = 0; q < COUT / 8; ++q)
-            if (q * 8 < a.Cout) mreg[q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * (OP ? a.opitch : a.Cout)) + q);
+          for (int i = 0; i < NCH; ++i)
+#pragma unroll
+            for (int q = 0; q < 2; ++q)
+              if (chan(i) + 8 * q < a.Cout)
+                mreg[i][q] = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * (OP ? a.opitch : a.Cout) + chan(i)) + q);
         }
         const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
-#pragma unroll
-        for (int pass = 0; pass < NPASS; ++pass) {
-        float acc[2][NW][NA / 2];
-        mma(hslot, hb, pass, acc);
+        float acc[NF][NN / 2];
+        mma(hslot, hb, sub, acc);
         // 16 output channels at a time: the kw = 0, 1, 2 partial sums, shuffle-combined across lanes, stored
 #pragma unroll
-        for (int cc = 0; cc < CW; cc += 16) {
-          const int c0 = pass * CW + cc;
+        for (int i = 0; i < NCH; ++i) {
+          const int c0 = chan(i);
           [[maybe_unused]] float4 ain[ACC ? 4 : 1];
-          if constexpr (ACC && !OP) {     // (OP: read after the combine, the prefetch would spill)
-            if (a.acc_in && valid) {      // partial sums of the earlier split-precision passes
+          if constexpr (ACC && !OP && PREF) {     // (otherwise read after the combine, the prefetch would spill)
+            if (a.acc_in && valid && c0 < COUT) {      // partial sums of the earlier split-precision passes
               const float4* ap = reinterpret_cast<const float4*>(a.acc_in + vox * COUT + c0);
 #pragma unroll
               for (int q = 0; q < 4; ++q) ain[q] = __ldg(ap + q);
             }
           }
           float v[16];
-          combine(acc, cc, v);
+          combine(acc, i, v);
+          if (NSUB > 1 && c0 >= COUT) continue;            // (48 channels: the second warp pair has one chunk less)
           bool handled = false;
           if constexpr (ACC) {
             if (a.acc_in && valid) {
-              if constexpr (OP) {
+              if constexpr (OP || !PREF) {
                 const float4* ap = reinterpret_cast<const float4*>(a.acc_in + vox * COUT + c0);
 #pragma unroll
                 for (int q = 0; q < 4; ++q) ain[q] = __ldg(ap + q);
@@ -428,7 +445,9 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
 #pragma unroll
                   for (int e = 0; e < 8; ++e) x[e] = v[q + e] + bias_at(c0 + q + e);
                   if (a.mask) {
-                    const uint4 m4 = mreg[(c0 + q) / 8];
+                    uint4 m4;
+                    if constexpr (PREF) m4 = mreg[i][q / 8];
+                    else m4 = __ldg(reinterpret_cast<const uint4*>(a.mask + vox * (OP ? a.opitch : a.Cout) + c0) + q / 8);
                     const __nv_bfloat16* mb = reinterpret_cast<const __nv_bfloat16*>(&m4);
 #pragma unroll
                     for (int e = 0; e < 8; ++e) if (__bfloat162float(mb[e]) < 0.f) x[e] *= a.slope;

@@ -143,6 +143,32 @@ __device__ __forceinline__ void acc_row16(const float* d0, const float* d1, int 
   for (int k = 0; k < 16; ++k) r[k] = __float_as_uint(mine[k]);
 }
 
+// Read-out of ONE m64 fragment d with two threads per row: `ncol` (16 or 32) columns [c0, c0 + ncol) pass through
+// `stage`, and thread t of the warpgroup receives row (t & 31) + 32 * ((t >> 5) & 1), columns [c0 + 16 * (t >> 6), +16)
+// (with ncol = 16, threads t >= 64 receive nothing meaningful).  c0 and ncol are compile-time after unrolling.
+constexpr int ACC_HALF_LD = 33;                      // padded 32-column row: conflict-free row reads
+static_assert(64 * ACC_HALF_LD <= ACC_STAGE_FLOATS, "half read-out fits the stage buffer");
+__device__ __forceinline__ void acc_half_row16(const float* d, int c0, int ncol, float* stage, int bar, uint32_t* r) {
+  const int t = threadIdx.x & 127, w = t >> 5, q = (t & 31) >> 2, p = t & 3;
+  named_bar(bar, 128);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float* srow = stage + (16 * w + 8 * i + q) * ACC_HALF_LD + 2 * p;
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj) {
+      if (8 * jj < ncol) {
+        const int j = c0 / 8 + jj;
+        srow[8 * jj] = d[4 * j + 2 * i];
+        srow[8 * jj + 1] = d[4 * j + 2 * i + 1];
+      }
+    }
+  }
+  named_bar(bar, 128);
+  const float* mine = stage + ((t & 31) + 32 * ((t >> 5) & 1)) * ACC_HALF_LD + 16 * (t >> 6);
+#pragma unroll
+  for (int k = 0; k < 16; ++k) r[k] = __float_as_uint(mine[k]);
+}
+
 // ---------------------------------------------------------------- descriptors ---------------
 // wgmma shared-memory matrix descriptor (sm_90): start address, LBO, SBO in 16-byte units; bits 62-63 = swizzle
 // (0 none, 1 = 128 B, 2 = 64 B, 3 = 32 B).
