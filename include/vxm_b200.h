@@ -230,6 +230,17 @@ int vxm_conv3d_tcs_fits(int cin, int coutp, int kd);
 int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
                            const void* mask, const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout,
                            int coutp, int kd, int out_mode, float slope, int opitch, void* stream);
+/* Polyphase launches of a 3-D concat layer whose first Ca = 32 input channels are a nearest-x2 upsampled source (the taps
+ * that read the same coarse voxel merged into one).  mode 1: forward of (32 upsampled + 16) -> 32 with bias + LeakyReLU
+ * (xa coarse, xb and out at the fine (D, H, W); kd taps merged).  mode 2: coarse dgrad (kd and kh taps merged): xa = the
+ * layer's 32-channel output gradient (B, D, H, W, 32), mask = the coarse source (B, D / 2, H / 2, W / 2, 32), a LeakyReLU
+ * activation of negative slope `slope`; out = the gradient w.r.t. its pre-activation, same shape.  Operands:
+ * vxm_conv3d_tcs_pack_desc_poly (same mode; Cout, Cin: the weight's, Ca: the upsampled channels),
+ * vxm_conv3d_tcs_poly_packed_bytes bytes (0: no such operand). */
+size_t vxm_conv3d_tcs_poly_packed_bytes(int mode, int Cout, int Cin, int Ca);
+int vxm_conv3d_tcs_pack_desc_poly(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int Ca, int mode, int begin);
+int vxm_conv3d_tcs_poly(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask, int B, int D,
+                        int H, int W, int Ca, int Cb, int Cout, int mode, float slope, void* stream);
 /* Weight (and bias) gradient on tensor cores.  x sources as in vxm_conv3d_tc_fwd (the layer's forward input);
  * gz = gradient w.r.t. the convolution output (already multiplied by the activation derivative): bf16 NDHWC with
  * Cg in {8,16,32} channels, or nplanar_g (<= 4) planar fp32 volumes (flow head).  grad_w: fp32

@@ -61,6 +61,21 @@ def build():
         m = rnd(FULL, cin) if mask else None
         L[name] = (lambda g=g, pk=pk, cp=cp, cin=cin, m=m, split=split: tc.conv_fwd_t(g, None, pk, cp, None, cin, 3, slope=0.2 if m is not None else None, mask=m, split=split))
         flops(name, cg if cg != 8 else 3, cin)
+    # polyphase forms of rem0 (the engine's default; VXM_B200_POLYPHASE=0 runs the two launches above and the gradient
+    # routing through the upsampler below, which the coarse dgrad does in its epilogue)
+    from voxelmorph_b200 import engine_bf16
+    xa, xb, g32, a32 = rnd(HALF, 32), rnd(FULL, 16), rnd(FULL, 32), rnd(HALF, 32)
+    W = w(32, 48); b = torch.zeros(32, device=dev)
+    pk_pf, pk_pd = tc.pack_weights_poly(W, 1, 32), tc.pack_weights_poly(W, 2, 32)
+    pk_ps = tc.pack_weights_blocks(W, True, (((2, 0, 32),), ((32, 16, 0, 0),)))
+    L["rem0_fwd poly 32^+16->32"] = lambda: tc.conv_fwd_poly(xa, xb, pk_pf, b, 32, 0.2)
+    flops("rem0_fwd poly 32^+16->32", 48, 32)
+    L["rem0_dgrad_up poly 32->32 coarse"] = lambda: tc.dgrad_poly(g32, pk_pd, a32, 0.2)
+    flops("rem0_dgrad_up poly 32->32 coarse", 32, 32)
+    L["rem0_dgrad_skip 32->16"] = lambda: tc.conv_fwd_t(g32, None, pk_ps[0, 0][0], (pk_ps[0, 0][1], "s"), None, 16, 3)
+    flops("rem0_dgrad_skip 32->16", 32, 16)
+    g_up = rnd(FULL, 32)
+    L["rem0 sumpool_mask 2x2x2 (split dgrad)"] = lambda: engine_bf16._sumpool_mask(g_up, a32, 3, 0.2)
     # wgrads
     for name, cx, up, cg in (("flow_wgrad x16 g8", 16, False, 8), ("rem2_wgrad x16 g16", 16, False, 16), ("rem1_wgrad x32 g16", 32, False, 16),
                              ("rem0_wgrad_a x32^ g32", 32, True, 32), ("rem0_wgrad_b x16 g32", 16, False, 32), ("enc0_wgrad x8 g16", 8, False, 16)):

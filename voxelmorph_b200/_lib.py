@@ -67,6 +67,9 @@ SIGNATURES = {
     "vxm_conv3d_tcs_fwd_acc": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f]),
     "vxm_conv3d_tcs_fits": (c_i, [c_i] * 3),
     "vxm_conv3d_tcs_fwd_blk": (c_i, [c_f] * 8 + [c_i] * 11 + [c_fl, c_i, c_f]),
+    "vxm_conv3d_tcs_poly_packed_bytes": (c_sz, [c_i] * 4),
+    "vxm_conv3d_tcs_pack_desc_poly": (c_i, [c_f, c_f, c_f] + [c_i] * 5),
+    "vxm_conv3d_tcs_poly": (c_i, [c_f] * 6 + [c_i] * 8 + [c_fl, c_f]),
     "vxm_conv3d_tc_wgrad_workspace_bytes": (c_sz, [c_i]),
     "vxm_conv3d_tc_wgrad": (c_i, [c_f, c_f, c_f, c_f, c_i, c_f, c_f, c_f, c_i, c_f, c_f, c_f] + [c_i] * 12 + [c_f]),
     "vxm_conv3d_tc_wgrad2_desc_bytes": (c_sz, []),

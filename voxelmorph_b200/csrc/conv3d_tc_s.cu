@@ -67,10 +67,27 @@ __device__ __forceinline__ uint64_t make_desc_kmajor_swz(uint32_t saddr, uint32_
 // 3 = raw sums with an optional channel split at a multiple of 16 (single-pass dgrad of a concat layer).
 // OP: the bf16 outputs and the mask are one channel block of a wider tensor (pitch a.opitch, no out2); the channel-blocked
 // execution of the layers whose weights do not fit shared memory in one piece (64 -> 64, 128 -> 64, ...).
-template <int KD, int G0, int G1, int COUT, int HT, bool ACC, int EPI, bool OP = false>
+// PD: polyphase forms of a layer that reads a nearest-x2 upsampled source (3-D, EPI != 0).  Along each axis the upsampled
+// data has one value per pair of fine positions, so two of the three taps always read the same coarse voxel:
+//   1 = forward: channel group 0 is the upsampled source.  An even output slice 2c reads slabs (2c - 1, 2c) with the merged
+//       weights (W0, W1 + W2), an odd one 2c + 1 reads slabs (2c + 1, 2c + 2) with (W0 + W1, W2): 2 kd steps instead of 3
+//       for that group.  Group 1 (the skip source) keeps its 3 kd steps.  The ring and the loader do not change.
+//   2 = coarse dgrad (EPI 2, G1 = 0, HT 8): the gradient w.r.t. the coarse source itself.  The same algebra holds along d
+//       and h: coarse slice c reads the 4 fine gradient slabs 2c - 1 .. 2c + 2 and coarse row q of a tile the 4 fine slab
+//       rows 2q .. 2q + 3, with the transposed taps (T0, T0 + T1, T1 + T2, T2) along each of the two axes: 16 (kd, kh)
+//       steps per coarse (d, h), against 2 x 2 x 9 over the fine ones.  The slab rows are staged parity-major (even rows
+//       first), so that the rows 2q + k of the coarse rows q, q + 1 of an m64 block are adjacent; an 8-row tile is ONE
+//       128-row event of 4 coarse rows, and the ring window advances by 2 slabs per coarse slice.  w stays fine (kw stacked
+//       in N, as everywhere): the epilogue adds the w' pairs (2c, 2c + 1) across lanes, applies the LeakyReLU derivative of
+//       the coarse activation (a.mask) and stores the coarse gradient.  Staged by cp.async only (no TMA box permutes rows).
+template <int KD, int G0, int G1, int COUT, int HT, bool ACC, int EPI, bool OP = false, int PD = 0>
 __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_constant__ ConvSArgs a) {
+  static_assert(PD == 0 || (KD == 3 && EPI != 0 && !ACC && !OP), "polyphase forms: 3-D, specialised epilogue");
+  static_assert(PD != 1 || G1 > 0, "the polyphase forward merges channel group 0 and keeps group 1");
+  static_assert(PD != 2 || (G1 == 0 && COUT == 32 && HT == 8 && EPI == 2), "the coarse dgrad: 32 -> 32 channels, 8-row tiles");
   constexpr int SROWS = (HT + 2) * WT;
-  constexpr int NH = HT / 4;
+  constexpr int NH = PD == 2 ? 1 : HT / 4;                // tile events per slab step (PD 2: 4 coarse rows = 128 rows)
+  constexpr int NEVEN = (HT + 3) / 2;                     // PD 2: even slab rows, staged first
   constexpr int W0 = G0 * 2, W1 = G1 * 2;                 // row bytes of the two channel groups
   constexpr int NC8 = (G0 + G1) / 8;                      // 16-byte chunks per voxel
   constexpr uint32_t SLAB0 = SROWS * W0, SLAB1 = SROWS * W1;
@@ -107,6 +124,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     }
   }
   const int HW_tiles = a.tiles_h * a.tiles_w;
+  const int Dout = PD == 2 ? a.D >> 1 : a.D;              // output slices (a.D: slices of the slab source)
 
   if (warp >= 8) {
     // ================================ LOADER (128 threads) ================================
@@ -124,8 +142,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     for (int item = blockIdx.x; item < a.nitems && !(all_tma && lt != 0); item += gridDim.x) {
       const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
       const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
-      const int h0 = ht * HT, w0 = wt * WUSE, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
-      const int s_begin = KD == 3 ? d0 - 1 : d0, s_end = KD == 3 ? d1 + 1 : d1;
+      const int h0 = ht * HT, w0 = wt * WUSE, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, Dout);
+      const int s_begin = PD == 2 ? 2 * d0 - 1 : (KD == 3 ? d0 - 1 : d0), s_end = PD == 2 ? 2 * d1 + 1 : (KD == 3 ? d1 + 1 : d1);
       int soff[KMAX];
       uint32_t doff[KMAX];
 #pragma unroll
@@ -137,7 +155,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
           const int c8 = id % NC8, row = id / NC8;
           const int r = row >> 5, c = row & 31;
           const int h = h0 - 1 + r, w = w0 - 1 + c;
-          doff[k] = c8 < G0 / 8 ? swz((uint32_t)row * W0 + (uint32_t)c8 * 16u, W0)
+          const int srow = PD == 2 ? ((r & 1) ? NEVEN + (r >> 1) : (r >> 1)) * WT + c : row;   // parity-major rows (PD 2)
+          doff[k] = c8 < G0 / 8 ? swz((uint32_t)srow * W0 + (uint32_t)c8 * 16u, W0)
                                 : SLAB0 + swz((uint32_t)row * W1 + (uint32_t)(c8 - G0 / 8) * 16u, W1 ? W1 : 32);
           if (c8 < G0 / 8 ? tma0 : tma1) soff[k] = -2;      // this chunk's group arrives by tensor copy
           else if (h >= 0 && h < a.H && w >= 0 && w < a.W && !(halfk && c8 > 0)) {
@@ -203,31 +222,42 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     auto observe = [&](uint32_t upto) {              // wait for every slab up to global index `upto`, in order
       for (; wcur <= upto; ++wcur) mbar_wait(&full[wcur % NSLOT], (wcur / NSLOT) & 1);
     };
-    // wgmma chain of sub-tile `sub` of tile half hb of the step whose kd window starts at ring slot `hslot`
-    auto mma = [&](uint32_t hslot, int hb, int sub, float (&acc)[NF][NN / 2]) {
-      uint64_t adesc0_kd[KD], adesc1_kd[KD];
+    // wgmma chain of sub-tile `sub` of tile half hb of the step whose kd window starts at ring slot `hslot`; `par`: parity
+    // of the output slice (PD 1)
+    constexpr int NKD = PD == 2 ? 4 : KD;            // slabs of the kd window
+    auto mma = [&](uint32_t hslot, int hb, int sub, float (&acc)[NF][NN / 2], int par) {
+      uint64_t adesc0_kd[NKD], adesc1_kd[NKD];
       uint32_t sl = hslot;
 #pragma unroll
-      for (int kd = 0; kd < KD; ++kd) {
+      for (int kd = 0; kd < NKD; ++kd) {
         adesc0_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes, W0);
         adesc1_kd[kd] = make_desc_kmajor_swz(slab_u32 + sl * slab_bytes + SLAB0, W1 ? W1 : 32);
         if (++sl == (uint32_t)NSLOT) sl = 0;
       }
       wg_fence();
 #pragma unroll
-      for (int kd = 0; kd < KD; ++kd) {
+      for (int kd = 0; kd < NKD; ++kd) {
 #pragma unroll
-        for (int kh = 0; kh < 3; ++kh) {
-          const int st = kd * 3 + kh;
+        for (int kh = 0; kh < (PD == 2 ? 4 : 3); ++kh) {
+          const int st = kd * (PD == 2 ? 4 : 3) + kh;
 #pragma unroll
           for (int k = 0; k < (G0 + G1) / 16; ++k) {  // start-address field is in 16-byte units: kh rows, 32 B per K step
             const bool g0 = k < G0 / 16;
+            if (PD == 1 && g0 && kd == 2) continue;    // the upsampled group has 2 kd steps (see PD)
             const int kk = g0 ? k : k - G0 / 16;
             const uint32_t wr = g0 ? W0 : W1;
-            const uint64_t adesc = (g0 ? adesc0_kd[kd] : adesc1_kd[kd]) + (uint64_t)(((hb * 4 + kh) * WT * wr + kk * 32) >> 4);
-            const uint64_t bdesc = (g0 ? bdesc0 : bdesc1) + (uint64_t)((st * WSTEP + kk * 32) >> 4);
+            uint64_t abase = g0 ? adesc0_kd[kd] : adesc1_kd[kd];
+            uint32_t wst = st * WSTEP;
+            if (PD == 1 && g0 && par) {                // odd slice: slabs (d, d + 1), tiles (W0 + W1 after the 9 steps, W2)
+              abase = adesc0_kd[kd + 1 < NKD ? kd + 1 : kd];
+              wst = kd == 0 ? 9 * WSTEP + kh * NN * W0 : (6 + kh) * WSTEP;
+            }
+            // first slab row of tap kh: row hb * 4 + kh; PD 2: row 2q + kh of coarse row q = 0 in the parity-major order
+            const int r0 = PD == 2 ? ((kh & 1) ? NEVEN : 0) + (kh >> 1) : hb * 4 + kh;
+            const uint64_t adesc = abase + (uint64_t)((r0 * WT * wr + kk * 32) >> 4);
+            const uint64_t bdesc = (g0 ? bdesc0 : bdesc1) + (uint64_t)((wst + kk * 32) >> 4);
 #pragma unroll
-            for (int f = 0; f < NF; ++f)                // m64 half sub + f of the tile half: two slab rows per half
+            for (int f = 0; f < NF; ++f)                // m64 half sub + f of the tile half: two (PD 2: coarse) rows per half
               Wgmma<NN, 0, 0>::mma(acc[f], adesc + (uint64_t)(((sub + f) * 2 * WT * wr) >> 4), bdesc, (st | k) ? 1u : 0u);
           }
         }
@@ -254,14 +284,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
 #pragma unroll
       for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, __uint_as_float(r[c]), 1);
     };
-    auto release = [&](int nd) {                     // end of an item: slabs nd and nd + 1 of a 3-D window
+    auto release = [&](int nd) {                     // end of an item: the last two slabs of a 3-D window
       if (KD == 3) {
-        observe(cnt_base + (uint32_t)nd + 1u);
+        const uint32_t last = PD == 2 ? 2u * nd : (uint32_t)nd;
+        observe(cnt_base + last + 1u);
         if (lane == 0) {
-          mbar_arrive(&empty[(cnt_base + nd) % NSLOT]);
-          mbar_arrive(&empty[(cnt_base + nd + 1) % NSLOT]);
+          mbar_arrive(&empty[(cnt_base + last) % NSLOT]);
+          mbar_arrive(&empty[(cnt_base + last + 1) % NSLOT]);
         }
-        cnt_base += nd + 2;
+        cnt_base += last + 2;
       } else {
         cnt_base += nd;
       }
@@ -269,27 +300,30 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     if constexpr (EPI != 0) {
       const float slope = a.slope;
       const int c1 = (EPI == 3 && a.out2) ? a.csplit : COUT;       // channels [0, c1) -> out, [c1, COUT) -> out2
-      const size_t HWp = (size_t)a.H * a.W;
+      const int Ho = PD == 2 ? a.H >> 1 : a.H, Wo = PD == 2 ? a.W >> 1 : a.W;   // output rows, columns
+      const size_t HWp = (size_t)Ho * Wo;
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
         const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
-        const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.D);
+        const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, Dout);
         const int nd = d1 - d0;
-        const bool wok = lane >= 1 && lane <= WUSE && w < a.W;
+        // PD 2: the odd lanes (even w) hold the sums of their w' pairs and store coarse column w / 2
+        const bool wok = lane >= 1 && lane <= WUSE && w < a.W && (PD != 2 || (lane & 1));
         bool ok[NH][NSUB];
         size_t vx[NH][NSUB];                                     // voxel index of this lane in slice d0
 #pragma unroll
         for (int hb = 0; hb < NH; ++hb) {
 #pragma unroll
           for (int sub = 0; sub < NSUB; ++sub) {
-            const int h = ht * HT + hb * 4 + trow0 + 2 * sub;
-            ok[hb][sub] = wok && h < a.H;
-            vx[hb][sub] = (((size_t)b * a.D + d0) * a.H + h) * a.W + w;
+            const int h = PD == 2 ? ht * (HT / 2) + trow0 : ht * HT + hb * 4 + trow0 + 2 * sub;
+            ok[hb][sub] = wok && h < Ho;
+            vx[hb][sub] = (((size_t)b * Dout + d0) * Ho + h) * Wo + (PD == 2 ? w >> 1 : w);
           }
         }
         for (int j = 0; j < nd; ++j) {
-          observe(cnt_base + (uint32_t)j + (KD == 3 ? 2u : 0u));
-          const uint32_t hslot = (cnt_base + j) % NSLOT;
+          const uint32_t js = PD == 2 ? 2u * j : (uint32_t)j;   // ring index of the window's first slab
+          observe(cnt_base + js + (PD == 2 ? 3u : (KD == 3 ? 2u : 0u)));
+          const uint32_t hslot = (cnt_base + js) % NSLOT;
 #pragma unroll
           for (int hb = 0; hb < NH; ++hb) {
             const bool mine = (int)(ecnt++ % NGRP) == grp;
@@ -311,13 +345,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                   if (valid && chan(i) < COUT) ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + chan(i), mreg[i]);
               }
               float acc[NF][NN / 2];
-              mma(hslot, hb, sub, acc);
+              mma(hslot, hb, sub, acc, (d0 + j) & 1);
 #pragma unroll
               for (int i = 0; i < NCH; ++i) {
                 const int c0 = chan(i);
                 float v[16];
                 combine(acc, i, v);
                 if (NSUB > 1 && c0 >= COUT) continue;            // (48 channels: the second warp pair has one chunk less)
+                if constexpr (PD == 2) {                         // coarse column: the sum of the w' pair (w, w + 1)
+#pragma unroll
+                  for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, v[c], 1);
+                }
                 if constexpr (EPI == 1) {
 #pragma unroll
                   for (int c = 0; c < 16; ++c) {
@@ -341,7 +379,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
               }
             }
           }
-          if (lane == 0) mbar_arrive(&empty[hslot]);    // this group no longer reads slab j
+          if (lane == 0) {                               // this group no longer reads slab js (PD 2: nor js + 1)
+            mbar_arrive(&empty[hslot]);
+            if (PD == 2) mbar_arrive(&empty[(hslot + 1) % NSLOT]);
+          }
         }
         release(nd);
       }
@@ -379,7 +420,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         }
         const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
         float acc[NF][NN / 2];
-        mma(hslot, hb, sub, acc);
+        mma(hslot, hb, sub, acc, 0);
         // 16 output channels at a time: the kw = 0, 1, 2 partial sums, shuffle-combined across lanes, stored
 #pragma unroll
         for (int i = 0; i < NCH; ++i) {
@@ -524,6 +565,11 @@ struct PackDesc {
   // channel block of an unfolded operand: operand output channels [n0, n0 + nb), input channels [k0, k0 + kb) (in the
   // operand's own orientation: transposed swaps the weight's Cout and Cin)
   int n0, nb, k0, kb;
+  // polyphase operand (conv_tcs_kernel PD): 1 = forward, group 0 (the upsampled source) holds W1 + W2 in its kd = 1
+  // tiles and 3 more group-0 tiles (one per kh) after the 9 steps hold W0 + W1; 2 = coarse dgrad, 4 x 4 (kd, kh) steps
+  // (step kd * 4 + kh) of transposed taps T0, T0 + T1, T1 + T2, T2 along both axes.  Merged taps are summed in fp32 (kd
+  // outer, kh inner) and rounded to bf16 once.
+  int poly;
 };
 __global__ void pack_weights_multi_kernel(const PackDesc* __restrict__ descs, int ndesc, int total) {
   for (int gi = blockIdx.x * blockDim.x + threadIdx.x; gi < total; gi += gridDim.x * blockDim.x) {
@@ -535,11 +581,31 @@ __global__ void pack_weights_multi_kernel(const PackDesc* __restrict__ descs, in
     const PackDesc d = descs[lo];
     const int i = gi - d.begin;
     const int T = d.KD * 9, CG = d.G0 + d.G1;
-    const int ci = i % CG, n = (i / CG) % d.NN, st = i / (CG * d.NN);
-    const int kd = st / 3, kh = st % 3, g = n / d.COUT, co = n % d.COUT;
+    const int base = d.KD * 3 * d.NN * CG;               // elements of the (kd, kh) step tiles
+    const bool extra = d.poly == 1 && i >= base;          // the W0 + W1 group-0 tiles of a polyphase forward operand
+    const int ie = i - base;
+    const int ci = extra ? ie % d.G0 : i % CG, n = extra ? (ie / d.G0) % d.NN : (i / CG) % d.NN;
+    const int st = extra ? ie / (d.G0 * d.NN) : i / (CG * d.NN);
+    const int kd = extra ? 0 : (d.poly == 2 ? st >> 2 : st / 3), kh = extra ? st : (d.poly == 2 ? st & 3 : st % 3);
+    const int g = n / d.COUT, co = n % d.COUT;
     const int tap = (kd * 3 + kh) * 3 + g;
     float v = 0.f;
-    if (d.fold) {
+    if (d.poly) {
+      if (co < d.nb && ci < d.kb) {
+        int t0 = kd, t1 = kd, u0 = kh, u1 = kh;            // the kd and kh taps merged into this tile
+        if (d.poly == 1 && ci < d.G0) t1 = extra ? 1 : (kd == 1 ? 2 : kd);
+        if (d.poly == 2) {                                 // 4 merged taps along d and along h: T0, T0 + T1, T1 + T2, T2
+          t0 = kd > 0 ? kd - 1 : 0; t1 = kd < 2 ? kd : 2;
+          u0 = kh > 0 ? kh - 1 : 0; u1 = kh < 2 ? kh : 2;
+        }
+        for (int t = t0; t <= t1; ++t)
+          for (int u = u0; u <= u1; ++u) {
+            const int tp = (t * 3 + u) * 3 + g;
+            v += !d.transposed ? d.w[((size_t)(d.n0 + co) * d.Cin + d.k0 + ci) * 27 + tp]
+                               : d.w[((size_t)(d.k0 + ci) * d.Cin + d.n0 + co) * 27 + (26 - tp)];
+          }
+      }
+    } else if (d.fold) {
       const int fk = ci / d.fold, c = ci % d.fold;              // folded kd tap, real input channel of the operand
       const int tap3 = (fk * 3 + kh) * 3 + g;
       if (fk < 3) {
@@ -552,9 +618,10 @@ __global__ void pack_weights_multi_kernel(const PackDesc* __restrict__ descs, in
     }
     const uint32_t W0 = d.G0 * 2, W1 = d.G1 * 2;
     uint32_t off;
-    if (ci < d.G0) off = swz((uint32_t)n * W0 + (uint32_t)ci * 2u, W0);
-    else off = (uint32_t)d.NN * W0 + swz((uint32_t)n * W1 + (uint32_t)(ci - d.G0) * 2u, W1);
-    d.out[((size_t)st * d.NN * (W0 + W1) + off) / 2] = __float2bfloat16_rn(v);
+    if (extra) off = (uint32_t)base * 2u + (uint32_t)(st * d.NN) * W0 + swz((uint32_t)n * W0 + (uint32_t)ci * 2u, W0);
+    else if (ci < d.G0) off = (uint32_t)(st * d.NN) * (W0 + W1) + swz((uint32_t)n * W0 + (uint32_t)ci * 2u, W0);
+    else off = (uint32_t)(st * d.NN) * (W0 + W1) + (uint32_t)d.NN * W0 + swz((uint32_t)n * W1 + (uint32_t)(ci - d.G0) * 2u, W1);
+    d.out[off / 2] = __float2bfloat16_rn(v);
   }
 }
 
@@ -628,7 +695,7 @@ extern "C" int vxm_conv3d_tcs_pack_desc_blk(void* desc_host, const float* w, voi
   PackDesc d;
   d.w = w; d.out = (__nv_bfloat16*)wpk; d.Cout = Cout; d.Cin = Cin; d.KD = kd; d.COUT = coutp; d.NN = 3 * coutp; d.G0 = g0; d.G1 = g1;
   d.transposed = transposed; d.begin = begin; d.count = kd * 3 * d.NN * (g0 + g1); d.fold = 0;
-  d.n0 = n0; d.nb = nb; d.k0 = k0; d.kb = kb;
+  d.n0 = n0; d.nb = nb; d.k0 = k0; d.kb = kb; d.poly = 0;
   memcpy(desc_host, &d, sizeof(d));
   return d.count;      // elements of this operand (>= 0), so the caller can chain `begin`
 }
@@ -651,7 +718,39 @@ extern "C" int vxm_conv3d_tcs_pack_desc_fold(void* desc_host, const float* w, vo
   PackDesc d;
   d.w = w; d.out = (__nv_bfloat16*)wpk; d.Cout = Cout; d.Cin = Cin; d.KD = 1; d.COUT = coutp; d.NN = 3 * coutp; d.G0 = g0; d.G1 = g1;
   d.transposed = transposed; d.begin = begin; d.count = 3 * d.NN * (g0 + g1); d.fold = real_in;
-  d.n0 = d.nb = d.k0 = d.kb = 0;
+  d.n0 = d.nb = d.k0 = d.kb = 0; d.poly = 0;
+  memcpy(desc_host, &d, sizeof(d));
+  return d.count;
+}
+
+// Polyphase operands of a 3-D concat layer whose first Ca input channels are a nearest-x2 upsampled source
+// (conv_tcs_kernel PD): mode 1 = forward ((Ca = 32) + (Cb = 16) -> Cout = 32), mode 2 = coarse dgrad (the Cout = 32
+// gradient channels -> the Ca = 32 channels of the coarse source).
+static int poly_geometry(int mode, int Cout, int Cin, int Ca, int* g0, int* g1, int* kd, int* coutp) {
+  if (mode == 1 && Ca == 32 && Cin == 48 && Cout == 32) { *g0 = 32; *g1 = 16; *kd = 3; *coutp = 32; return 1; }
+  if (mode == 2 && Ca == 32 && Cin > Ca && Cout == 32) { *g0 = 32; *g1 = 0; *kd = 4; *coutp = 32; return 1; }
+  return 0;
+}
+
+static size_t poly_bytes(int mode) {
+  const size_t NN = 3 * 32;
+  return (mode == 1 ? 9 * NN * (32 + 16) + 3 * NN * 32 : 16 * NN * 32) * sizeof(__nv_bfloat16);
+}
+
+extern "C" size_t vxm_conv3d_tcs_poly_packed_bytes(int mode, int Cout, int Cin, int Ca) {
+  int g0, g1, kd, coutp;
+  return poly_geometry(mode, Cout, Cin, Ca, &g0, &g1, &kd, &coutp) ? poly_bytes(mode) : 0;
+}
+
+extern "C" int vxm_conv3d_tcs_pack_desc_poly(void* desc_host, const float* w, void* wpk, int Cout, int Cin, int Ca, int mode, int begin) {
+  int g0, g1, kd, coutp;
+  VXM_REQUIRE(desc_host && w && wpk && poly_geometry(mode, Cout, Cin, Ca, &g0, &g1, &kd, &coutp),
+              "conv3d_tcs_pack_desc_poly: no polyphase operand for mode %d, (%d of %d) -> %d", mode, Ca, Cin, Cout);
+  PackDesc d;
+  d.w = w; d.out = (__nv_bfloat16*)wpk; d.Cout = Cout; d.Cin = Cin; d.KD = kd; d.COUT = coutp; d.NN = 3 * coutp; d.G0 = g0; d.G1 = g1;
+  d.transposed = mode == 2; d.begin = begin; d.fold = 0; d.poly = mode;
+  d.n0 = 0; d.nb = mode == 1 ? Cout : Ca; d.k0 = 0; d.kb = mode == 1 ? Cin : Cout;
+  d.count = (int)(vxm_conv3d_tcs_poly_packed_bytes(mode, Cout, Cin, Ca) / sizeof(__nv_bfloat16));
   memcpy(desc_host, &d, sizeof(d));
   return d.count;
 }
@@ -671,7 +770,20 @@ extern "C" int vxm_conv3d_tcs_supported(int Ca, int Cb, int Cout) {
 
 static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                            int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, void* stream);
+                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, int poly,
+                           void* stream);
+
+// Polyphase launches (conv_tcs_kernel PD, operands from vxm_conv3d_tcs_pack_desc_poly).  mode 1: forward of a
+// (32 upsampled + 16) -> 32 concat layer, bias + LeakyReLU, bf16 (B, D, H, W, 32) out; xa is the coarse source, (D, H, W)
+// the fine grid.  mode 2: xa = the 32-channel gradient (B, D, H, W, 32) of a layer whose first 32 input channels are an
+// upsampled source, mask = that source (B, D / 2, H / 2, W / 2, 32), its LeakyReLU activation; out = the gradient w.r.t.
+// it, (B, D / 2, H / 2, W / 2, 32), times the LeakyReLU derivative (slope).
+extern "C" int vxm_conv3d_tcs_poly(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask, int B,
+                                   int D, int H, int W, int Ca, int Cb, int Cout, int mode, float slope, void* stream) {
+  VXM_REQUIRE(mode == 1 || mode == 2, "conv3d_tcs_poly: mode must be 1 (forward) or 2 (coarse dgrad)");
+  return conv_tcs_launch(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, mode == 1 ? 1 : 0, Cout, 32, 3, 0, slope, nullptr, 0,
+                         nullptr, nullptr, 0, mode, stream);
+}
 
 // shared memory of one launch outside the slab ring: packed weights, accumulator read-out buffers, barriers
 static size_t fixed_smem(uint32_t wbytes) { return ((wbytes + 1023u) & ~1023u) + NGRP * ACC_STAGE_FLOATS * sizeof(float) + 1024 + 512; }
@@ -688,7 +800,7 @@ extern "C" int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wp
                                   float slope, void* out2, int csplit, void* stream) {
   VXM_REQUIRE(out_mode == 0 || out_mode == 1, "conv3d_tcs_fwd: out_mode must be 0 (bf16 channels-last) or 1 (fp32 planar)");
   return conv_tcs_launch(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, out2, csplit,
-                         nullptr, nullptr, 0, stream);
+                         nullptr, nullptr, 0, 0, stream);
 }
 
 extern "C" int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
@@ -698,7 +810,7 @@ extern "C" int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void
   VXM_REQUIRE(out_mode != 3 || out_lo, "conv3d_tcs_fwd_blk: out_mode 3 needs out_lo");
   VXM_REQUIRE(opitch == 0 || (opitch >= Cout && opitch % 8 == 0 && out_mode != 2), "conv3d_tcs_fwd_blk: bad output pitch %d", opitch);
   return conv_tcs_launch(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, nullptr, 0,
-                         acc_in, out_lo, opitch == Cout ? 0 : opitch, stream);
+                         acc_in, out_lo, opitch == Cout ? 0 : opitch, 0, stream);
 }
 
 extern "C" int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
@@ -713,12 +825,13 @@ extern "C" int vxm_conv3d_tcs_fwd_acc(const void* xa, const void* xb, const void
   VXM_REQUIRE(out_mode >= 1 && out_mode <= 3, "conv3d_tcs_fwd_acc: out_mode must be 1 (fp32 planar), 2 (fp32 partial sums) or 3 (bf16 hi/lo pair)");
   VXM_REQUIRE(out_mode != 3 || out_lo, "conv3d_tcs_fwd_acc: out_mode 3 needs out_lo");
   return conv_tcs_launch(xa, xb, wpk, bias, out, nullptr, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, nullptr, 0,
-                         acc_in, out_lo, 0, stream);
+                         acc_in, out_lo, 0, 0, stream);
 }
 
 static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                            int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, void* stream) {
+                           float slope, void* out2, int csplit, const float* acc_in, void* out_lo, int opitch, int poly,
+                           void* stream) {
   VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0 && wpk && out, "conv3d_tcs_fwd: bad argument");
   VXM_REQUIRE(kd == 1 || kd == 3, "conv3d_tcs_fwd: kd must be 1 or 3");
   VXM_REQUIRE(coutp == 16 || coutp == 32 || coutp == 48 || coutp == 64, "conv3d_tcs_fwd: padded Cout must be 16, 32, 48 or 64");
@@ -727,6 +840,10 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   VXM_REQUIRE(vxm_conv3d_tcs_supported(Ca, Cb, Cout), "conv3d_tcs_fwd: channel counts (%d,%d)->%d unsupported", Ca, Cb, Cout);
   VXM_REQUIRE((Ca == 0 || xa) && (Cb == 0 || xb), "conv3d_tcs_fwd: missing source tensor");
   VXM_REQUIRE(!up || (H % 2 == 0 && W % 2 == 0 && (kd == 1 || D % 2 == 0)), "conv3d_tcs_fwd: upsampled source needs even sizes");
+  VXM_REQUIRE(poly == 0 || (kd == 3 && coutp == 32 && Cout == 32 && out_mode == 0 && !out2 && !acc_in && !opitch &&
+                            (poly == 1 ? up && Ca == 32 && Cb == 16 && bias && !mask && slope >= 0.f && slope <= 1.f
+                                       : !up && Ca == 32 && Cb == 0 && !bias && mask && D % 2 == 0 && H % 2 == 0 && W % 2 == 0)),
+              "conv3d_tcs_poly: no polyphase mode %d kernel for (%d,%d)->%d", poly, Ca, Cb, Cout);
   ConvSArgs a{};
   const int cin = Ca + Cb;
   int g0, g1;
@@ -739,7 +856,7 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   // the channel-blocked launches: 32-channel blocks of a 3-D layer, K groups of 64 or 32 + 16 channels (see tc.conv_blocks)
   VXM_REQUIRE(!opitch || (!out2 && out_mode != 1 && kd == 3 && coutp == 32 && ((g0 == 64 && g1 == 0) || (g0 == 32 && g1 == 16))),
               "conv3d_tcs_fwd: no blocked kernel for (%d,%d)->%d/%d, kd %d", Ca, Cb, Cout, coutp, kd);
-  a.wbytes = (uint32_t)vxm_conv3d_tcs_packed_bytes(cin, coutp, kd);
+  a.wbytes = (uint32_t)(poly ? poly_bytes(poly) : vxm_conv3d_tcs_packed_bytes(cin, coutp, kd));
   const size_t fixed = fixed_smem(a.wbytes);
   // tile height: 8 rows (two tile halves per slab step, one per MMA warpgroup) when the ring still holds >= 5 slabs
   int HTv = 4;
@@ -748,6 +865,7 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     const int ns8 = (int)((227 * 1024 - fixed) / slab8);
     const char* e = getenv("VXM_B200_TCS_HT");
     if (g0 <= 32 && coutp <= 32 && ns8 >= (kd == 3 ? 5 : 3) && H > 4 && !(e && e[0] == '4') && !opitch) HTv = 8;
+    if (poly) HTv = poly == 2 ? 8 : 4;               // the polyphase kernels exist at one tile height each
   }
   a.tiles_h = (H + HTv - 1) / HTv; a.tiles_w = (W + WUSE - 1) / WUSE;
   int nsm = sm_count();
@@ -755,14 +873,16 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
   int best_nch = 1;
   double best_cost = 1e300;
-  for (int nch = 1; nch <= 40 && nch <= D; ++nch) {
-    const int dc = (D + nch - 1) / nch;
-    const long long items = tiles * ((D + dc - 1) / dc);
+  // (the coarse dgrad: output slices of 2 fine slabs each, so the halo weighs half as much)
+  const int Do = poly == 2 ? D / 2 : D;
+  for (int nch = 1; nch <= 40 && nch <= Do; ++nch) {
+    const int dc = (Do + nch - 1) / nch;
+    const long long items = tiles * ((Do + dc - 1) / dc);
     const long long waves = (items + nsm - 1) / nsm;
-    const double cost = (double)waves * (dc + (kd == 3 ? 2.5 : 0.5));
+    const double cost = (double)waves * (dc + (poly == 2 ? 1.25 : (kd == 3 ? 2.5 : 0.5)));
     if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
   }
-  a.dchunk = (D + best_nch - 1) / best_nch; a.nchunks = (D + a.dchunk - 1) / a.dchunk;
+  a.dchunk = (Do + best_nch - 1) / best_nch; a.nchunks = (Do + a.dchunk - 1) / a.dchunk;
   a.nitems = (int)(tiles * a.nchunks);
   const size_t slab = (size_t)(HTv + 2) * WT * (g0 + g1) * 2;
   int nslot = (int)((227 * 1024 - fixed) / slab);
@@ -779,7 +899,7 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   size_t smem = fixed + (size_t)nslot * slab;
   int grid = a.nitems < nsm ? a.nitems : nsm;
   cudaStream_t st = as_stream(stream);
-  if (plan_tma(a, g0, g1, HTv) != 0) return VXM_ERR_CUDA;
+  if (poly != 2 && plan_tma(a, g0, g1, HTv) != 0) return VXM_ERR_CUDA;   // (the coarse dgrad permutes its slab rows)
   const bool acc_epi = acc_in != nullptr || out_mode >= 2;
   // epilogue specialisation: 3-D, bf16 channels-last output, every padded channel real
   int epi = 0;
@@ -789,6 +909,7 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     if (plain && !out2 && !mask && slope >= 0.f && slope <= 1.f) epi = 1;
     else if (plain && !out2 && mask && !bias) epi = 2;
     else if (plain && !mask && !bias && slope < 0.f && (!out2 || csplit % 16 == 0)) epi = 3;
+    if (poly) epi = poly;               // the polyphase forms exist with their specialised epilogue only
   }
 #define VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, ACC_, E_, ...)                                                                  \
   do {                                                                                                                            \
@@ -825,7 +946,10 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     else if (g0 == 32) VXM_TCS_LAUNCH(KD_, 32, 16, CO_, 4);                   \
     else VXM_TCS_LAUNCH(KD_, 64, 0, CO_, 4);                                  \
   } while (0)
-  if (opitch) {
+  if (poly) {
+    if (poly == 1) VXM_TCS_LAUNCH_E(3, 32, 16, 32, 4, false, 1, false, 1);
+    else VXM_TCS_LAUNCH_E(3, 32, 0, 32, 8, false, 2, false, 2);
+  } else if (opitch) {
     if (g0 == 64) VXM_TCS_LAUNCH_OP(64, 0); else VXM_TCS_LAUNCH_OP(32, 16);
   } else if (HTv == 8) {
     if (kd == 3) { if (coutp == 16) VXM_TCS_G8(3, 16); else VXM_TCS_G8(3, 32); }

@@ -23,9 +23,10 @@ def bump_weights_epoch():
 class _Layer:
     """One convolution of a model's plan: its parameters, its inputs (tensor ids of the walk: 0 = the images, then every
     convolution and pooling output in execution order) and how it runs.  `fwd` / `dgrad`: the execution form of the
-    forward and of the dgrad (see _run); `fwd_x3`: the block grid of the split-precision forward."""
+    forward and of the dgrad (see _run); `fwd_x3`: the block grid of the split-precision forward; `dgrad_skip`: with a
+    polyphase dgrad, the form of the skip part (the dgrad's own form then yields the upsampled part only)."""
     __slots__ = ("w", "bias", "slope", "role", "a", "b", "out", "up", "ca", "cb", "cin", "cout", "fwd", "fwd_x3", "dgrad", "khm",
-                 "pk_fwd", "pk_dgrad", "pk_hi", "pk_lo", "w_hi", "w_lo")
+                 "dgrad_skip", "pk_fwd", "pk_dgrad", "pk_dgrad_skip", "pk_hi", "pk_lo", "w_hi", "w_lo")
 
 
 def _refuse(what):
@@ -53,6 +54,7 @@ def _walk(model):
         _refuse("2-D or 3-D convolutions only")
     kd = 3 if w0.dim() == 5 else 1
     fold = kd == 3 and tc.kdfold_enabled()
+    poly = kd == 3 and tc.polyphase_enabled()
     ops = []
     chans = [8]           # channels of every tensor id: the images enter as one bf16 channels-last tensor of 8 channels
     cur, pending_up, skips = 0, None, [None]
@@ -89,6 +91,16 @@ def _walk(model):
             L.dgrad = "fold"
         else:                             # the flow gradient enters as 8 channels; a concatenation's dgrad splits its output
             L.dgrad = _form(8 if role == "flow" else L.cout, 0, L.cin, kd, L.cout, L.ca if L.b is not None else None)
+        # polyphase forms of a concatenation with a 32-channel upsampled source (taps that read the same coarse voxel
+        # merged): the forward of 32 + 16 -> 32 (kd), and the dgrad as a coarse launch for the upsampled source (kd, kh;
+        # LeakyReLU derivative included) plus a fine launch for the skip channels
+        L.dgrad_skip = None
+        if poly and L.up and L.b is not None and L.ca == 32 and L.cout == 32:
+            if L.cb == 16:
+                L.fwd = ("poly", 1, L.ca)
+            L.dgrad = ("poly", 2, L.ca)
+            L.dgrad_skip = (((2, 0, L.cout),), ((L.ca, L.cb, 0, 0),))
+            _form(L.cout, 0, L.cb, kd, L.cout)          # (refuses a skip width no launch takes)
         L.khm = L.cout <= 16              # weight gradient of the folded first layer: kh-in-M takes at most 16 outputs
         L.out = cur = len(chans)
         chans.append(L.cout)
@@ -143,12 +155,14 @@ class _Plan:
         for L in self.layers:
             w = L.w.detach()
             L.w_hi, L.w_lo = torch.empty_like(w), torch.empty_like(w)
-            bf16 += [(w, False, L.fwd)] + ([(w, True, L.dgrad)] if L.dgrad is not None else [])
+            bf16 += [(w, False, L.fwd)] + ([(w, True, L.dgrad)] if L.dgrad is not None else []) + \
+                    ([(w, True, L.dgrad_skip)] if L.dgrad_skip is not None else [])
             x3 += [(L.w_hi, False, L.fwd_x3), (L.w_lo, False, L.fwd_x3)]
         self.bf16, self.x3 = tc.PackTable(bf16), tc.PackTable(x3)
         packs, packs3 = iter(self.bf16.packs), iter(self.x3.packs)
         for L in self.layers:
             L.pk_fwd, L.pk_dgrad = next(packs), (next(packs) if L.dgrad is not None else None)
+            L.pk_dgrad_skip = next(packs) if L.dgrad_skip is not None else None
             L.pk_hi, L.pk_lo = next(packs3), next(packs3)
         self.ptrs = self.weight_ptrs()
         self.stamps = [None, None]
@@ -214,7 +228,11 @@ def _unpool_combine(e_fine, g_skip, g_pool, nd, slope):
 def _run(form, packs, xa, xb, nout, kd, bias=None, lo=None, **kw):
     """The engine's one kernel selection: runs a convolution of the plan (a forward, or a dgrad on the transposed operand) in
     its execution form.  "fold": one 2-D launch over kd-folded channels; a 1 x 1 grid: one launch of the swizzled
-    kw-stacked kernel (tc.conv_fwd_t); channel blocks, and every split-precision forward (lo): tc.conv_fwd_blocked."""
+    kw-stacked kernel (tc.conv_fwd_t); ("poly", mode, ca): a polyphase launch (tc.conv_fwd_poly; tc.dgrad_poly, whose
+    `mask` is the coarse activation); channel blocks, and every split-precision forward (lo): tc.conv_fwd_blocked."""
+    if form[0] == "poly":
+        wpk = packs[0, 0][0]
+        return tc.conv_fwd_poly(xa, xb, wpk, bias, nout, kw["slope"]) if form[1] == 1 else tc.dgrad_poly(xa, wpk, kw["mask"], kw["slope"])
     if form == "fold" or (lo is None and len(form[0]) == len(form[1]) == 1):
         wpk, coutp = packs[0, 0]
         return tc.conv_fwd_t(xa, xb, wpk, (coutp, "s"), bias, nout, 1 if form == "fold" else kd, **kw)
@@ -335,6 +353,10 @@ def backward_tape(ctx, g_flow):
             sl = plan.slope.get(t)         # None: a pooling output, no activation to differentiate
             res = _run(L.dgrad, L.pk_dgrad, g_in, None, L.cin, kd, slope=sl, mask=None if sl is None else tensors[t])
             (graw if sl is None else gz)[t] = res
+        elif L.dgrad_skip is not None:
+            # polyphase: the coarse source's gradient (its 8 children summed, LeakyReLU derivative applied) in one launch
+            gz[t] = _run(L.dgrad, L.pk_dgrad, g_in, None, L.ca, kd, mask=tensors[t], slope=plan.slope[t])
+            gskip[L.b] = _run(L.dgrad_skip, L.pk_dgrad_skip, g_in, None, L.cb, kd)
         else:
             # single dgrad pass over the whole concat input: N = Ca + Cb output channels, split on store
             g_up, g_sk = _run(L.dgrad, L.pk_dgrad, g_in, None, L.cin, kd, split=L.ca)

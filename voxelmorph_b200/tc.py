@@ -157,6 +157,46 @@ def kdfold_enabled():
     return os.environ.get("VXM_B200_KDFOLD", "1") != "0"
 
 
+def polyphase_enabled():
+    """Polyphase execution of the 3-D concat layers with a 32-channel upsampled source (VXM_B200_POLYPHASE=0: A/B
+    switch back to the 27-tap forms over the duplicated slices)."""
+    import os
+    return os.environ.get("VXM_B200_POLYPHASE", "1") != "0"
+
+
+def pack_weights_poly(w, mode, ca):
+    """Packed polyphase operand (vxm_conv3d_tcs_pack_desc_poly) of the 3-D weight w (Cout, Cin, 3, 3, 3) of a concat
+    layer whose first `ca` input channels are upsampled: mode 1 forward, 2 coarse dgrad.  Stand-alone helper (tests /
+    tools); the engine packs through its model plan."""
+    table = PackTable([(w.contiguous(), mode == 2, ("poly", mode, ca))])
+    table.refresh()
+    torch.cuda.current_stream(w.device).synchronize()       # the descriptor table must outlive the launch
+    return table.packs[0][0, 0][0]
+
+
+def conv_fwd_poly(xa, xb, wpk, bias, cout, slope):
+    """Forward of a (32 upsampled + 16) -> 32 concat layer on its polyphase operand: xa the coarse source, xb the skip
+    (B, D, H, W, 16); bias + LeakyReLU; returns bf16 (B, D, H, W, cout)."""
+    lib = _lib.load()
+    B, D, H, W = xb.shape[:4]
+    out = torch.empty((B, D, H, W, cout), dtype=torch.bfloat16, device=xb.device)
+    _lib.check(lib.vxm_conv3d_tcs_poly(_lib.ptr(xa), _lib.ptr(xb), _lib.ptr(wpk), _lib.ptr(bias), _lib.ptr(out), None, B, D, H, W,
+                                       xa.shape[-1], xb.shape[-1], cout, 1, float(slope), _lib.stream_ptr()), "vxm_conv3d_tcs_poly")
+    return out
+
+
+def dgrad_poly(g, wpk, act, slope):
+    """Coarse dgrad on the polyphase operand: g (B, D, H, W, 32) the layer's output gradient, act (B, D / 2, H / 2, W / 2, C)
+    the upsampled source, a LeakyReLU activation of negative slope `slope` -> bf16 (B, D / 2, H / 2, W / 2, C), the gradient
+    w.r.t. that source's pre-activation (sum over its 8 children, times the LeakyReLU derivative)."""
+    lib = _lib.load()
+    B, D, H, W, C = g.shape
+    out = torch.empty_like(act)
+    _lib.check(lib.vxm_conv3d_tcs_poly(_lib.ptr(g), None, _lib.ptr(wpk), None, _lib.ptr(out), _lib.ptr(act), B, D, H, W, C, 0,
+                                       act.shape[-1], 2, float(slope), _lib.stream_ptr()), "vxm_conv3d_tcs_poly")
+    return out
+
+
 def planar_fold_kd(planes, cout):
     """<= cout/3 planar fp32 (B,1,D,H,W) volumes -> bf16 (B,D,H,W,cout) with channel kd * n + p = plane p at slice d + kd - 1
     (zero outside the volume): the kd taps of a 3-D convolution folded into the channels (csrc/ndhwc_ops.cu)."""
@@ -260,22 +300,28 @@ def one_block(cin, nout):
 
 class PackTable:
     """Packed bf16 operands of several weights, all refreshed by ONE vxm_conv3d_tcs_pack_multi launch.  `operands`:
-    [(w, transposed, form)] with form "fold" (the kd-folded 2-D operand of a 3-D weight, see vxm_conv3d_tcs_pack_desc_fold)
-    or channel blocks (conv_blocks, one_block).  packs[i] = {(ki, ni): (tensor, coutp)} of operand i ((0, 0) for a folded
-    one).  The descriptor table is uploaded once and points at the (contiguous fp32) weights themselves, so `refresh`
-    repacks their current values and can be captured in a CUDA graph."""
+    [(w, transposed, form)] with form "fold" (the kd-folded 2-D operand of a 3-D weight, see vxm_conv3d_tcs_pack_desc_fold),
+    ("poly", mode, ca) (a polyphase operand, see vxm_conv3d_tcs_pack_desc_poly) or channel blocks (conv_blocks,
+    one_block).  packs[i] = {(ki, ni): (tensor, coutp)} of operand i ((0, 0) for a folded or polyphase one).  The
+    descriptor table is uploaded once and points at the (contiguous fp32) weights themselves, so `refresh` repacks their
+    current values and can be captured in a CUDA graph."""
 
     def __init__(self, operands):
         lib = _lib.load()
         dsz = int(lib.vxm_conv3d_tcs_pack_desc_bytes())
-        host = ctypes.create_string_buffer(dsz * sum(1 if f == "fold" else len(f[0]) * len(f[1]) for _, _, f in operands))
+        host = ctypes.create_string_buffer(dsz * sum(1 if f == "fold" or f[0] == "poly" else len(f[0]) * len(f[1]) for _, _, f in operands))
         self.packs, self.n, self.total = [], 0, 0
         for w, transposed, form in operands:
             w5 = w if w.dim() == 5 else w.unsqueeze(2)
             Cout, Cin, kd = w5.shape[0], w5.shape[1], w5.shape[2]
             t = 1 if transposed else 0
             packs = {}
-            if form == "fold":
+            if form != "fold" and form[0] == "poly":
+                _, mode, ca = form
+                out = torch.empty(int(lib.vxm_conv3d_tcs_poly_packed_bytes(mode, Cout, Cin, ca)) // 2, dtype=torch.bfloat16, device=w.device)
+                cnt = lib.vxm_conv3d_tcs_pack_desc_poly(self._slot(host, dsz), _lib.ptr(w5), _lib.ptr(out), Cout, Cin, ca, mode, self.total)
+                self._add(packs, (0, 0), out, 32, cnt)
+            elif form == "fold":
                 real_in, nout = (Cout, Cin) if transposed else (Cin, Cout)
                 coutp = 16 if nout <= 16 else 32
                 out = torch.empty(int(lib.vxm_conv3d_tcs_packed_bytes(3 * real_in, coutp, 1)) // 2, dtype=torch.bfloat16, device=w.device)
