@@ -1,0 +1,386 @@
+"""Every tensor-core convolution launch of the training step, checked exactly at the step's own size, and the persistent
+kernels' item loops checked under every decomposition a GPU with 1, 2, 5 or 13 SMs would run (VXM_B200_CONV_CTAS).
+
+Operands are chosen so that every fp32 sum the kernels form is exact, whatever the MMA or reduction order: activations
+and gradients in {-1, 0, 1} (each nonzero with probability 1/2), weights and biases 2^-6 k with |k| <= 8 (merged polyphase
+taps |k| <= 32, still bf16-exact), image and flow-gradient planes in {-1, 0, 1} / 16.  Every product and partial sum is
+then an integer multiple of one power of two below 2^24 of those units; the test asserts the bounds (printed as the
+margin: the bound over 2^24) rather than assuming them.  The kernels' results must equal the fp64 tap sums of
+conv_exact_ref.py, with the epilogue (bias add, LeakyReLU or its derivative with the model's slope 0.2, bf16 rounding)
+emulated in fp32: any dropped, doubled or misplaced contribution fails.  Run with -s to print every launch's mismatch
+count next to its margin."""
+import pytest
+import torch
+
+import conv_exact_ref as ref
+
+pytestmark = pytest.mark.gpu
+
+SLOPE = 0.2                      # the model's LeakyReLU slope: its fp32 products round, as in the step
+PLANE = 2.0 ** -4                # image and flow-gradient planes: {-1, 0, 1} * PLANE
+DOUBLED = [[32, 64, 64, 64], [64, 64, 64, 64, 64, 32, 32]]
+CAPS = ["1", "2", "5", "13", None]
+
+
+@pytest.fixture(scope="module")
+def vx(cuda):
+    import voxelmorph_b200 as vxm
+    from voxelmorph_b200 import engine_bf16, tc
+    vxm._lib.load()
+    return vxm, engine_bf16, tc
+
+
+def ternary(shape, g, dtype=torch.bfloat16):
+    """{-1, 0, 1}, each nonzero with probability 1/2"""
+    nz = torch.randint(0, 2, shape, generator=g, device=g.device)
+    return (nz * (2 * torch.randint(0, 2, shape, generator=g, device=g.device) - 1)).to(dtype)
+
+
+def qweight(shape, g):
+    return torch.randint(-8, 9, shape, generator=g, device=g.device).float() * 2.0 ** -6
+
+
+def mism(a, b):
+    assert a.shape == b.shape, (a.shape, b.shape)
+    return int((a != b.to(a.dtype)).sum())
+
+
+def _margin(cin, children=1):
+    """bound on |partial sums| of a forward / dgrad over 2^24, in units of (operand unit) x 2^-6: 27 taps x cin channels x
+    |x| <= 1 unit x |w| <= 8 units (merged taps partition the same terms), x 8 for a sum over upsampled children, plus a bias
+    of <= 8 units of 2^-6 (128 units of the image planes' 2^-10)"""
+    return (27 * cin * 8 * children + 128) / 2 ** 24
+
+
+def _form_name(f, split=False):
+    if f == "fold":
+        return "kd-folded"
+    if f[0] == "poly":
+        return "polyphase %s" % ("forward" if f[1] == 1 else "coarse")
+    kind = "one launch" if len(f[0]) == len(f[1]) == 1 else "%dx%d blocks" % (len(f[0]), len(f[1]))
+    return kind + (" split" if split else "")
+
+
+def _report(title, rows):
+    """rows (launch, form, mismatches, margin): every mismatch count must be 0 and every margin below 1/4"""
+    print("\n[%s] launch | form | mismatches (expected 0) | margin" % title)
+    for name, form, n, margin in rows:
+        print("  %-34s %-26s %8d   %.2e" % (name, form, n, margin))
+    bad = [r for r in rows if r[2] or r[3] >= 0.25]
+    assert not bad, bad
+
+
+# ---- a. every convolution of the plan, exactly, at the plan's own size -------------------------------------------------
+
+MODELS = {"default": dict(inshape=(160, 192, 224)), "doubled": dict(inshape=(64, 96, 112), nb_unet_features=DOUBLED)}
+
+
+@pytest.mark.parametrize("forms", ["polyphase+kdfold", "split+unfolded"])
+@pytest.mark.parametrize("name", sorted(MODELS))
+def test_plan_launches_exact(vx, cuda, monkeypatch, name, forms):
+    """Forward, dgrad and weight gradient of every layer of the plan through the engine's own calls (_run, WgradBatch), with
+    the arguments forward_tape / backward_tape pass.  "split+unfolded" (VXM_B200_POLYPHASE=0, VXM_B200_KDFOLD=0) runs the
+    layers whose form that changes."""
+    vxm, eng, tc = vx
+    kw = MODELS[name]
+    g = torch.Generator(device=cuda).manual_seed(1 + len(name))
+    model = vxm.networks.VxmDense(**kw).to(cuda)
+    with torch.no_grad():
+        for p in model.parameters():
+            p.copy_(qweight(p.shape, g))
+    monkeypatch.setenv("VXM_B200_POLYPHASE", "1")
+    monkeypatch.setenv("VXM_B200_KDFOLD", "1")
+    base = [L for L in eng._walk(model) if isinstance(L, eng._Layer)]
+    if forms == "split+unfolded":
+        monkeypatch.setenv("VXM_B200_POLYPHASE", "0")
+        monkeypatch.setenv("VXM_B200_KDFOLD", "0")
+    plan = eng._plan_of(model, False)
+    layers = plan.layers
+    only = {i for i, (L, L0) in enumerate(zip(layers, base)) if forms == "polyphase+kdfold" or L.fwd != L0.fwd or L.dgrad != L0.dgrad}
+    assert only
+    if forms == "polyphase+kdfold":
+        assert layers[0].fwd == "fold"
+        if name == "default":
+            assert sum(1 for L in layers if L.dgrad_skip is not None) == 4 and layers[-1].dgrad == "fold"
+    # shapes and channels of every tensor id from the plan: 0 = the images, a pool halves, a convolution after an upsample
+    # works at its skip's (twice its source's) size
+    size, chans = {0: tuple(kw["inshape"])}, {}
+    for op in plan.ops:
+        if isinstance(op, eng._Layer):
+            size[op.out], chans[op.out] = size[op.b if op.b is not None else op.a], op.cout
+        else:
+            _, s, d = op
+            size[d], chans[d] = tuple(v // 2 for v in size[s]), chans[s]
+    first, flow = layers[0], layers[-1]
+    B = 1
+    planes = [ternary((B, 1) + size[0], g, torch.float32) * PLANE for _ in range(first.cin)]
+    images = torch.cat(planes, 1).permute(0, 2, 3, 4, 1)
+    X = {i: ternary((B,) + size[i] + (c,), g) for i, c in chans.items() if i != flow.out}
+    X[0] = tc.planar_fold_kd(planes, 8) if first.fwd == "fold" else tc.planar_to_ndhwc8(planes)
+    G = {L.out: ternary((B,) + size[L.out] + (L.cout,), g) for L in layers if L is not flow}
+    gplanes = [ternary((B, 1) + size[flow.out], g, torch.float32) * PLANE for _ in range(flow.cout)]
+    gflow = torch.cat(gplanes, 1).permute(0, 2, 3, 4, 1)
+    for L in layers:
+        assert bool(((L.w * 64).abs() <= 8).all()) and bool(((L.bias * 64).abs() <= 8).all())
+
+    def srcs(L):
+        return [(images, False)] if L is first else [(X[L.a], L.up)] + ([(X[L.b], False)] if L.b is not None else [])
+
+    def lname(i, L):
+        return "%02d %s (%d%s+%d)->%d %s" % (i, L.role, L.ca, "^" if L.up else "", L.cb, L.cout, "x".join(map(str, size[L.out])))
+
+    rows = []
+    for i, L in enumerate(layers):
+        if i not in only:
+            continue
+        w, bias, D = L.w.detach(), L.bias.detach(), size[L.out][0]
+        # ---- forward ----
+        out = eng._run(L.fwd, L.pk_fwd, X[0] if L is first else X[L.a], X.get(L.b), L.cout, 3, bias, up=L.up, slope=L.slope,
+                       out_fp32_planar=L is flow)
+        if L is flow:
+            out = out.permute(0, 2, 3, 4, 1)
+        n = sum(ref.conv(srcs(L), w, D, finish=lambda y, d0, d1: mism(out[:, d0:d1], ref.epilogue(y, bias, L.slope, bf16=L is not flow))))
+        rows.append((lname(i, L), "fwd " + _form_name(L.fwd), n, _margin(L.cin)))
+        # ---- dgrad, in the plan's form ----
+        if L.dgrad is None:
+            continue
+        wt = ref.dgrad_weight(w)
+        if L is flow:
+            g_in = tc.planar_fold_kd(gplanes, 16) if L.dgrad == "fold" else tc.planar_to_ndhwc8(gplanes)
+            sl, mask = plan.slope[L.a], X[L.a]
+            res = eng._run(L.dgrad, L.pk_dgrad, g_in, None, L.cin, 3, slope=sl, mask=mask)
+            n = sum(ref.conv([(gflow, False)], wt, D, finish=lambda y, d0, d1: mism(res[:, d0:d1], ref.epilogue(y, slope=sl, mask=mask[:, d0:d1]))))
+            rows.append((lname(i, L), "dgrad " + _form_name(L.dgrad), n, _margin(L.cout)))
+        elif L.b is None:
+            sl = plan.slope.get(L.a)        # None: a pooling output, no activation to differentiate
+            mask = None if sl is None else X[L.a]
+            res = eng._run(L.dgrad, L.pk_dgrad, G[L.out], None, L.cin, 3, slope=sl, mask=mask)
+            n = sum(ref.conv([(G[L.out], False)], wt, D, finish=lambda y, d0, d1: mism(
+                res[:, d0:d1], ref.epilogue(y, slope=sl, mask=None if mask is None else mask[:, d0:d1]))))
+            rows.append((lname(i, L), "dgrad " + _form_name(L.dgrad) + (" masked" if mask is not None else ""), n, _margin(L.cout)))
+        elif L.dgrad_skip is not None:
+            sl, act = plan.slope[L.a], X[L.a]
+            coarse = eng._run(L.dgrad, L.pk_dgrad, G[L.out], None, L.ca, 3, mask=act, slope=sl)
+            skip = eng._run(L.dgrad_skip, L.pk_dgrad_skip, G[L.out], None, L.cb, 3)
+            ns = ref.conv([(G[L.out], False)], wt, D, finish=lambda y, d0, d1: (
+                mism(coarse[:, d0 // 2:d1 // 2], ref.epilogue(ref.children_sum(y[..., :L.ca]), slope=sl, mask=act[:, d0 // 2:d1 // 2])),
+                mism(skip[:, d0:d1], ref.epilogue(y[..., L.ca:]))))
+            rows.append((lname(i, L), "dgrad " + _form_name(L.dgrad), sum(a for a, _ in ns), _margin(L.cout, 8)))
+            rows.append((lname(i, L), "dgrad skip " + _form_name(L.dgrad_skip), sum(b for _, b in ns), _margin(L.cout)))
+        else:
+            sl, act = plan.slope[L.a], X[L.a]
+            g_up, g_sk = eng._run(L.dgrad, L.pk_dgrad, G[L.out], None, L.cin, 3, split=L.ca)
+            gzc = eng._sumpool_mask(g_up, act, 3, sl)
+
+            def fin(y, d0, d1):
+                up = ref.epilogue(y[..., :L.ca])
+                return (mism(g_up[:, d0:d1], up), mism(g_sk[:, d0:d1], ref.epilogue(y[..., L.ca:])),
+                        mism(gzc[:, d0 // 2:d1 // 2], ref.epilogue(ref.children_sum(up.double()), slope=sl, mask=act[:, d0 // 2:d1 // 2])))
+            ns = ref.conv([(G[L.out], False)], wt, D, finish=fin)
+            rows.append((lname(i, L), "dgrad " + _form_name(L.dgrad, True), sum(a + b for a, b, _ in ns), _margin(L.cout)))
+            rows.append((lname(i, L), "sumpool_mask", sum(c for _, _, c in ns), _margin(L.cout, 8)))
+        del out
+    # ---- weight gradients: every layer into one WgradBatch in backward_tape's order, one flush; fresh, then accumulated ----
+    refs = {}
+    for i, L in enumerate(layers):
+        if i in only:
+            gz = gflow if L is flow else G[L.out]
+            wunit, bunit = (PLANE if L is first or L is flow else 1.0), (PLANE if L is flow else 1.0)    # x * gz, gz
+            gw, gb = ref.wgrad(srcs(L), gz)
+            aw, ab = ref.wgrad(srcs(L), gz, absolute=True)
+            margin = max(float(aw.max()) / wunit, float(ab.max()) / bunit / 2) / 2 ** 24    # weights < 2^22, biases < 2^23 units
+            refs[i] = (gw.float(), gb.float(), margin)
+    for accumulate in (False, True):
+        batch = tc.WgradBatch.get(cuda)
+        batch.reset()
+        got = []
+        for i, L in reversed(list(enumerate(layers))):
+            if i not in only:
+                continue
+            if L is flow and L.dgrad == "fold":
+                gwf = torch.empty((9, L.cin, 1, 3, 3), device=cuda)
+                gbf = torch.empty(9, device=cuda)
+                batch.add_khm(X[L.a], tc.planar_fold_kd(gplanes, 16), gwf, gbf, L.cin, 9)
+                got.append((i, "wgrad kd-folded (kh in M)", lambda gwf=gwf, gbf=gbf, L=L: eng.unfold_grad_flow(gwf, gbf, 3, L.cin), None))
+            elif L is first and L.fwd == "fold":
+                gwf = torch.empty((L.cout, 3 * L.cin, 1, 3, 3), device=cuda)
+                gbf = torch.empty(L.cout, device=cuda)
+                if L.khm:
+                    batch.add_khm(X[0], G[L.out], gwf, gbf, 3 * L.cin, L.cout)
+                else:
+                    batch.add(X[0], None, G[L.out], gwf, gbf, 3 * L.cin, L.cout, 1, False, False)
+                got.append((i, "wgrad kd-folded" + (" (kh in M)" if L.khm else ""),
+                            lambda gwf=gwf, gbf=gbf, L=L: (eng.unfold_grad_first(gwf, L.cout, L.cin), gbf), None))
+            else:
+                g_in = tc.planar_to_ndhwc8(gplanes) if L is flow else G[L.out]
+                xa = X[0] if L is first else X[L.a]
+                prior = None
+                if accumulate:         # the flat-gradient path: integer-valued prior content
+                    prior = (torch.randint(-4, 5, L.w.shape, generator=g, device=cuda).float(),
+                             torch.randint(-4, 5, L.bias.shape, generator=g, device=cuda).float())
+                    gw, gb = tc.conv_wgrad(xa, X.get(L.b), g_in, L.cin, L.cout, 3, up=L.up, out_w=prior[0].clone(),
+                                           out_b=prior[1].clone(), batch=batch)
+                else:
+                    gw, gb = tc.conv_wgrad(xa, X.get(L.b), g_in, L.cin, L.cout, 3, up=L.up, batch=batch)
+                got.append((i, "wgrad" + (" accumulated" if accumulate else ""), lambda gw=gw, gb=gb: (gw, gb), prior))
+        batch.flush()
+        for i, form, res, prior in got:
+            gw, gb = res()
+            rw, rb, margin = refs[i]
+            if prior is not None:
+                rw, rb = prior[0] + rw, prior[1] + rb
+            rows.append((lname(i, layers[i]), form, mism(gw, rw) + mism(gb, rb), margin))
+    _report("exact %s %s" % (name, forms), rows)
+
+
+# ---- b. the glue kernels of the full-size backward ------------------------------------------------------------------
+
+def _children(x):
+    B, D, H, W, C = x.shape
+    return x.reshape(B, D // 2, 2, H // 2, 2, W // 2, 2, C).permute(0, 1, 3, 5, 2, 4, 6, 7).reshape(B, D // 2, H // 2, W // 2, 8, C)
+
+
+def _unchildren(c):
+    B, Dc, Hc, Wc, _, C = c.shape
+    return c.reshape(B, Dc, Hc, Wc, 2, 2, 2, C).permute(0, 1, 4, 2, 5, 3, 6, 7).reshape(B, 2 * Dc, 2 * Hc, 2 * Wc, C)
+
+
+@pytest.mark.parametrize("with_skip", [True, False])
+def test_glue_kernels_exact_at_full_size(vx, cuda, with_skip):
+    """pool, unpool_combine (gradient to the FIRST maximal child, ties frequent with ternary activations) and sumpool_mask
+    at the full-resolution shapes of the default model, against fp64 / fp32 emulations."""
+    _, eng, _ = vx
+    g = torch.Generator(device=cuda).manual_seed(9)
+    s32 = torch.tensor(SLOPE, dtype=torch.float32, device=cuda)
+    x = ternary((1, 160, 192, 224, 16), g)
+    y = eng._pool(x, 3)
+    ch = _children(x).double()
+    mx = ch.max(4, keepdim=True).values
+    assert mism(y, mx.squeeze(4)) == 0
+    is_max = ch == mx
+    first = is_max & (is_max.cumsum(4) == 1)
+    assert bool((first.sum(4) == 1).all()) and bool((is_max.sum(4) > 1).any())
+    gs = ternary(x.shape, g) if with_skip else None
+    gp = ternary(y.shape, g)
+    out = eng._unpool_combine(x, gs, gp, 3, SLOPE)
+    r = first.float() * gp.float().unsqueeze(4) + (_children(gs).float() if with_skip else 0)
+    r = torch.where(ch < 0, r * s32, r)
+    n_unpool = mism(out, _unchildren(r).to(torch.bfloat16))
+    gf = ternary((1, 160, 192, 224, 32), g)
+    act = ternary((1, 80, 96, 112, 32), g)
+    sp = eng._sumpool_mask(gf, act, 3, SLOPE)
+    s = ref.children_sum(gf.double()).float()
+    n_sum = mism(sp, torch.where(act < 0, s * s32, s).to(torch.bfloat16))
+    print("\n[glue, full size] pool 0 | unpool_combine%s %d | sumpool_mask %d mismatches" % ("" if with_skip else " (no skip)", n_unpool, n_sum))
+    assert n_unpool == 0 and n_sum == 0
+
+
+# ---- c. the decomposition sweep: VXM_B200_CONV_CTAS caps the persistent grid ------------------------------------------
+
+def _ops(kind, quantised, cuda):
+    """operands of one sweep launch: ragged shapes (partial w tiles, H not a multiple of the tile height, odd depth, B = 2)"""
+    g = torch.Generator(device=cuda).manual_seed(100 + len(kind) + quantised)
+    act = (lambda s: ternary(s, g)) if quantised else (lambda s: torch.randn(s, generator=g, device=cuda).to(torch.bfloat16))
+    wt = (lambda s: qweight(s, g)) if quantised else (lambda s: torch.randn(s, generator=g, device=cuda) * 0.05)
+    plane = (lambda s: ternary(s, g, torch.float32) * PLANE) if quantised else (lambda s: torch.randn(s, generator=g, device=cuda))
+    if kind == "plain":
+        return dict(x=act((2, 11, 21, 67, 16)), w=wt((32, 16, 3, 3, 3)), b=wt((32,)))
+    if kind == "masked_dgrad":
+        return dict(gz=act((2, 11, 21, 67, 32)), w=wt((32, 16, 3, 3, 3)), act=act((2, 11, 21, 67, 16)))
+    if kind == "concat_up":
+        return dict(xa=act((2, 5, 11, 33, 32)), xb=act((2, 10, 22, 66, 32)), w=wt((32, 64, 3, 3, 3)), b=wt((32,)))
+    if kind == "polyphase":
+        return dict(xa=act((2, 7, 11, 33, 32)), xb=act((2, 14, 22, 66, 16)), w=wt((32, 48, 3, 3, 3)), b=wt((32,)),
+                    gz=act((2, 14, 22, 66, 32)), act=act((2, 7, 11, 33, 32)))
+    if kind == "blocked64":
+        return dict(x=act((2, 7, 13, 37, 64)), w=wt((64, 64, 3, 3, 3)), b=wt((64,)))
+    assert kind == "wgrad"
+    return dict(xa=act((2, 7, 11, 33, 32)), xb=act((2, 14, 22, 66, 16)), gz=act((2, 14, 22, 66, 32)),      # rem0: 32^ + 16 -> 32
+                x64=act((1, 9, 14, 40, 64)), g64=act((1, 9, 14, 40, 64)),                                # 64 x 64 slices
+                planes=[plane((2, 1, 11, 21, 67)) for _ in range(2)], g16=act((2, 11, 21, 67, 16)))       # kd-folded, kh in M
+
+
+def _launch(vx, kind, o):
+    _, eng, tc = vx
+    if kind == "plain":
+        wpk, cp = tc.pack_weights_t(o["w"], variant="s")
+        return (tc.conv_fwd_t(o["x"], None, wpk, cp, o["b"], 32, 3, slope=SLOPE),)
+    if kind == "masked_dgrad":
+        wpk, cp = tc.pack_weights_t(o["w"], transposed=True, variant="s")
+        return (tc.conv_fwd_t(o["gz"], None, wpk, cp, None, 16, 3, slope=SLOPE, mask=o["act"]),)
+    if kind == "concat_up":
+        assert tc.conv_blocks(32, 32, 32, 3) is None
+        wpk, cp = tc.pack_weights_t(o["w"], variant="s")
+        return (tc.conv_fwd_t(o["xa"], o["xb"], wpk, cp, o["b"], 32, 3, up=True, slope=SLOPE),)
+    if kind == "polyphase":
+        fwd = tc.conv_fwd_poly(o["xa"], o["xb"], tc.pack_weights_poly(o["w"], 1, 32), o["b"], 32, SLOPE)
+        return fwd, tc.dgrad_poly(o["gz"], tc.pack_weights_poly(o["w"], 2, 32), o["act"], SLOPE)
+    if kind == "blocked64":
+        blocks = tc.conv_blocks(64, 0, 64, 3)
+        assert blocks is not None
+        return (tc.conv_fwd_blocked(o["x"], None, blocks, tc.pack_weights_blocks(o["w"], False, blocks), o["b"], 64, 3, slope=SLOPE),)
+    batch = tc.WgradBatch.get(o["gz"].device)
+    batch.reset()
+    w1, b1 = tc.conv_wgrad(o["xa"], o["xb"], o["gz"], 48, 32, 3, up=True, batch=batch)
+    w2, b2 = tc.conv_wgrad(o["x64"], None, o["g64"], 64, 64, 3, batch=batch)
+    gwf = torch.empty((16, 6, 1, 3, 3), device=o["gz"].device)
+    gbf = torch.empty(16, device=o["gz"].device)
+    batch.add_khm(tc.planar_fold_kd(o["planes"], 8), o["g16"], gwf, gbf, 6, 16)
+    batch.flush()
+    return w1, b1, w2, b2, gwf, gbf
+
+
+def _reference(vx, kind, o):
+    _, eng, _ = vx
+    if kind == "plain":
+        return (torch.cat(ref.conv([(o["x"], False)], o["w"], 11, finish=lambda y, *_: ref.epilogue(y, o["b"], SLOPE)), 1),)
+    if kind == "masked_dgrad":
+        return (torch.cat(ref.conv([(o["gz"], False)], ref.dgrad_weight(o["w"]), 11,
+                                   finish=lambda y, d0, d1: ref.epilogue(y, slope=SLOPE, mask=o["act"][:, d0:d1])), 1),)
+    if kind == "concat_up":
+        return (ref.epilogue(ref.conv([(o["xa"], True), (o["xb"], False)], o["w"], 10), o["b"], SLOPE),)
+    if kind == "polyphase":
+        fwd = ref.epilogue(ref.conv([(o["xa"], True), (o["xb"], False)], o["w"], 14), o["b"], SLOPE)
+        y = ref.conv([(o["gz"], False)], ref.dgrad_weight(o["w"]), 14)[..., :32]
+        return fwd, ref.epilogue(ref.children_sum(y), slope=SLOPE, mask=o["act"])
+    if kind == "blocked64":
+        return (ref.epilogue(ref.conv([(o["x"], False)], o["w"], 7), o["b"], SLOPE),)
+    out = []
+    for srcs, gz, kd in (([(o["xa"], True), (o["xb"], False)], o["gz"], 3), ([(o["x64"], False)], o["g64"], 3),
+                         ([(eng.fold_planes(o["planes"]), False)], o["g16"], 1)):
+        gw, gb = ref.wgrad(srcs, gz, kd)
+        aw, ab = ref.wgrad(srcs, gz, kd, absolute=True)
+        assert float(aw.max()) < 2 ** 22 * (PLANE if kd == 1 else 1) and float(ab.max()) < 2 ** 23
+        out += [gw.float(), gb.float()]
+    return tuple(out)
+
+
+@pytest.mark.parametrize("kind", ["plain", "masked_dgrad", "concat_up", "polyphase", "blocked64", "wgrad"])
+def test_decomposition_sweep(vx, cuda, monkeypatch, kind):
+    """Each launch kind with its persistent grid capped at 1, 2, 5 and 13 CTAs (many items per CTA, partial last waves,
+    other depth chunkings) and uncapped.  Quantised operands: every cap equals fp64 exactly.  Ordinary operands: the
+    forward and dgrad outputs are bit-identical across caps (one CTA writes each output tile, in a fixed MMA order); the
+    weight gradient is bit-identical between two runs at the same cap, and the cap does change its per-CTA partition."""
+    def run(o, cap):
+        if cap is None:
+            monkeypatch.delenv("VXM_B200_CONV_CTAS", raising=False)
+        else:
+            monkeypatch.setenv("VXM_B200_CONV_CTAS", cap)
+        res = [t.clone() for t in _launch(vx, kind, o)]
+        torch.cuda.synchronize()
+        return res
+
+    o = _ops(kind, True, cuda)
+    refs = _reference(vx, kind, o)
+    counts = {cap: [mism(a, r) for a, r in zip(run(o, cap), refs)] for cap in CAPS}
+    print("\n[sweep %s, quantised] mismatches per output by VXM_B200_CONV_CTAS: %s" % (kind, counts))
+    assert all(n == 0 for c in counts.values() for n in c), counts
+    o = _ops(kind, False, cuda)
+    outs = {cap: run(o, cap) for cap in CAPS}
+    if kind == "wgrad":
+        for cap in CAPS:
+            assert all(torch.equal(a, b) for a, b in zip(outs[cap], run(o, cap))), cap
+        assert not all(torch.equal(a, b) for a, b in zip(outs["1"], outs[None]))
+    else:
+        for cap in CAPS:
+            assert all(torch.equal(a, b) for a, b in zip(outs[cap], outs[None])), cap

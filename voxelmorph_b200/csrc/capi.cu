@@ -1,5 +1,6 @@
 // Error text, version string, launch counter and small device queries of the C ABI.
 #include <stdarg.h>
+#include <stdlib.h>
 
 #include <atomic>
 
@@ -40,6 +41,16 @@ int sm_count() {
     cached_dev = dev;
   }
   return cached;
+}
+
+// Persistent CTAs of a tensor-core convolution launch: one per SM, or at most n with VXM_B200_CONV_CTAS=n (n >= 1; read
+// at every launch).  The depth-chunk cost model and the grid both take this count, so a capped launch runs the
+// decomposition of a GPU with n SMs.
+int conv_ctas() {
+  const int n = sm_count();
+  const char* e = getenv("VXM_B200_CONV_CTAS");
+  const int cap = e ? atoi(e) : 0;
+  return cap >= 1 && cap < n ? cap : n;
 }
 
 namespace tc {

@@ -12,6 +12,7 @@ void set_error(const char* fmt, ...);
 void count_launch(int n = 1);
 int check_launch(const char* what);  // cudaGetLastError -> VXM_OK / VXM_ERR_CUDA (+ counts one launch)
 int sm_count();
+int conv_ctas();                     // sm_count(), capped by VXM_B200_CONV_CTAS (tensor-core convolution grids)
 
 #define VXM_REQUIRE(cond, ...)          \
   do {                                  \

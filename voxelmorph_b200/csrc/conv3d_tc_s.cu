@@ -868,7 +868,7 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     if (poly) HTv = poly == 2 ? 8 : 4;               // the polyphase kernels exist at one tile height each
   }
   a.tiles_h = (H + HTv - 1) / HTv; a.tiles_w = (W + WUSE - 1) / WUSE;
-  int nsm = sm_count();
+  int nsm = conv_ctas();
   // depth chunking: balance the persistent CTAs (waves of nsm items) against the 2 halo slabs every chunk re-loads
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
   int best_nch = 1;

@@ -408,7 +408,7 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
     a.dbg = de ? atoi(de) : 0;
   }
   const int G = Cx <= 16 ? 16 : 32, GOUT = Cg <= 16 ? 16 : 32;
-  const int nsm = sm_count();
+  const int nsm = conv_ctas();
   // depth chunking: balance the persistent CTAs (waves of nsm items) against the 2 halo slabs every chunk re-loads
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
   int best_nch = 1;
