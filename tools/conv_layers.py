@@ -113,6 +113,21 @@ def build():
     return L
 
 
+if sys.argv[1:2] == ["--dump"]:
+    # the output of every forward and dgrad launch on seeded operands, one file per launch under DIR, for a bit-for-bit
+    # comparison of two builds: `tools/conv_layers.py --dump DIR` with each, then torch.equal on every pair of files
+    out_dir = sys.argv[2]
+    os.makedirs(out_dir, exist_ok=True)
+    torch.manual_seed(0)
+    for name, fn in build().items():
+        if "wgrad" in name or "fold: planar" in name or "plain:" in name or "sumpool" in name:
+            continue
+        y = fn()
+        ys = y if isinstance(y, tuple) else (y,)
+        fname = "".join(c if c.isalnum() else "_" for c in name) + ".pt"
+        torch.save([t.cpu() for t in ys], os.path.join(out_dir, fname))
+    torch.cuda.synchronize()
+    sys.exit(0)
 if sys.argv[1:2] == ["--once"]:
     # every selected layer once (ncu replays the launch itself): `ncu --set full -k regex:"conv_tcs|wgrad2_kernel" ... tools/conv_layers.py --once`
     for name, fn in build().items():

@@ -98,7 +98,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
   const int NSLOT = a.nslot;
   uint8_t* s_w = smem;
   uint8_t* s_slab = smem + ((a.wbytes + 1023u) & ~1023u);
-  float* s_stage = reinterpret_cast<float*>(s_slab + NSLOT * slab_bytes);   // one accumulator read-out buffer per group
+  // one accumulator read-out (or seam exchange) buffer per group
+  float* s_stage = reinterpret_cast<float*>(s_slab + NSLOT * slab_bytes);
   uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + NGRP * ACC_STAGE_FLOATS);
   uint64_t* full = bars;
   uint64_t* empty = bars + MAXSLOT;
@@ -298,87 +299,192 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
       }
     };
     if constexpr (EPI != 0) {
+      // Drain in the wgmma fragment layout: thread (warp wq, lane = 4 q + p) of the group holds, in m64 accumulator
+      // `blk` = sub + f of a tile half, tile row 2 blk + (wq >> 1) and the columns w' = 16 (wq & 1) + q + 8 i (i = 0, 1),
+      // channels 8 jj + 2 p + {0, 1} of each kw partial sum P0 | P1 | P2.  The kw neighbours w' -/+ 1 are lane -/+ 4
+      // (lane -/+ 28 and the other i at the q = 0 / 7 seam); only the 15 | 16 seam between the two warps of a slab row
+      // crosses warps: warp 2k publishes P0 of w' = 15, warp 2k + 1 P2 of w' = 16 in the group's exchange buffer, one
+      // warp-pair barrier per chain.  The buffer alternates between two halves, so a write never overtakes the other
+      // warp's last read.  The 48 / 64-output chains and the coarse dgrad (PD 2) keep the row read-out (see ROWS).
       const float slope = a.slope;
       const int c1 = (EPI == 3 && a.out2) ? a.csplit : COUT;       // channels [0, c1) -> out, [c1, COUT) -> out2
       const int Ho = PD == 2 ? a.H >> 1 : a.H, Wo = PD == 2 ? a.W >> 1 : a.W;   // output rows, columns
       const size_t HWp = (size_t)Ho * Wo;
+      const int q = lane >> 2, p = lane & 3, half = wq & 1, pair = wq >> 1;
+      const int xbar = 3 + 2 * grp + pair;                      // named barrier of this warp pair
+      // Row read-out instead: the 48 / 64-output chains (in the fragment form their bias / mask loads spill next to the
+      // 72 / 96 accumulator floats) and the coarse dgrad (its 32-channel mask, prefetched before the chain, spills there)
+      constexpr bool ROWS = NSUB > 1 || PD == 2;
+      constexpr int XPAIR = NF * 2 * COUT;                       // floats per warp pair and buffer half: P0 of 15, P2 of 16
+      static_assert(2 * 2 * XPAIR <= ACC_STAGE_FLOATS, "seam exchange fits the stage buffer");
+      uint32_t xpar = 0;
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
         const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
-        const int w = wt * WUSE - 1 + lane, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, Dout);
+        const int d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, Dout);
         const int nd = d1 - d0;
-        // PD 2: the odd lanes (even w) hold the sums of their w' pairs and store coarse column w / 2
-        const bool wok = lane >= 1 && lane <= WUSE && w < a.W && (PD != 2 || (lane & 1));
-        bool ok[NH][NSUB];
-        size_t vx[NH][NSUB];                                     // voxel index of this lane in slice d0
+        // column i of block blk of tile half hb: voxel vbase + (4 hb + 2 blk) Wo + 8 i, written iff bit 4 hb + 2 blk + i of okm
+        const int wp = 16 * half + q, w = wt * WUSE - 1 + wp;
+        const int hbase = ht * HT + pair;
+        uint32_t okm = 0;
 #pragma unroll
-        for (int hb = 0; hb < NH; ++hb) {
+        for (int hb = 0; hb < NH; ++hb)
 #pragma unroll
-          for (int sub = 0; sub < NSUB; ++sub) {
-            const int h = PD == 2 ? ht * (HT / 2) + trow0 : ht * HT + hb * 4 + trow0 + 2 * sub;
-            ok[hb][sub] = wok && h < Ho;
-            vx[hb][sub] = (((size_t)b * Dout + d0) * Ho + h) * Wo + (PD == 2 ? w >> 1 : w);
-          }
-        }
+          for (int blk = 0; blk < 2; ++blk)
+#pragma unroll
+            for (int i = 0; i < 2; ++i)
+              if (wp + 8 * i >= 1 && wp + 8 * i <= WUSE && w + 8 * i < a.W && hbase + 4 * hb + 2 * blk < Ho)
+                okm |= 1u << (4 * hb + 2 * blk + i);
+        size_t vbase = (((size_t)b * Dout + d0) * Ho + hbase) * Wo + (size_t)(long long)w;
         for (int j = 0; j < nd; ++j) {
           const uint32_t js = PD == 2 ? 2u * j : (uint32_t)j;   // ring index of the window's first slab
           observe(cnt_base + js + (PD == 2 ? 3u : (KD == 3 ? 2u : 0u)));
           const uint32_t hslot = (cnt_base + js) % NSLOT;
 #pragma unroll
           for (int hb = 0; hb < NH; ++hb) {
-            const bool mine = (int)(ecnt++ % NGRP) == grp;
-            size_t voxs[NSUB];
+            if ((int)(ecnt++ % NGRP) != grp) continue;
+            auto vox_of = [&](int blk, int i) { return vbase + (size_t)((4 * hb + 2 * blk) * Wo + 8 * i); };
 #pragma unroll
             for (int sub = 0; sub < NSUB; ++sub) {
-              voxs[sub] = vx[hb][sub];
-              vx[hb][sub] += HWp;
-            }
-            if (!mine) continue;
+              // the saved activations (EPI 2) of this thread's columns in accumulator f: loaded before the chain where
+              // they fit beside it (16 outputs), else at the start of f's drain
+              [[maybe_unused]] uint32_t mreg[EPI == 2 && !ROWS ? NF : 1][2][COUT / 8];
+              auto load_mask = [&](int f) {
+                if constexpr (EPI == 2 && !ROWS) {
 #pragma unroll
-            for (int sub = 0; sub < NSUB; ++sub) {
-              const size_t vox = voxs[sub];
-              const bool valid = ok[hb][sub];
-              [[maybe_unused]] uint32_t mreg[EPI == 2 ? NCH : 1][8];
-              if constexpr (EPI == 2) {
+                  for (int i = 0; i < 2; ++i)
+                    if (okm >> (4 * hb + 2 * f + i) & 1u) {
+                      const uint32_t* mp = reinterpret_cast<const uint32_t*>(a.mask + vox_of(f, i) * (OP ? a.opitch : COUT) + 2 * p);
+#pragma unroll
+                      for (int jj = 0; jj < COUT / 8; ++jj) mreg[f][i][jj] = __ldg(mp + 4 * jj);
+                    }
+                }
+              };
+              if constexpr (COUT == 16) {
+#pragma unroll
+                for (int f = 0; f < NF; ++f) load_mask(f);
+              }
+              // ROWS: thread t of the group drains voxel row t of the tile half (48 / 64 outputs: of its m64 sub-tile, two
+              // threads per row, the warp pair wq >> 1 taking every other 16-channel chunk); PD 2: the odd lanes (even w)
+              // hold the sums of their w' pairs and store coarse column w / 2
+              const int rh = PD == 2 ? ht * (HT / 2) + trow0 : ht * HT + hb * 4 + trow0 + 2 * sub, rw = wt * WUSE - 1 + lane;
+              const bool rvalid = lane >= 1 && lane <= WUSE && rw < a.W && rh < Ho && (PD != 2 || (lane & 1));
+              const size_t rvox = (((size_t)b * Dout + d0 + j) * Ho + rh) * Wo + (PD == 2 ? rw >> 1 : rw);
+              [[maybe_unused]] uint32_t mrow[PD == 2 ? NCH : 1][8];
+              if constexpr (PD == 2) {
 #pragma unroll
                 for (int i = 0; i < NCH; ++i)
-                  if (valid && chan(i) < COUT) ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + chan(i), mreg[i]);
+                  if (rvalid) ld_global_nc_v8(a.mask + rvox * COUT + chan(i), mrow[i]);
               }
               float acc[NF][NN / 2];
               mma(hslot, hb, sub, acc, (d0 + j) & 1);
+              if constexpr (ROWS) {
+                const bool valid = rvalid;
+                const size_t vox = rvox;
 #pragma unroll
-              for (int i = 0; i < NCH; ++i) {
-                const int c0 = chan(i);
-                float v[16];
-                combine(acc, i, v);
-                if (NSUB > 1 && c0 >= COUT) continue;            // (48 channels: the second warp pair has one chunk less)
-                if constexpr (PD == 2) {                         // coarse column: the sum of the w' pair (w, w + 1)
+                for (int i = 0; i < NCH; ++i) {
+                  const int c0 = chan(i);
+                  float v[16];
+                  combine(acc, i, v);
+                  if (c0 >= COUT) continue;                      // (48 channels: the second warp pair has one chunk less)
+                  if constexpr (PD == 2) {                       // coarse column: the sum of the w' pair (w, w + 1)
 #pragma unroll
-                  for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, v[c], 1);
-                }
-                if constexpr (EPI == 1) {
-#pragma unroll
-                  for (int c = 0; c < 16; ++c) {
-                    const float x = v[c] + (a.bias ? __ldg(a.bias + c0 + c) : 0.f);
-                    v[c] = fmaxf(x, x * slope);                    // LeakyReLU for 0 <= slope <= 1
+                    for (int c = 0; c < 16; ++c) v[c] += __shfl_down_sync(0xffffffffu, v[c], 1);
                   }
-                } else if constexpr (EPI == 2) {
+                  if constexpr (EPI == 1) {
 #pragma unroll
-                  for (int e = 0; e < 8; ++e) {                    // sign bits of the saved bf16 activations
-                    const uint32_t mw = mreg[i][e];
-                    if (mw & 0x8000u) v[2 * e] *= slope;
-                    if (mw & 0x80000000u) v[2 * e + 1] *= slope;
+                    for (int c = 0; c < 16; ++c) {
+                      const float x = v[c] + (a.bias ? __ldg(a.bias + c0 + c) : 0.f);
+                      v[c] = fmaxf(x, x * slope);
+                    }
+                  } else if constexpr (EPI == 2) {
+                    uint32_t mreg[8];
+                    if constexpr (PD == 2) {
+#pragma unroll
+                      for (int e = 0; e < 8; ++e) mreg[e] = mrow[i][e];
+                    } else if (valid) {
+                      ld_global_nc_v8(a.mask + vox * (OP ? a.opitch : COUT) + c0, mreg);
+                    }
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                      if (mreg[e] & 0x8000u) v[2 * e] *= slope;
+                      if (mreg[e] & 0x80000000u) v[2 * e + 1] *= slope;
+                    }
+                  }
+                  if (valid) {
+                    __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
+                                                                : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + c0;
+                    st_global_v8(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
+                                 pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
                   }
                 }
-                if (valid) {
-                  __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
-                                                              : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + c0;
-                  st_global_v8(dst, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]), pack_bf16x2(v[6], v[7]),
-                               pack_bf16x2(v[8], v[9]), pack_bf16x2(v[10], v[11]), pack_bf16x2(v[12], v[13]), pack_bf16x2(v[14], v[15]));
+                continue;
+              }
+              float* xb = stage + xpar * (2 * XPAIR) + pair * XPAIR;
+              xpar ^= 1u;
+              if (half == 0 ? q == 7 : q == 0) {                 // publish the seam rows (one 8-byte store per channel pair)
+#pragma unroll
+                for (int f = 0; f < NF; ++f)
+#pragma unroll
+                  for (int jj = 0; jj < COUT / 8; ++jj) {
+                    float2* xs = reinterpret_cast<float2*>(xb + f * 2 * COUT + 8 * jj + 2 * p);
+                    const int k0 = 4 * jj + 2, k2 = 4 * (COUT / 4 + jj);       // P0 of row q + 8, P2 of row q
+                    if (half == 0) xs[0] = make_float2(acc[f][k0], acc[f][k0 + 1]);        // P0 of w' = 15
+                    else xs[COUT / 2] = make_float2(acc[f][k2], acc[f][k2 + 1]);           // P2 of w' = 16
+                  }
+              }
+              named_bar(xbar, 64);
+#pragma unroll
+              for (int f = 0; f < NF; ++f) {
+                const int blk = sub + f;
+                if constexpr (COUT != 16) load_mask(f);
+#pragma unroll
+                for (int jj = 0; jj < COUT / 8; ++jj) {
+                  const int c0 = 8 * jj + 2 * p;
+                  float v[2][2];                                 // [i][e]: channel c0 + e of column w' + 8 i
+#pragma unroll
+                  for (int e = 0; e < 2; ++e) {
+                    const float* xs = xb + f * 2 * COUT + c0 + e;
+                    const int k0 = 4 * jj + e, k1 = 4 * (COUT / 8 + jj) + e, k2 = 4 * (COUT / 4 + jj) + e;
+                    // P0[w' - 1], P2[w' + 1] from the lanes 4 below / above (the sender picks the other i at the seam)
+                    const float a1 = __shfl_sync(0xffffffffu, q == 7 ? acc[f][k0] : acc[f][k0 + 2], (lane + 28) & 31);
+                    const float a0 = __shfl_sync(0xffffffffu, acc[f][k0], (lane + 28) & 31);
+                    const float b0 = __shfl_sync(0xffffffffu, q == 0 ? acc[f][k2 + 2] : acc[f][k2], (lane + 4) & 31);
+                    const float b1 = __shfl_sync(0xffffffffu, acc[f][k2 + 2], (lane + 4) & 31);
+                    float x0 = q == 0 ? xs[0] : a0;
+                    x0 += acc[f][k1];
+                    x0 += b0;
+                    float x1 = a1;
+                    x1 += acc[f][k1 + 2];
+                    x1 += q == 7 ? xs[COUT] : b1;
+                    v[0][e] = x0;
+                    v[1][e] = x1;
+                  }
+#pragma unroll
+                  for (int i = 0; i < 2; ++i) {
+                    if constexpr (EPI == 1) {
+#pragma unroll
+                      for (int e = 0; e < 2; ++e) {
+                        const float x = v[i][e] + (a.bias ? __ldg(a.bias + c0 + e) : 0.f);
+                        v[i][e] = fmaxf(x, x * slope);           // LeakyReLU for 0 <= slope <= 1
+                      }
+                    } else if constexpr (EPI == 2) {             // sign bits of the saved bf16 activations
+                      const uint32_t mw = mreg[f][i][jj];
+                      if (mw & 0x8000u) v[i][0] *= slope;
+                      if (mw & 0x80000000u) v[i][1] *= slope;
+                    }
+                    if (okm >> (4 * hb + 2 * blk + i) & 1u) {
+                      const size_t vox = vox_of(blk, i);
+                      __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
+                                                                  : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + c0;
+                      *reinterpret_cast<uint32_t*>(dst) = pack_bf16x2(v[i][0], v[i][1]);
+                    }
+                  }
                 }
               }
             }
           }
+          vbase += HWp;
           if (lane == 0) {                               // this group no longer reads slab js (PD 2: nor js + 1)
             mbar_arrive(&empty[hslot]);
             if (PD == 2) mbar_arrive(&empty[(hslot + 1) % NSLOT]);
