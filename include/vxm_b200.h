@@ -107,6 +107,15 @@ int vxm_ncc_fwd(const float* I, const float* J, float* loss, float* saved, void*
 /* grad_J = grad_loss[0] * d(-mean cc)/dJ.  grad_loss is a device scalar. */
 int vxm_ncc_bwd(const float* I, const float* J, const float* saved, const float* grad_loss,
                 float* grad_J, int B, int D, int H, int W, int wd, int wh, int ww, void* stream);
+/* NCC differentiated w.r.t. either image.  `which`: bit 0 = y_true (I), bit 1 = y_pred (J); 1, 2 or 3.
+ * vxm_ncc_fwd2 stores 3 fields per voxel (which = 1 or 2; which = 2 is vxm_ncc_fwd itself) or 5 (which = 3) in `saved`
+ * (that many * B*D*H*W floats); vxm_ncc_bwd2 takes them with the same `which` and writes grad_I and / or grad_J
+ * (= grad_loss[0] * d(-mean cc)/dI, dJ; the pointer of a gradient that is not asked for is ignored).  which = 3 is
+ * one launch for both gradients. */
+int vxm_ncc_fwd2(const float* I, const float* J, float* loss, float* saved, void* work, int which,
+                 int B, int D, int H, int W, int wd, int wh, int ww, void* stream);
+int vxm_ncc_bwd2(const float* I, const float* J, const float* saved, const float* grad_loss, float* grad_I,
+                 float* grad_J, int which, int B, int D, int H, int W, int wd, int wh, int ww, void* stream);
 
 /* ---- Jacobian determinant of x -> x + disp(x): reference voxelmorph/py/utils.py:473-516 (numpy, np.gradient) ----
  * disp: (B,nd,D,H,W) displacement in voxels (the layout VxmDense(registration=True) returns).  det (B,D,H,W), may be NULL;
@@ -133,6 +142,8 @@ int vxm_mse_bwd(const float* y_true, const float* y_pred, const float* grad_loss
 size_t vxm_dice_workspace_bytes(int BL);
 int vxm_dice_fwd(const float* y_true, const float* y_pred, float* loss, float* sums, void* work,
                  int BL, size_t V, void* stream);
+/* grad_pred = grad_loss[0] * d loss / d y_pred.  The loss is symmetric in its two arguments, so the gradient w.r.t.
+ * y_true is the same call with y_pred in the place of y_true. */
 int vxm_dice_bwd(const float* y_true, const float* sums, const float* grad_loss, float* grad_pred,
                  int BL, size_t V, void* stream);
 

@@ -35,6 +35,8 @@ SIGNATURES = {
     "vxm_ncc_workspace_bytes": (c_sz, [c_i] * 4),
     "vxm_ncc_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 7 + [c_f]),
     "vxm_ncc_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 7 + [c_f]),
+    "vxm_ncc_fwd2": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 8 + [c_f]),
+    "vxm_ncc_bwd2": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 8 + [c_f]),
     "vxm_jacdet": (c_i, [c_f, c_f, c_f] + [c_i] * 5 + [c_f]),
     "vxm_reduce_workspace_bytes": (c_sz, []),
     "vxm_gradloss_fwd": (c_i, [c_f, c_f, c_f] + [c_i] * 7 + [c_fl, c_f]),

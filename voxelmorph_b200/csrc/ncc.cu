@@ -13,8 +13,18 @@
 //   dL/dJ = -(1/N) [ I S(A) + 2 J S(Bq) - S(T) ]
 // The forward stores A, Bq, T (3 fields); the backward box-sums them with the same machinery.
 //
+// By the symmetry of cc in (I, J) the gradient w.r.t. I is the same expression with the roles swapped:
+//   Bp = -cross^2 Jvar/den^2,  Tp = A u_J + 2 Bp u_I
+//   dL/dI = -(1/N) [ J S(A) + 2 I S(Bp) - S(Tp) ]
+// The two-sided entry points (vxm_ncc_fwd2 / vxm_ncc_bwd2) store A, Bq, T, Bp, Tp and box-sum the five fields in one
+// launch (S(A) is shared); with y_true alone they store A, Bp, Tp and run the three-field backward with I and J swapped.
+//
 // Algorithmic bytes (fp32): forward 8 B/voxel (read I, J); backward 12 B/voxel (I, J, dJ)
-// (+ 12 B/voxel written and read again for the three saved fields in training).
+// (+ 12 B/voxel written and read again for the three saved fields in training).  Two-sided: backward 16 B/voxel
+// (I, J, dI, dJ) + 20 B/voxel of saved fields.
+//
+// Kernel MODE: 0 forward (saves A, Bq, T), 1 backward over three fields, 2 forward saving for y_true (`which`),
+// 3 backward over five fields -> dJ and dI.
 #include "common.cuh"
 
 namespace vxm {
@@ -51,12 +61,25 @@ struct NccArgs {
   int B, D, H, W, wd, wh, ww, zchunk;
   float nwin;              // prod(win)
   double scale;            // -1 / (B*D*H*W)
+  float* out2;             // bwd over five fields: grad_I (`out` is grad_J)
+  int which;               // MODE 2: 1 = save A, Bp, Tp (y_true alone), 3 = save A, Bq, T, Bp, Tp
 };
+
+constexpr bool ncc_is_fwd(int mode) { return mode == 0 || mode == 2; }
+constexpr int ncc_fields(int mode) { return mode == 1 ? 3 : 5; }     // box-summed fields of a kernel mode
+
+// The saved fields of one voxel (MODE 2; MODE 0 stores A, Bq, T in place).
+__device__ __forceinline__ void ncc_save2(float* so, size_t DHW, int which, float A, float Bq, float T, float Bp, float Tp) {
+  so[0] = A;
+  if (which == 3) { so[DHW] = Bq; so[2 * DHW] = T; so[3 * DHW] = Bp; so[4 * DHW] = Tp; }
+  else { so[DHW] = Bp; so[2 * DHW] = Tp; }
+}
 
 template <int MODE, int WD>
 __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs per SM: the per-slice barriers of one overlap the loads of the other
-  constexpr int NF = MODE == 0 ? 2 : 3;
-  constexpr int NS = MODE == 0 ? 5 : 3;
+  constexpr bool FWD = ncc_is_fwd(MODE);
+  constexpr int NS = ncc_fields(MODE);
+  constexpr int NF = FWD ? 2 : NS;
   __shared__ __align__(16) float s_in[NF][NIH][NIW];
   __shared__ __align__(16) float s_w[NS][NIH + 2][NTW];
   __shared__ double s_red[32];
@@ -69,9 +92,8 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
   const int z0 = chunk * a.zchunk, z1 = min(z0 + a.zchunk, a.D);
   const int pd = WD / 2, ph = a.wh / 2, pw = a.ww / 2;
   const size_t HW = (size_t)a.H * a.W, DHW = HW * a.D;
-  const float* f0 = (MODE == 0 ? a.I : a.saved_in) + (size_t)b * (MODE == 0 ? 1 : 3) * DHW;
-  const float* f1 = MODE == 0 ? a.J + (size_t)b * DHW : f0 + DHW;
-  const float* f2 = MODE == 0 ? nullptr : f0 + 2 * DHW;
+  const float* f0 = (FWD ? a.I : a.saved_in) + (size_t)b * (FWD ? 1 : NS) * DHW;
+  const float* f1 = FWD ? a.J + (size_t)b * DHW : f0 + DHW;      // backward: field f at f0 + f * DHW
 
   float ring[2][WD][NS];
 #pragma unroll
@@ -99,24 +121,21 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
             size_t off = (size_t)zi * HW + (size_t)h * a.W + w;
             s_in[0][r][c] = ok ? __ldg(f0 + off) : 0.f;
             s_in[1][r][c] = ok ? __ldg(f1 + off) : 0.f;
-            if (NF == 3) s_in[2][r][c] = ok ? __ldg(f2 + off) : 0.f;
+#pragma unroll
+            for (int f = 2; f < NF; ++f) s_in[f][r][c] = ok ? __ldg(f0 + f * DHW + off) : 0.f;
           }
           __syncthreads();
           // ---- W pass: each thread forms 4 adjacent window sums of one row from 12 staged values (register blocked) ----
           if (tid < rows_in * (NTW / 4)) {
             const int r = tid >> 3, c4 = (tid & 7) * 4;
-            float x0[12], x1[12], x2[12];
+            float x[NF][12];
 #pragma unroll
-            for (int q = 0; q < 3; ++q) {
-              const float4 a4 = *reinterpret_cast<const float4*>(&s_in[0][r][c4 + 4 * q]);
-              const float4 b4 = *reinterpret_cast<const float4*>(&s_in[1][r][c4 + 4 * q]);
-              x0[4 * q] = a4.x; x0[4 * q + 1] = a4.y; x0[4 * q + 2] = a4.z; x0[4 * q + 3] = a4.w;
-              x1[4 * q] = b4.x; x1[4 * q + 1] = b4.y; x1[4 * q + 2] = b4.z; x1[4 * q + 3] = b4.w;
-              if (MODE == 1) {
-                const float4 c4v = *reinterpret_cast<const float4*>(&s_in[NF - 1][r][c4 + 4 * q]);
-                x2[4 * q] = c4v.x; x2[4 * q + 1] = c4v.y; x2[4 * q + 2] = c4v.z; x2[4 * q + 3] = c4v.w;
+            for (int f = 0; f < NF; ++f)
+#pragma unroll
+              for (int q = 0; q < 3; ++q) {
+                const float4 a4 = *reinterpret_cast<const float4*>(&s_in[f][r][c4 + 4 * q]);
+                x[f][4 * q] = a4.x; x[f][4 * q + 1] = a4.y; x[f][4 * q + 2] = a4.z; x[f][4 * q + 3] = a4.w;
               }
-            }
             float acc[NS][4];
 #pragma unroll
             for (int s = 0; s < NS; ++s)
@@ -127,11 +146,12 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
               if (k < a.ww) {
 #pragma unroll
                 for (int o = 0; o < 4; ++o) {
-                  const float u = x0[o + k], v = x1[o + k];
-                  if (MODE == 0) {
+                  if (FWD) {
+                    const float u = x[0][o + k], v = x[1][o + k];
                     acc[0][o] += u; acc[1][o] += v; acc[2][o] += u * u; acc[3][o] += v * v; acc[4][o] += u * v;
                   } else {
-                    acc[0][o] += u; acc[1][o] += v; acc[2][o] += x2[o + k];
+#pragma unroll
+                    for (int s = 0; s < NS; ++s) acc[s][o] += x[s][o + k];
                   }
                 }
               }
@@ -177,7 +197,7 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
                 S[s] = acc;
               }
               size_t off = (size_t)zo * HW + (size_t)h * a.W + w;
-              if (MODE == 0) {
+              if (FWD) {
                 // losses.py:57-65, evaluated left to right with one rounding per op
                 float Is = S[0], Js = S[1], I2s = S[2], J2s = S[3], IJs = S[4];
                 float uI = __fdiv_rn(Is, a.nwin), uJ = __fdiv_rn(Js, a.nwin);
@@ -194,13 +214,20 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
                   float A = 2.f * cross / den;
                   float Bq = -(cross * cross) * Ivar / (den * den);
                   float T = A * uI + 2.f * Bq * uJ;
-                  float* so = a.saved_out + (size_t)b * 3 * DHW + off;
-                  so[0] = A; so[DHW] = Bq; so[2 * DHW] = T;
+                  if (MODE == 0) {
+                    float* so = a.saved_out + (size_t)b * 3 * DHW + off;
+                    so[0] = A; so[DHW] = Bq; so[2 * DHW] = T;
+                  } else {
+                    float Bp = -(cross * cross) * Jvar / (den * den);
+                    float Tp = A * uJ + 2.f * Bp * uI;
+                    ncc_save2(a.saved_out + (size_t)b * (a.which == 3 ? 5 : 3) * DHW + off, DHW, a.which, A, Bq, T, Bp, Tp);
+                  }
                 }
               } else {
                 float Iv = __ldg(a.I + (size_t)b * DHW + off), Jv = __ldg(a.J + (size_t)b * DHW + off);
                 float gl = __ldg(a.grad_loss) * (float)a.scale;
                 a.out[(size_t)b * DHW + off] = gl * (Iv * S[0] + 2.f * Jv * S[1] - S[2]);
+                if (MODE == 3) a.out2[(size_t)b * DHW + off] = gl * (Jv * S[0] + 2.f * Iv * S[3] - S[4]);
               }
             }
           }
@@ -209,7 +236,7 @@ __global__ void __launch_bounds__(256, 2) ncc_kernel(NccArgs a) {   // 2 CTAs pe
       }
     }
   }
-  if (MODE == 0) {
+  if (FWD) {
     double tot = block_sum<double>(local, s_red);
     int nblocks = gridDim.x * gridDim.y * gridDim.z;
     int bid = blockIdx.x + gridDim.x * (blockIdx.y + gridDim.y * blockIdx.z);
@@ -248,11 +275,12 @@ struct Args9 {
 };
 
 template <int MODE>
-constexpr size_t smem_bytes() { return (size_t)(MODE == 0 ? 5 : 3) * HR * (PD + PW) * sizeof(float); }
+constexpr size_t smem_bytes() { return (size_t)ncc_fields(MODE) * HR * (PD + PW) * sizeof(float); }
 
 template <int MODE, int WD>
 __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
-  constexpr int NS = MODE == 0 ? 5 : 3;
+  constexpr bool FWD = ncc_is_fwd(MODE);
+  constexpr int NS = ncc_fields(MODE);
   constexpr int PDZ = WD / 2;
   const NccArgs& a = q.a;
   extern __shared__ __align__(16) float sm9[];
@@ -269,9 +297,9 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
     const int ch = (item / (q.tiles_w * q.tiles_h)) % q.nchunks, b = item / (q.tiles_w * q.tiles_h * q.nchunks);
     const int z0 = ch * a.zchunk, z1 = min(z0 + a.zchunk, a.D);
     const int h0 = ht * TH - 4, w0 = wt * TW - 4;
-    const float* f0 = (MODE == 0 ? a.I : a.saved_in) + (size_t)b * (MODE == 0 ? 1 : 3) * DHW;
-    const float* f1 = MODE == 0 ? a.J + (size_t)b * DHW : f0 + DHW;
-    const float* f2 = MODE == 0 ? nullptr : f0 + 2 * DHW;
+    const float* f0 = (FWD ? a.I : a.saved_in) + (size_t)b * (FWD ? 1 : NS) * DHW;
+    const float* f1 = FWD ? a.J + (size_t)b * DHW : f0 + DHW;    // backward: field f at f0 + f * DHW
+    const float* f2 = FWD ? nullptr : f0 + 2 * DHW;
     int goff[KC], soff[KC];
 #pragma unroll
     for (int k = 0; k < KC; ++k) {
@@ -280,14 +308,14 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
       goff[k] = (h >= 0 && h < a.H && w >= 0 && w < a.W) ? h * a.W + w : -1;
       soff[k] = r * PD + c;
     }
-    if (MODE == 1) {
+    if (!FWD) {
       for (int i = tid; i < NS * HR * PD; i += NT) s_d[i] = 0.f;
       __syncthreads();
     }
     // forward: one iteration per output slice; backward: the window's leading halo slices first (running sum)
-    for (int zi = MODE == 0 ? z0 + PDZ : z0 - PDZ; zi < z1 + PDZ; ++zi) {
+    for (int zi = FWD ? z0 + PDZ : z0 - PDZ; zi < z1 + PDZ; ++zi) {
       const int zo = zi - PDZ;
-      if (MODE == 0) {
+      if (FWD) {
         // ---------------- D pass (forward): every halo'd column summed directly over the WD slices of the window ----
         // (zero padded).  A running sum (S += new - old) keeps the rounding of the larger values it slid past: where a
         // window then holds only zeros or faint values (the background and rims of skull-stripped images) that residue
@@ -317,8 +345,9 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
         }
       } else {
         // ---------------- D pass (backward): slide the window of every halo'd column by one slice ----------------
-        // S += P(zi) - P(zi - WD) over the saved A, Bq, T.  No division follows, so the residue of this running sum stays
+        // S += P(zi) - P(zi - WD) over the saved fields.  No division follows, so the residue of this running sum stays
         // at the rounding level of the values it slid past (the test suite checks d/dJ on skull-stripped images).
+        // The two-sided backward slides Bp, Tp in a second pass, so that no more than 30 values are in flight per thread.
         const int zold = zi - WD;
         const bool has_new = zi >= 0 && zi < a.D;
         const bool has_old = WD > 1 && zold >= z0 - PDZ && zold >= 0;   // it was added earlier in this chunk
@@ -345,6 +374,35 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
 #pragma unroll
             for (int f = 0; f < 3; ++f) {
               if (WD > 1) d[f * HR * PD] += dl[f]; else d[f * HR * PD] = dl[f];
+            }
+          }
+        }
+        if (MODE == 3) {
+          const float* f3 = f0 + 3 * DHW;
+          const float* f4 = f0 + 4 * DHW;
+#pragma unroll
+          for (int k = 0; k < KC; ++k) {
+            un[k] = vn[k] = uo[k] = vo[k] = 0.f;
+            if (goff[k] >= 0) {
+              if (has_new) {
+                const size_t o = (size_t)zi * HW + goff[k];
+                un[k] = __ldg(f3 + o); vn[k] = __ldg(f4 + o);
+              }
+              if (has_old) {
+                const size_t o = (size_t)zold * HW + goff[k];
+                uo[k] = __ldg(f3 + o); vo[k] = __ldg(f4 + o);
+              }
+            }
+          }
+#pragma unroll
+          for (int k = 0; k < KC; ++k) {
+            if (goff[k] >= 0) {
+              float* d = s_d + 3 * HR * PD + soff[k];
+              const float dl[2] = {un[k] - uo[k], vn[k] - vo[k]};
+#pragma unroll
+              for (int f = 0; f < 2; ++f) {
+                if (WD > 1) d[f * HR * PD] += dl[f]; else d[f * HR * PD] = dl[f];
+              }
             }
           }
         }
@@ -395,13 +453,13 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
           const int w = wt * TW + wl;
           if (w < a.W) {
             float gl = 0.f;
-            if (MODE == 1) gl = __ldg(a.grad_loss) * (float)a.scale;
+            if (!FWD) gl = __ldg(a.grad_loss) * (float)a.scale;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
               const int h = ht * TH + hq * 4 + j;
               if (h < a.H) {
                 const size_t off = (size_t)zo * HW + (size_t)h * a.W + w;
-                if (MODE == 0) {
+                if (FWD) {
                   // losses.py:57-65
                   const float Is = S[0][j], Js = S[1][j], I2s = S[2][j], J2s = S[3][j], IJs = S[4][j];
                   const float uI = Is * inv_n, uJ = Js * inv_n;
@@ -416,12 +474,19 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
                     const float A = 2.f * cross * rden;
                     const float Bq = -cc * Ivar * rden;
                     const float T = A * uI + 2.f * Bq * uJ;
-                    float* so = a.saved_out + (size_t)b * 3 * DHW + off;
-                    so[0] = A; so[DHW] = Bq; so[2 * DHW] = T;
+                    if (MODE == 0) {
+                      float* so = a.saved_out + (size_t)b * 3 * DHW + off;
+                      so[0] = A; so[DHW] = Bq; so[2 * DHW] = T;
+                    } else {
+                      const float Bp = -cc * Jvar * rden;
+                      const float Tp = A * uJ + 2.f * Bp * uI;
+                      ncc_save2(a.saved_out + (size_t)b * (a.which == 3 ? 5 : 3) * DHW + off, DHW, a.which, A, Bq, T, Bp, Tp);
+                    }
                   }
                 } else {
                   const float Iv = __ldg(a.I + (size_t)b * DHW + off), Jv = __ldg(a.J + (size_t)b * DHW + off);
                   a.out[(size_t)b * DHW + off] = gl * (Iv * S[0][j] + 2.f * Jv * S[1][j] - S[2][j]);
+                  if (MODE == 3) a.out2[(size_t)b * DHW + off] = gl * (Jv * S[0][j] + 2.f * Iv * S[3][j] - S[4][j]);
                 }
               }
             }
@@ -431,7 +496,7 @@ __global__ void __launch_bounds__(NT, 2) ncc9_kernel(const Args9 q) {
     }
     __syncthreads();   // every thread is done with s_w / s_d before the next item writes them
   }
-  if (MODE == 0) {
+  if (FWD) {
     double tot = block_sum<double>(local, s_red);
     finish_reduce(tot, a.rw, gridDim.x, blockIdx.x, a.scale, a.out, s_red);
   }
@@ -476,7 +541,7 @@ static int launch(NccArgs a, cudaStream_t st) {
     VXM_CUDA(cudaFuncSetAttribute(ncc9_kernel<MODE, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     ncc9_kernel<MODE, 1><<<grid, NT, smem, st>>>(q);
   }
-  return check_launch(MODE == 0 ? "ncc_fwd" : "ncc_bwd");
+  return check_launch(ncc_is_fwd(MODE) ? "ncc_fwd" : "ncc_bwd");
 }
 static bool applies(int wd, int wh, int ww) {
   const char* e = getenv("VXM_B200_NCC_KERNEL");
@@ -495,7 +560,7 @@ static int ncc_launch(const NccArgs& a, dim3 grid, cudaStream_t st) {
     case 9: ncc_kernel<MODE, 9><<<grid, 256, 0, st>>>(a); break;
     default: set_error("ncc: unsupported window depth %d", a.wd); return VXM_ERR_UNSUPPORTED;
   }
-  return check_launch(MODE == 0 ? "ncc_fwd" : "ncc_bwd");
+  return check_launch(ncc_is_fwd(MODE) ? "ncc_fwd" : "ncc_bwd");
 }
 
 static int ncc_check(int B, int D, int H, int W, int wd, int wh, int ww, dim3* grid, int* zchunk) {
@@ -575,4 +640,52 @@ extern "C" int vxm_ncc_bwd(const float* I, const float* J, const float* saved, c
   if (rc) return rc;
   a.zchunk = zchunk;
   return ncc_launch<1>(a, grid, as_stream(stream));
+}
+
+// Two-sided NCC.  `which`: bit 0 = y_true (I) needs a gradient, bit 1 = y_pred (J).  The forward saves, per voxel,
+// which == 2: A, Bq, T (exactly vxm_ncc_fwd); 1: A, Bp, Tp; 3: A, Bq, T, Bp, Tp — `saved` holds that many fields of B*D*H*W.
+extern "C" int vxm_ncc_fwd2(const float* I, const float* J, float* loss, float* saved, void* work, int which, int B,
+                            int D, int H, int W, int wd, int wh, int ww, void* stream) {
+  VXM_REQUIRE(which >= 1 && which <= 3, "ncc_fwd2: which must be 1 (y_true), 2 (y_pred) or 3 (both), got %d", which);
+  if (which == 2) return vxm_ncc_fwd(I, J, loss, saved, work, B, D, H, W, wd, wh, ww, stream);
+  if (int rcw = ncc_window_check(wd, wh, ww)) return rcw;
+  VXM_REQUIRE(I && J && loss && saved && work, "ncc_fwd2: null pointer");
+  VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "ncc: non-positive dimension");
+  NccArgs a{};
+  a.I = I; a.J = J; a.saved_out = saved; a.out = loss; a.rw = as_reduce_work(work); a.which = which;
+  a.B = B; a.D = D; a.H = H; a.W = W; a.wd = wd; a.wh = wh; a.ww = ww;
+  a.nwin = (float)(wd * wh * ww);
+  a.scale = -1.0 / ((double)B * D * H * W);
+  if (ncc9::applies(wd, wh, ww)) return ncc9::launch<2>(a, as_stream(stream));
+  dim3 grid;
+  int zchunk = 0;
+  int rc = ncc_check(B, D, H, W, wd, wh, ww, &grid, &zchunk);
+  if (rc) return rc;
+  a.zchunk = zchunk;
+  return ncc_launch<2>(a, grid, as_stream(stream));
+}
+
+// grad_I / grad_J = grad_loss[0] * d(-mean cc)/d(I | J) from the fields vxm_ncc_fwd2 saved with the same `which`; the
+// pointer of a gradient that is not asked for is ignored.  which == 3 is one launch over five box sums.
+extern "C" int vxm_ncc_bwd2(const float* I, const float* J, const float* saved, const float* grad_loss, float* grad_I,
+                            float* grad_J, int which, int B, int D, int H, int W, int wd, int wh, int ww, void* stream) {
+  VXM_REQUIRE(which >= 1 && which <= 3, "ncc_bwd2: which must be 1 (y_true), 2 (y_pred) or 3 (both), got %d", which);
+  if (which == 2) return vxm_ncc_bwd(I, J, saved, grad_loss, grad_J, B, D, H, W, wd, wh, ww, stream);
+  // y_true alone: A, Bp, Tp are what the three-field backward expects once I and J trade places
+  if (which == 1) return vxm_ncc_bwd(J, I, saved, grad_loss, grad_I, B, D, H, W, wd, wh, ww, stream);
+  if (int rcw = ncc_window_check(wd, wh, ww)) return rcw;
+  VXM_REQUIRE(I && J && saved && grad_loss && grad_I && grad_J, "ncc_bwd2: null pointer");
+  VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "ncc: non-positive dimension");
+  NccArgs a{};
+  a.I = I; a.J = J; a.saved_in = saved; a.out = grad_J; a.out2 = grad_I; a.grad_loss = grad_loss; a.which = which;
+  a.B = B; a.D = D; a.H = H; a.W = W; a.wd = wd; a.wh = wh; a.ww = ww;
+  a.nwin = (float)(wd * wh * ww);
+  a.scale = -1.0 / ((double)B * D * H * W);
+  if (ncc9::applies(wd, wh, ww)) return ncc9::launch<3>(a, as_stream(stream));
+  dim3 grid;
+  int zchunk = 0;
+  int rc = ncc_check(B, D, H, W, wd, wh, ww, &grid, &zchunk);
+  if (rc) return rc;
+  a.zchunk = zchunk;
+  return ncc_launch<3>(a, grid, as_stream(stream));
 }

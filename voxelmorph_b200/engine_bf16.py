@@ -24,9 +24,11 @@ class _Layer:
     """One convolution of a model's plan: its parameters, its inputs (tensor ids of the walk: 0 = the images, then every
     convolution and pooling output in execution order) and how it runs.  `fwd` / `dgrad`: the execution form of the
     forward and of the dgrad (see _run); `fwd_x3`: the block grid of the split-precision forward; `dgrad_skip`: with a
-    polyphase dgrad, the form of the skip part (the dgrad's own form then yields the upsampled part only)."""
+    polyphase dgrad, the form of the skip part (the dgrad's own form then yields the upsampled part only); `dgrad_img`
+    (first convolution only): the form of the dgrad into the image planes, which runs only when an image asks for its
+    gradient (_Plan.image_dgrad_packs)."""
     __slots__ = ("w", "bias", "slope", "role", "a", "b", "out", "up", "ca", "cb", "cin", "cout", "fwd", "fwd_x3", "dgrad", "khm",
-                 "dgrad_skip", "pk_fwd", "pk_dgrad", "pk_dgrad_skip", "pk_hi", "pk_lo", "w_hi", "w_lo")
+                 "dgrad_skip", "dgrad_img", "pk_fwd", "pk_dgrad", "pk_dgrad_skip", "pk_hi", "pk_lo", "w_hi", "w_lo")
 
 
 def _refuse(what):
@@ -85,8 +87,13 @@ def _walk(model):
         # tile): the forward of the first convolution (bf16), the dgrad of the flow head
         if role == "first" and fold and 3 * L.cin <= 8 and L.cout in (8, 16, 32):
             L.fwd = "fold"
+        L.dgrad_img = None
         if role == "first":
-            L.dgrad = None                # the images need no gradient
+            # no dgrad in the step's own launch sequence: the images of a training step need no gradient.  When one does
+            # (_UnetFlowFn), the masked output gradient (cout channels) is convolved with the transposed weights into
+            # cin <= 8 fp32 planes: the shape of the flow head's forward, and its launch
+            L.dgrad = None
+            L.dgrad_img = _form(L.cout, 0, L.cin, kd, L.cout)
         elif role == "flow" and fold and L.b is None and L.cin in (8, 16) and 3 * L.cout <= 16:
             L.dgrad = "fold"
         else:                             # the flow gradient enters as 8 channels; a concatenation's dgrad splits its output
@@ -166,6 +173,7 @@ class _Plan:
             L.pk_hi, L.pk_lo = next(packs3), next(packs3)
         self.ptrs = self.weight_ptrs()
         self.stamps = [None, None]
+        self.img_table, self.img_stamp = None, None
 
     def weight_ptrs(self):
         return tuple(L.w.data_ptr() for L in self.layers)
@@ -182,6 +190,20 @@ class _Plan:
                 torch.sub(w, L.w_hi, out=L.w_lo)
             self.x3.refresh()
             self.stamps[1] = stamp
+
+    def image_dgrad_packs(self):
+        """The transposed operand of the first convolution (its dgrad into the image planes), refreshed.  It lives in a
+        table of its own, built on first use and repacked by one launch of its own per weight update: the pack launch
+        of a step whose images need no gradient keeps its descriptors and its size.  (Build it in an eager step — the
+        warm-up of a graph capture — since the descriptor upload is a host-to-device copy.)"""
+        first = self.layers[0]
+        if self.img_table is None:
+            self.img_table = tc.PackTable([(first.w.detach(), True, first.dgrad_img)])
+        stamp = (_weights_epoch, first.w._version)
+        if stamp != self.img_stamp:
+            self.img_table.refresh()
+            self.img_stamp = stamp
+        return self.img_table.packs[0]
 
 
 def _plan_of(model, split):
@@ -293,8 +315,9 @@ def forward_tape(model, source, target, split=False):
     return flow, dict(plan=plan, tensors=tensors, split=split)
 
 
-def backward_tape(ctx, g_flow):
-    """Hand-written backward over the plan.  Returns {param: grad}."""
+def backward_tape(ctx, g_flow, image_grad=False):
+    """Hand-written backward over the plan.  Returns {param: grad}; with `image_grad`, the fp32 planar gradient w.r.t. the
+    image planes (B, src_feats + trg_feats, D, H, W) (D = 1 for a 2-D model) under the key "images" as well."""
     plan, tensors = ctx["plan"], ctx["tensors"]
     nd = plan.nd
     kd = 3 if nd == 3 else 1
@@ -347,6 +370,10 @@ def backward_tape(ctx, g_flow):
                 grads[L.bias] = gb
         # ---- dgrad ----
         if L.dgrad is None:
+            if image_grad and L.role == "first":
+                # bf16 operands as in every other dgrad; no bias, activation or mask (the images are the leaves), and the
+                # layer's input is not read, so a kd-folded image tensor on the tape does not matter
+                grads["images"] = _run(L.dgrad_img, plan.image_dgrad_packs(), g_in, None, L.cin, kd, out_fp32_planar=True)
             continue
         t = L.a
         if L.b is None:
@@ -424,6 +451,9 @@ class _UnetFlowFn(torch.autograd.Function):
         ctx.tape = tape
         ctx.params = params
         ctx.model_ref = model
+        # (source, target) that ask for their gradient, and how the image planes split between them
+        ctx.image_grads = tuple(ctx.needs_input_grad[1:3])
+        ctx.src_feats = source.shape[1]
         return flow
 
     @staticmethod
@@ -431,9 +461,18 @@ class _UnetFlowFn(torch.autograd.Function):
         dp = getattr(ctx.model_ref, "_dp", None)
         if dp is not None:
             dp.schedule()      # gradients written straight into .grad views bypass the parameter hooks
-        grads = backward_tape(ctx.tape, g_flow)
+        grads = backward_tape(ctx.tape, g_flow, image_grad=any(ctx.image_grads))
         ctx.tape = None
-        return (None, None, None, None) + tuple(grads.get(p) for p in ctx.params)
+        g_source = g_target = None
+        if any(ctx.image_grads):
+            g_img = grads.pop("images")
+            if g_flow.dim() == 4:         # 2-D: drop the depth axis, as forward_tape does for the flow
+                g_img = g_img.squeeze(2)
+            if ctx.image_grads[0]:
+                g_source = g_img[:, :ctx.src_feats]
+            if ctx.image_grads[1]:
+                g_target = g_img[:, ctx.src_feats:]
+        return (None, g_source, g_target, None) + tuple(grads.get(p) for p in ctx.params)
 
 
 def unet_flow(model, source, target, split=False):

@@ -27,29 +27,37 @@ class _NccFn(torch.autograd.Function):
         wd, wh, ww = (1, win[0], win[1]) if nd == 2 else tuple(win)
         lib = _lib.load()
         loss = _scalar(I.device)
-        need = ctx.needs_input_grad[1]
-        if ctx.needs_input_grad[0]:
-            raise _lib.VxmError("NCC: gradients w.r.t. y_true are not implemented (the training loop "
-                                "only differentiates y_pred, reference scripts/torch/train.py:210)")
-        saved = torch.empty((B, 3, D, H, W), dtype=torch.float32, device=I.device) if need else None
+        # which gradients the backward owes: bit 0 = y_true, bit 1 = y_pred.  y_pred alone (the training loop) runs the
+        # three-field kernels as ever; y_true adds Bp, Tp to the saved fields (5 per voxel for both, 3 for y_true alone)
+        which = (1 if ctx.needs_input_grad[0] else 0) | (2 if ctx.needs_input_grad[1] else 0)
+        saved = torch.empty((B, 5 if which == 3 else 3, D, H, W), dtype=torch.float32, device=I.device) if which else None
         ws = _lib.reduce_workspace(I.device)
-        _lib.check(lib.vxm_ncc_fwd(_lib.ptr(I), _lib.ptr(J), _lib.ptr(loss), _lib.ptr(saved), _lib.ptr(ws),
-                                   B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_fwd")
+        if which in (0, 2):
+            _lib.check(lib.vxm_ncc_fwd(_lib.ptr(I), _lib.ptr(J), _lib.ptr(loss), _lib.ptr(saved), _lib.ptr(ws),
+                                       B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_fwd")
+        else:
+            _lib.check(lib.vxm_ncc_fwd2(_lib.ptr(I), _lib.ptr(J), _lib.ptr(loss), _lib.ptr(saved), _lib.ptr(ws), which,
+                                        B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_fwd2")
         ctx.save_for_backward(I, J)
         ctx.saved_fields = saved
-        ctx.cfg = (B, D, H, W, wd, wh, ww)
+        ctx.cfg = (B, D, H, W, wd, wh, ww, which)
         return loss
 
     @staticmethod
     def backward(ctx, gl):
         I, J = ctx.saved_tensors
-        B, D, H, W, wd, wh, ww = ctx.cfg
+        B, D, H, W, wd, wh, ww, which = ctx.cfg
         gl = gl.contiguous().float()
-        gJ = torch.empty_like(J)
+        gI = torch.empty_like(I) if which & 1 else None
+        gJ = torch.empty_like(J) if which & 2 else None
         lib = _lib.load()
-        _lib.check(lib.vxm_ncc_bwd(_lib.ptr(I), _lib.ptr(J), _lib.ptr(ctx.saved_fields), _lib.ptr(gl), _lib.ptr(gJ),
-                                   B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_bwd")
-        return None, gJ, None
+        if which == 2:
+            _lib.check(lib.vxm_ncc_bwd(_lib.ptr(I), _lib.ptr(J), _lib.ptr(ctx.saved_fields), _lib.ptr(gl), _lib.ptr(gJ),
+                                       B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_bwd")
+        else:
+            _lib.check(lib.vxm_ncc_bwd2(_lib.ptr(I), _lib.ptr(J), _lib.ptr(ctx.saved_fields), _lib.ptr(gl), _lib.ptr(gI), _lib.ptr(gJ),
+                                        which, B, D, H, W, wd, wh, ww, _lib.stream_ptr()), "vxm_ncc_bwd2")
+        return gI, gJ, None
 
 
 class NCC:
@@ -115,22 +123,28 @@ class _DiceFn(torch.autograd.Function):
         work = torch.empty(int(lib.vxm_dice_workspace_bytes(BL)), dtype=torch.uint8, device=a.device)
         _lib.check(lib.vxm_dice_fwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(loss), _lib.ptr(sums), _lib.ptr(work), BL, V,
                                     _lib.stream_ptr()), "vxm_dice_fwd")
-        ctx.save_for_backward(a, sums)
+        # the backward of either argument reads the OTHER tensor (and the two sums)
+        ctx.save_for_backward(a if ctx.needs_input_grad[1] else None, b if ctx.needs_input_grad[0] else None, sums)
         ctx.cfg = (BL, V)
-        if ctx.needs_input_grad[0]:
-            raise _lib.VxmError("Dice: gradients w.r.t. y_true are not implemented")
         return loss
 
     @staticmethod
     def backward(ctx, gl):
-        a, sums = ctx.saved_tensors
+        a, b, sums = ctx.saved_tensors
         BL, V = ctx.cfg
         gl = gl.contiguous().float()
-        gp = torch.empty_like(a)
         lib = _lib.load()
-        _lib.check(lib.vxm_dice_bwd(_lib.ptr(a), _lib.ptr(sums), _lib.ptr(gl), _lib.ptr(gp), BL, V, _lib.stream_ptr()),
-                   "vxm_dice_bwd")
-        return None, gp
+        grads = []
+        # top = 2 sum(ab) and bottom = clamp(sum(a + b)) are symmetric in (a, b): d/dy_pred = k1 y_true - k2 and
+        # d/dy_true = k1 y_pred - k2 with the same k1, k2 (clamp branch included), so one kernel serves both
+        for other in (b, a):
+            g = None
+            if other is not None:
+                g = torch.empty_like(other)
+                _lib.check(lib.vxm_dice_bwd(_lib.ptr(other), _lib.ptr(sums), _lib.ptr(gl), _lib.ptr(g), BL, V, _lib.stream_ptr()),
+                           "vxm_dice_bwd")
+            grads.append(g)
+        return tuple(grads)
 
 
 class Dice:
