@@ -334,6 +334,20 @@ int vxm_adam_step(float* p, const float* g, float* m, float* v, size_t n, int st
 int vxm_adam_step_dev(float* p, const float* g, float* m, float* v, size_t n, int* step_counter, float lr,
                       float beta1, float beta2, float eps, float weight_decay, float grad_scale, void* stream);
 
+/* ---- MeanStream(cap): the capped running mean TemplateCreation keeps of its inverse flow (reference
+ * voxelmorph/tf/networks.py:761-853, neurite's MeanStream) ----
+ * x (B, n) fp32 (n = nd * voxels, 2-D or 3-D alike), mean (n) and count (1) fp32 device state:
+ *   S = sum_b x_b, n' = count + B, alpha = B / min(n', cap), m' = mean (1 - alpha) + (S / B) alpha,
+ *   out (n) = min(1, n' / cap) m'; commit = 1 (training) also writes mean <- m', count <- n' (0: state untouched).
+ * saved (1 float) receives min(1, n' / cap) alpha / B for the backward; work is the reduce workspace
+ * (vxm_reduce_workspace_bytes: only its ticket counter is used).  count is read and written on the device only. */
+int vxm_mean_stream_fwd(const float* x, float* mean, float* count, float* out, float* saved, void* work, int B, size_t n,
+                        float cap, int commit, void* stream);
+/* grad_x_b = saved[0] * sum_b' grad_out_b' for every b (sum in b' order); grad_out's batch stride is n, or 0 for a
+ * gradient that is itself broadcast over the batch */
+int vxm_mean_stream_bwd(const float* grad_out, const float* saved, float* grad_x, int B, size_t n, size_t gout_bstride,
+                        void* stream);
+
 #ifdef __cplusplus
 }
 #endif

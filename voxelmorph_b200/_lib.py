@@ -94,6 +94,8 @@ SIGNATURES = {
     "vxm_upcat_bwd": (c_i, [c_f, c_f, c_f] + [c_i] * 7 + [c_f]),
     "vxm_adam_step": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_i] + [c_fl] * 6 + [c_f]),
     "vxm_adam_step_dev": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_f] + [c_fl] * 6 + [c_f]),
+    "vxm_mean_stream_fwd": (c_i, [c_f] * 6 + [c_i, c_sz, c_fl, c_i, c_f]),
+    "vxm_mean_stream_bwd": (c_i, [c_f, c_f, c_f, c_i, c_sz, c_sz, c_f]),
 }
 
 _lib = None

@@ -25,7 +25,8 @@ from collections import OrderedDict
 
 import numpy as np
 
-__all__ = ["VolumeCache", "load_volfile", "volgen", "scan_to_scan", "scan_to_atlas", "semisupervised", "Prefetcher"]
+__all__ = ["VolumeCache", "load_volfile", "volgen", "scan_to_scan", "scan_to_atlas", "semisupervised", "template_creation",
+           "Prefetcher"]
 
 
 def _cuda_ready():
@@ -285,6 +286,21 @@ def scan_to_atlas(vol_names, atlas, bidir=False, batch_size=1, no_warp=False, se
             outvols = [res[1], scan] if bidir else [res[1]]
         if not no_warp:
             outvols.append(zeros)
+        yield (invols, outvols)
+
+
+def template_creation(vol_names, bidir=False, batch_size=1, zeros_dtype=np.float32, **kwargs):
+    """Unconditional template creation; arguments, yields and random draws as reference generators.py:197-219:
+    ([scan], [scan, zeros, zeros(, zeros)]), zeros of shape (1, *vol, nd) (the mean stream's and the flow's targets,
+    float32 like scan_to_atlas's)."""
+    zeros = None
+    gen = volgen(vol_names, batch_size=batch_size, **kwargs)
+    while True:
+        scan = next(gen)[0]
+        if zeros is None:
+            zeros = _zero_flow(1, scan.shape[1:-1], zeros_dtype)
+        invols = [scan]
+        outvols = [scan, zeros, zeros, zeros] if bidir else [scan, zeros, zeros]
         yield (invols, outvols)
 
 

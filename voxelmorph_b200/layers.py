@@ -222,3 +222,55 @@ class ResizeTransform(nn.Module):
         if self.factor < 1:   # resize first, then rescale (layers.py:86-89)
             return _ResizeFn.apply(x, out_spatial, 1.0, float(self.factor))
         return _ResizeFn.apply(x, out_spatial, float(self.factor), 1.0)  # layers.py:91-94
+
+
+class _MeanStreamFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, mean, count, cap, commit):
+        _lib.require_cuda(x, mean, count, what="MeanStream")
+        x = _lib.contig(x)
+        B, n = x.shape[0], mean.numel()
+        if tuple(x.shape[1:]) != tuple(mean.shape) or not mean.is_contiguous() or count.numel() != 1:
+            raise _lib.VxmError("MeanStream: input %s does not match the state %s" % (tuple(x.shape), tuple(mean.shape)))
+        out = torch.empty_like(mean)
+        saved = torch.empty(1, dtype=torch.float32, device=x.device)
+        _lib.check(_lib.load().vxm_mean_stream_fwd(_lib.ptr(x), _lib.ptr(mean), _lib.ptr(count), _lib.ptr(out), _lib.ptr(saved),
+                                                   _lib.ptr(_lib.reduce_workspace(x.device)), B, n, float(cap), int(commit),
+                                                   _lib.stream_ptr()), "vxm_mean_stream_fwd")
+        ctx.saved = saved
+        ctx.cfg = (B, n)
+        # one copy of the output, broadcast over the batch (stride 0)
+        return out.unsqueeze(0).expand((B,) + tuple(mean.shape))
+
+    @staticmethod
+    def backward(ctx, gout):
+        B, n = ctx.cfg
+        if B > 1 and gout.stride(0) == 0 and gout[0].is_contiguous():
+            bstride = 0
+        else:
+            gout, bstride = _lib.contig(gout), n
+        gx = torch.empty(gout.shape, dtype=torch.float32, device=gout.device)
+        _lib.check(_lib.load().vxm_mean_stream_bwd(_lib.ptr(gout), _lib.ptr(ctx.saved), _lib.ptr(gx), B, n, bstride,
+                                                   _lib.stream_ptr()), "vxm_mean_stream_bwd")
+        return gx, None, None, None, None
+
+
+class MeanStream(nn.Module):
+    """Capped running mean of its input over the batches seen in training (neurite's MeanStream, which the reference's
+    TemplateCreation wraps around the inverse flow, voxelmorph/tf/networks.py:761-853).
+
+    State: buffers `mean` (`shape`, the input's shape without the batch axis) and `count` (1,), zero at first.  For x
+    (B, *shape): n' = count + B, alpha = B / min(n', cap), m' = mean (1 - alpha) + mean_b(x) alpha, and the output is
+    min(1, n' / cap) m' for every batch entry (one tensor expanded over B).  In training mode the call commits
+    mean <- m' and count <- n' on the device; in eval mode the output is still computed from the batch, nothing is
+    committed (Keras skips `add_update` outside training).  The gradient reaches x only: d out / d x_b =
+    min(1, n' / cap) alpha / B."""
+
+    def __init__(self, shape, cap=100):
+        super().__init__()
+        self.cap = float(cap)
+        self.register_buffer("mean", torch.zeros(tuple(int(s) for s in shape), dtype=torch.float32))
+        self.register_buffer("count", torch.zeros(1, dtype=torch.float32))
+
+    def forward(self, x):
+        return _MeanStreamFn.apply(x, self.mean, self.count, self.cap, self.training)

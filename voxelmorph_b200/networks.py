@@ -9,7 +9,7 @@ import torch
 import torch.nn as nn
 from torch.distributions.normal import Normal
 
-from . import layers, ops
+from . import _lib, layers, ops
 from .modelio import LoadableModel, store_config_args
 
 
@@ -310,3 +310,64 @@ class VxmDenseSemiSupervisedSeg(LoadableModel):
         mode = 'bilinear' if interp_method == 'linear' else interp_method
         flow = self.register(source, target)
         return layers.SpatialTransformer(tuple(img.shape[2:]), mode=mode)(img, flow)
+
+
+class TemplateCreation(LoadableModel):
+    """VoxelMorph network to learn an unconditional template (atlas) image.
+
+    The torch backend of the reference has no such class; the semantics are those of its TensorFlow model
+    (voxelmorph/tf/networks.py:761-853): the atlas is a learnable image, registered to every input by a bidirectional
+    VxmDense (atlas = moving image, input = fixed image), and a MeanStream keeps the capped running mean of the
+    full-resolution inverse flow so that a loss can pull the atlas towards the centre of the data:
+
+        y_source, y_target, mean_stream, pos_flow = model(image)
+        loss = w_img * L(image, y_source) + (1 - w_img) * L(atlas, y_target) + w_mean * MSE(0, mean_stream)
+               + w_grad * Grad('l2', loss_mult=2)(pos_flow)
+
+    `self.atlas` is an nn.Parameter of shape (1, atlas_feats, *inshape); the inner network is `self.vxm_model`
+    (checkpoint keys `vxm_model.*`), the mean stream's state the buffers `mean_stream.mean` / `mean_stream.count`.
+    `kwargs` are forwarded to the inner VxmDense."""
+
+    @store_config_args
+    def __init__(self, inshape, nb_unet_features=None, mean_cap=100, atlas_feats=1, src_feats=1, **kwargs):
+        super().__init__()
+        ndims = len(inshape)
+        self.atlas = nn.Parameter(Normal(0, 1e-7).sample((1, atlas_feats) + tuple(inshape)))
+        self.vxm_model = VxmDense(inshape, nb_unet_features, bidir=True, src_feats=atlas_feats, trg_feats=src_feats, **kwargs)
+        self.mean_stream = layers.MeanStream((ndims,) + tuple(inshape), cap=mean_cap)
+
+    def forward(self, image, registration=False):
+        from . import dist as vdist
+        if vdist.env_world()[0] > 1:
+            raise _lib.VxmError("TemplateCreation does not run data parallel yet: each rank would keep its own mean "
+                                "stream, and the atlas lies outside the inner model's gradient exchange; train it on "
+                                "one GPU (WORLD_SIZE=1)")
+        atlas_b = self.atlas.expand((image.shape[0],) + tuple(self.atlas.shape[1:]))
+        pos_flow, neg_flow, _ = self.vxm_model.flows(atlas_b, image)
+        y_source = self.vxm_model.transformer(atlas_b, pos_flow)
+        if registration:
+            return y_source, pos_flow
+        y_target = self.vxm_model.transformer(image, neg_flow)
+        return y_source, y_target, self.mean_stream(neg_flow), pos_flow
+
+    def set_atlas(self, atlas):
+        """Copy `atlas` into the atlas parameter in place (the Parameter object, and so an optimizer holding it, stays
+        the same).  Accepts a tensor or an array of shape (1, C, *vol), (C, *vol), or *vol when C == 1."""
+        a = torch.as_tensor(np.asarray(atlas) if not torch.is_tensor(atlas) else atlas, dtype=torch.float32)
+        shape = tuple(self.atlas.shape)
+        if a.dim() == len(shape) - 2 and shape[1] == 1:
+            a = a.reshape(shape)
+        elif a.dim() == len(shape) - 1:
+            a = a.unsqueeze(0)
+        if tuple(a.shape) != shape:
+            raise ValueError("set_atlas: expected an atlas of shape %s, got %s" % (shape, tuple(np.shape(atlas))))
+        with torch.no_grad():
+            self.atlas.copy_(a)
+
+    def get_atlas(self):
+        """The atlas as a squeezed numpy array, like the reference's get_atlas."""
+        return self.atlas.detach().cpu().numpy().squeeze()
+
+    # the transform from source to target and its application to an image, through the inner VxmDense
+    register = VxmDenseSemiSupervisedSeg.register
+    apply_transform = VxmDenseSemiSupervisedSeg.apply_transform

@@ -60,8 +60,10 @@ class GraphedTrainStep:
             dst.copy_(x)
         # the warm-up steps are real optimizer steps on the first inputs: snapshot the optimizer state and put it back, so
         # that a captured run follows the same trajectory as an eager run from the same seed (keep_warmup=True keeps
-        # them, e.g. to compare with an eager loop that also took them)
+        # them, e.g. to compare with an eager loop that also took them).  The model's buffers (a TemplateCreation's mean
+        # stream) are state the warm-up advances too
         snap = None if self.keep_warmup else self.opt.snapshot()
+        bufs = None if self.keep_warmup else [(b, b.clone()) for b in self.model.buffers()]
         dev = inputs[0].device
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream())
@@ -72,6 +74,9 @@ class GraphedTrainStep:
         torch.cuda.synchronize()
         if snap is not None:
             self.opt.restore(snap)
+            with torch.no_grad():
+                for b, saved in bufs:
+                    b.copy_(saved)
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.loss = self._step()
