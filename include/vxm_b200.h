@@ -307,6 +307,10 @@ int vxm_planar_to_ndhwc8_split_bf16(const float* const* planes, const long long*
                                     void* out_lo, int B, size_t V, void* stream);
 int vxm_pool2_split_ndhwc_bf16(const void* x_hi, const void* x_lo, void* y_hi, void* y_lo, int B, int Dc, int Hc, int Wc,
                                int C, int nd, void* stream);
+/* vxm_unpool_combine_ndhwc_bf16 after a split-precision pool: the pool gradient goes to the first child with the largest
+ * e_hi + e_lo (the child vxm_pool2_split_ndhwc_bf16 copied); the LeakyReLU derivative reads e_hi < 0 */
+int vxm_unpool_combine_split_ndhwc_bf16(const void* e_hi, const void* e_lo, const void* g_skip_fine, const void* g_pool_coarse,
+                                        void* out_fine, int B, int Dc, int Hc, int Wc, int C, int nd, float slope, void* stream);
 /* out[c] = sum_{b,v} x[b][c][v] for planar fp32 x (B,C,V), C <= 32; work: 128*C floats */
 int vxm_planar_channel_sums(const float* x, float* out, void* work, int B, int C, size_t V, void* stream);
 

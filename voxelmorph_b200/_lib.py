@@ -87,6 +87,7 @@ SIGNATURES = {
     "vxm_planar_to_ndhwc8_split_bf16": (c_i, [c_f, c_f, c_i, c_f, c_f, c_i, c_sz, c_f]),
     "vxm_planar_fold_kd_bf16": (c_i, [c_f, c_f, c_i, c_f, c_i, c_i, c_sz, c_i, c_f]),
     "vxm_pool2_split_ndhwc_bf16": (c_i, [c_f, c_f, c_f, c_f] + [c_i] * 6 + [c_f]),
+    "vxm_unpool_combine_split_ndhwc_bf16": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 6 + [c_fl, c_f]),
     "vxm_planar_channel_sums": (c_i, [c_f, c_f, c_f, c_i, c_i, c_sz, c_f]),
     "vxm_maxpool2_fwd": (c_i, [c_f, c_f, c_f] + [c_i] * 6 + [c_f]),
     "vxm_maxpool2_bwd": (c_i, [c_f, c_f, c_f] + [c_i] * 6 + [c_f]),

@@ -3,7 +3,8 @@
 //   sumpool_mask   : gradient through nearest-x2 upsampling (sum over the 2^nd children) times the LeakyReLU
 //                    derivative of the (coarse) decoder activation it belongs to;
 //   unpool_combine : gradient through MaxPool(2) (routed to the first maximal child, ATen's tie rule) plus the
-//                    skip-connection gradient, times the LeakyReLU derivative of the encoder activation.
+//                    skip-connection gradient, times the LeakyReLU derivative of the encoder activation (a split
+//                    variant routes to the child the split-precision pool chose on hi + lo).
 // All tensors are bf16 (B, D, H, W, C) with C % 8 == 0; one thread moves 8 channels (16 bytes) per voxel.
 // These are HBM-bound: algorithmic bytes = every operand once.
 #include <cuda_bf16.h>
@@ -97,9 +98,24 @@ __global__ void __launch_bounds__(256) sumpool_mask_kernel(const __nv_bfloat16* 
   st8(out + co, s);
 }
 
+// The split-precision MaxPool's choice, shared by its forward (pool_split_ndhwc_kernel) and its backward
+// (unpool_combine_kernel<true>): child (h, l) replaces the best so far when h + l is larger or NaN, so the first child with
+// the largest h + l wins ties (ATen's rule on the value the pair carries).
+__device__ __forceinline__ bool split_pool_takes(float h, float l, float& best) {
+  const float t = h + l;
+  if (t > best || t != t) {
+    best = t;
+    return true;
+  }
+  return false;
+}
+
+// SPLIT: the forward was the split-precision one, whose pool chose on hi + lo; e_fine holds hi and e_lo the lo parts.
+// The LeakyReLU derivative reads the sign of hi, as every other mask of the (bf16-operand) backward does.
+template <bool SPLIT>
 __global__ void __launch_bounds__(256) unpool_combine_kernel(const __nv_bfloat16* __restrict__ e_fine, const __nv_bfloat16* __restrict__ g_skip,
                                                              const __nv_bfloat16* __restrict__ g_pool, __nv_bfloat16* __restrict__ out,
-                                                             PoolGeom g, float slope) {
+                                                             PoolGeom g, float slope, const __nv_bfloat16* __restrict__ e_lo) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   int b, d, h, w, c8;
   if (!decode(g, i, b, d, h, w, c8)) return;
@@ -115,9 +131,16 @@ __global__ void __launch_bounds__(256) unpool_combine_kernel(const __nv_bfloat16
     if (k < nchild) {
       const int kd = g.fd == 2 ? (k >> 2) : 0, kh = (k >> 1) & 1, kw = k & 1;
       ev[k] = ld8(e_fine + fine_index(g, b, d, h, w, kd, kh, kw) * C + c8 * 8);
+      if constexpr (SPLIT) {
+        const V8 el = ld8(e_lo + fine_index(g, b, d, h, w, kd, kh, kw) * C + c8 * 8);
 #pragma unroll
-      for (int e = 0; e < 8; ++e)
-        if (ev[k].v[e] > best[e] || ev[k].v[e] != ev[k].v[e]) { best[e] = ev[k].v[e]; arg[e] = k; }
+        for (int e = 0; e < 8; ++e)
+          if (split_pool_takes(ev[k].v[e], el.v[e], best[e])) arg[e] = k;
+      } else {
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if (ev[k].v[e] > best[e] || ev[k].v[e] != ev[k].v[e]) { best[e] = ev[k].v[e]; arg[e] = k; }
+      }
     }
   }
   V8 gp;
@@ -241,7 +264,7 @@ __global__ void __launch_bounds__(256) planar_to_ndhwc8_split_kernel(PlanarSrc s
 }
 
 // MaxPool(2) of a (hi, lo) pair tensor: the maximum is taken on hi + lo, the winning child's pair is copied (first
-// maximal child wins ties, like ATen)
+// maximal child wins ties, like ATen; split_pool_takes)
 __global__ void __launch_bounds__(256) pool_split_ndhwc_kernel(const __nv_bfloat16* __restrict__ xh, const __nv_bfloat16* __restrict__ xl,
                                                                __nv_bfloat16* __restrict__ yh, __nv_bfloat16* __restrict__ yl, PoolGeom g) {
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -257,10 +280,8 @@ __global__ void __launch_bounds__(256) pool_split_ndhwc_kernel(const __nv_bfloat
         const size_t o = fine_index(g, b, d, h, w, kd, kh, kw) * C + c8 * 8;
         V8 th = ld8(xh + o), tl = ld8(xl + o);
 #pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float t = th.v[e] + tl.v[e];
-          if (t > m.v[e] || t != t) { m.v[e] = t; mh.v[e] = th.v[e]; ml.v[e] = tl.v[e]; }
-        }
+        for (int e = 0; e < 8; ++e)
+          if (split_pool_takes(th.v[e], tl.v[e], m.v[e])) { mh.v[e] = th.v[e]; ml.v[e] = tl.v[e]; }
       }
   const size_t o = ((((size_t)b * g.Dc + d) * g.Hc + h) * g.Wc + w) * C + c8 * 8;
   st8(yh + o, mh);
@@ -309,9 +330,21 @@ extern "C" int vxm_unpool_combine_ndhwc_bf16(const void* e_fine, const void* g_s
   int rc = make_pool_geom(B, Dc, Hc, Wc, C, nd, &g);
   if (rc) return rc;
   VXM_REQUIRE(e_fine && out && (g_skip || g_pool), "unpool_combine: null pointer");
-  unpool_combine_kernel<<<pool_grid(g), 256, 0, as_stream(stream)>>>((const __nv_bfloat16*)e_fine, (const __nv_bfloat16*)g_skip,
-                                                                     (const __nv_bfloat16*)g_pool, (__nv_bfloat16*)out, g, slope);
+  unpool_combine_kernel<false><<<pool_grid(g), 256, 0, as_stream(stream)>>>((const __nv_bfloat16*)e_fine, (const __nv_bfloat16*)g_skip,
+                                                                            (const __nv_bfloat16*)g_pool, (__nv_bfloat16*)out, g, slope, nullptr);
   return check_launch("unpool_combine");
+}
+
+extern "C" int vxm_unpool_combine_split_ndhwc_bf16(const void* e_hi, const void* e_lo, const void* g_skip, const void* g_pool, void* out,
+                                                   int B, int Dc, int Hc, int Wc, int C, int nd, float slope, void* stream) {
+  PoolGeom g;
+  int rc = make_pool_geom(B, Dc, Hc, Wc, C, nd, &g);
+  if (rc) return rc;
+  VXM_REQUIRE(e_hi && e_lo && out && (g_skip || g_pool), "unpool_combine_split: null pointer");
+  unpool_combine_kernel<true><<<pool_grid(g), 256, 0, as_stream(stream)>>>((const __nv_bfloat16*)e_hi, (const __nv_bfloat16*)g_skip,
+                                                                           (const __nv_bfloat16*)g_pool, (__nv_bfloat16*)out, g, slope,
+                                                                           (const __nv_bfloat16*)e_lo);
+  return check_launch("unpool_combine_split");
 }
 
 extern "C" int vxm_planar_channel_sums(const float* x, float* out, void* work, int B, int C, size_t V, void* stream) {

@@ -237,13 +237,20 @@ def _sumpool_mask(g_fine, act_coarse, nd, slope):
     return out
 
 
-def _unpool_combine(e_fine, g_skip, g_pool, nd, slope):
+def _unpool_combine(e_fine, g_skip, g_pool, nd, slope, e_lo=None):
+    """Gradient through MaxPool(2) plus the skip gradient, times the LeakyReLU derivative.  e_lo: the lo parts of a
+    split-precision forward, whose pool chose the child on hi + lo; the gradient then goes to that child."""
     lib = _lib.load()
     B, D, H, W, C = e_fine.shape
     Dc = D // 2 if nd == 3 else D
     out = torch.empty_like(e_fine)
-    _lib.check(lib.vxm_unpool_combine_ndhwc_bf16(_lib.ptr(e_fine), _lib.ptr(g_skip), _lib.ptr(g_pool), _lib.ptr(out), B, Dc, H // 2,
-                                                 W // 2, C, nd, slope, _lib.stream_ptr()), "vxm_unpool_combine_ndhwc_bf16")
+    if e_lo is None:
+        _lib.check(lib.vxm_unpool_combine_ndhwc_bf16(_lib.ptr(e_fine), _lib.ptr(g_skip), _lib.ptr(g_pool), _lib.ptr(out), B, Dc, H // 2,
+                                                     W // 2, C, nd, slope, _lib.stream_ptr()), "vxm_unpool_combine_ndhwc_bf16")
+    else:
+        _lib.check(lib.vxm_unpool_combine_split_ndhwc_bf16(_lib.ptr(e_fine), _lib.ptr(e_lo), _lib.ptr(g_skip), _lib.ptr(g_pool),
+                                                           _lib.ptr(out), B, Dc, H // 2, W // 2, C, nd, slope, _lib.stream_ptr()),
+                   "vxm_unpool_combine_split_ndhwc_bf16")
     return out
 
 
@@ -271,7 +278,8 @@ def _flat_grads(L):
 def forward_tape(model, source, target, split=False):
     """Runs Unet + flow head, returns (flow fp32 (B,nd,*vol), tape).  `split`: split-precision (bf16x3) forward — every
     activation is a (hi, lo) bf16 pair and every layer three tensor-core passes; the tape keeps the hi parts, which is
-    what the (bf16-operand) backward reads."""
+    what the (bf16-operand) backward reads, and the lo parts of the pool inputs, so that the backward routes each pool
+    gradient to the child the pool chose on hi + lo."""
     nd = source.dim() - 2
     kd = 3 if nd == 3 else 1
     _lib.require_cuda(source, target, what="VxmDense")
@@ -284,6 +292,7 @@ def forward_tape(model, source, target, split=False):
                             % (first.cin, plan.nd, len(planes), nd))
     tensors = {}         # tensor id -> bf16 NDHWC tensor
     lows = {}            # tensor id -> lo part (split precision only)
+    pool_lows = {}       # pool input id -> lo part, kept on the tape
     if split:
         tensors[0], lows[0] = tc.planar_to_ndhwc8_split(planes)
     elif first.fwd == "fold":
@@ -295,6 +304,7 @@ def forward_tape(model, source, target, split=False):
             _, src, dst = L
             if split:
                 tensors[dst], lows[dst] = tc.pool_split((tensors[src], lows[src]), nd)
+                pool_lows[src] = lows[src]
             else:
                 tensors[dst] = _pool(tensors[src], nd)
             continue
@@ -312,7 +322,7 @@ def forward_tape(model, source, target, split=False):
             tensors[L.out] = out
     if nd == 2:
         flow = flow.squeeze(2)
-    return flow, dict(plan=plan, tensors=tensors, split=split)
+    return flow, dict(plan=plan, tensors=tensors, split=split, pool_lows=pool_lows)
 
 
 def backward_tape(ctx, g_flow, image_grad=False):
@@ -335,7 +345,7 @@ def backward_tape(ctx, g_flow, image_grad=False):
     for L in reversed(plan.ops):
         if not isinstance(L, _Layer):
             _, src, dst = L
-            gz[src] = _unpool_combine(tensors[src], gskip.pop(src, None), graw.pop(dst), nd, plan.slope[src])
+            gz[src] = _unpool_combine(tensors[src], gskip.pop(src, None), graw.pop(dst), nd, plan.slope[src], ctx["pool_lows"].pop(src, None))
             continue
         xa, xb = tensors[L.a], tensors.get(L.b)
         if L.role == "flow":
