@@ -1,6 +1,7 @@
-"""The fp64 references of the exact convolution tests (conv_exact_ref.py) against fp64 autograd of F.conv3d, on small shapes
-with kd = 1 and 3, upsampled sources, concatenations and several depth slabs; and their epilogue emulation against a
-direct per-element fp32 computation with an explicit round-to-nearest-even to bf16."""
+"""The fp64 references of the exact convolution tests (conv_exact_ref.py) against fp64 autograd of F.conv3d (F.conv2d for
+2-D layers, held as (B, 1, H, W, C)), on small shapes with kd = 1 and 3, upsampled sources, concatenations and several
+depth slabs; and their epilogue emulation against a direct per-element fp32 computation with an explicit
+round-to-nearest-even to bf16."""
 import numpy as np
 import pytest
 import torch
@@ -9,31 +10,37 @@ import torch.nn.functional as F
 import conv_exact_ref as ref
 
 CASES = [
-    # (B, (D, H, W), Ca, Cb, up, Cout, kd)
+    # (B, (D, H, W) or (H, W) for a 2-D layer, Ca, Cb, up, Cout, kd)
     (2, (6, 5, 7), 3, 0, False, 4, 3),
     (1, (8, 6, 4), 3, 2, True, 5, 3),          # upsampled source + skip
     (2, (7, 4, 6), 4, 3, False, 2, 3),          # concatenation, odd depth
     (1, (5, 6, 5), 3, 2, False, 4, 1),          # kd = 1 (the kd-folded layers)
+    (2, (10, 6), 3, 2, True, 4, 1),             # 2-D: upsampled source (h and w only) + skip
+    (3, (5, 7), 4, 0, False, 3, 1),             # 2-D, odd sizes
 ]
 
 
 def _case(B, shape, Ca, Cb, up, Cout, kd, integer):
-    g = torch.Generator().manual_seed(B * 100 + Ca * 10 + Cb + kd)
-    D, H, W = shape
+    g = torch.Generator().manual_seed(B * 100 + Ca * 10 + Cb + kd + 1000 * (len(shape) == 2))
+    D, H, W = shape if len(shape) == 3 else (1,) + shape
+    Dc = D if len(shape) == 2 else D // 2
     gen = (lambda s: torch.randint(-3, 4, s, generator=g).double()) if integer else (lambda s: torch.randn(s, generator=g, dtype=torch.float64))
-    xa = gen((B, D // 2, H // 2, W // 2, Ca) if up else (B, D, H, W, Ca))
+    xa = gen((B, Dc, H // 2, W // 2, Ca) if up else (B, D, H, W, Ca))
     xb = gen((B, D, H, W, Cb)) if Cb else None
     w, b, gy = gen((Cout, Ca + Cb, kd, 3, 3)), gen((Cout,)), gen((B, D, H, W, Cout))
     return xa, xb, w, b, gy
 
 
-def _autograd(xa, xb, w, b, gy, up):
+def _autograd(xa, xb, w, b, gy, up, nd):
     xa, w, b = xa.clone().requires_grad_(True), w.clone().requires_grad_(True), b.clone().requires_grad_(True)
     xb = None if xb is None else xb.clone().requires_grad_(True)
-    x = ref.upsample2(xa) if up else xa
+    x = ref.upsample2(xa, nd) if up else xa
     if xb is not None:
         x = torch.cat([x, xb], -1)
-    y = F.conv3d(x.permute(0, 4, 1, 2, 3), w, b, padding=(w.shape[2] // 2, 1, 1)).permute(0, 2, 3, 4, 1)
+    if nd == 2:
+        y = F.conv2d(x[:, 0].permute(0, 3, 1, 2), w[:, :, 0], b, padding=1).permute(0, 2, 3, 1)[:, None]
+    else:
+        y = F.conv3d(x.permute(0, 4, 1, 2, 3), w, b, padding=(w.shape[2] // 2, 1, 1)).permute(0, 2, 3, 4, 1)
     (y * gy).sum().backward()
     return y.detach(), xa.grad, (None if xb is None else xb.grad), w.grad, b.grad
 
@@ -42,27 +49,28 @@ def _autograd(xa, xb, w, b, gy, up):
 @pytest.mark.parametrize("slab", [2, 3, ref.SLAB])
 @pytest.mark.parametrize("B,shape,Ca,Cb,up,Cout,kd", CASES)
 def test_reference_helpers_match_autograd(B, shape, Ca, Cb, up, Cout, kd, slab, integer):
+    nd = len(shape)
     xa, xb, w, b, gy = _case(B, shape, Ca, Cb, up, Cout, kd, integer)
-    y, gxa, gxb, gw, gb = _autograd(xa, xb, w, b, gy, up)
+    y, gxa, gxb, gw, gb = _autograd(xa, xb, w, b, gy, up, nd)
     srcs = [(xa, up)] + ([(xb, False)] if xb is not None else [])
-    D = shape[0]
+    D = gy.shape[1]
     # integer operands: both sides exact, so equal; random ones: fp64 rounding in different orders
     same = torch.equal if integer else (lambda a, c: torch.allclose(a, c, rtol=1e-12, atol=1e-12))
-    assert same(ref.conv(srcs, w, D, slab=slab) + b, y)
+    assert same(ref.conv(srcs, w, D, slab=slab, nd=nd) + b, y)
     # the finish hook sees every slab once, in order
-    parts = ref.conv(srcs, w, D, finish=lambda t, d0, d1: (d0, d1, t), slab=slab)
+    parts = ref.conv(srcs, w, D, finish=lambda t, d0, d1: (d0, d1, t), slab=slab, nd=nd)
     assert [(d0, d1) for d0, d1, _ in parts] == [(d, min(d + slab, D)) for d in range(0, D, slab)]
     assert same(torch.cat([t for _, _, t in parts], 1) + b, y)
     # dgrad: the transposed, flipped weight over the output gradient; the upsampled source's part summed over its children
     gx = ref.conv([(gy, False)], ref.dgrad_weight(w), D, slab=slab)
-    assert same(ref.children_sum(gx[..., :Ca]) if up else gx[..., :Ca], gxa)
+    assert same(ref.children_sum(gx[..., :Ca], nd) if up else gx[..., :Ca], gxa)
     if xb is not None:
         assert same(gx[..., Ca:], gxb)
-    gw_r, gb_r = ref.wgrad(srcs, gy, kd, slab=slab)
+    gw_r, gb_r = ref.wgrad(srcs, gy, kd, slab=slab, nd=nd)
     assert gw_r.shape == gw.shape and same(gw_r, gw) and same(gb_r, gb)
     # the absolute sums are the same sums over |x| and |gz|
-    ga, gba = ref.wgrad([(xa.abs(), up)] + ([(xb.abs(), False)] if xb is not None else []), gy.abs(), kd, slab=slab)
-    gw_a, gb_a = ref.wgrad(srcs, gy, kd, absolute=True, slab=slab)
+    ga, gba = ref.wgrad([(xa.abs(), up)] + ([(xb.abs(), False)] if xb is not None else []), gy.abs(), kd, slab=slab, nd=nd)
+    gw_a, gb_a = ref.wgrad(srcs, gy, kd, absolute=True, slab=slab, nd=nd)
     assert torch.equal(gw_a, ga) and torch.equal(gb_a, gba) and bool((gw_a >= gw_r.abs()).all())
 
 

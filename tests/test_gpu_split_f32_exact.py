@@ -22,7 +22,7 @@ import torch
 import torch.nn.functional as F
 
 import conv_exact_ref as ref
-from test_gpu_conv_exact import CAPS, DOUBLED, MODELS, _children, _unchildren, mism, ternary
+from test_gpu_conv_exact import CAPS, MODELS, _children, _unchildren, check_resolves, mism, plan_sizes, ternary
 
 pytestmark = pytest.mark.gpu
 
@@ -92,11 +92,11 @@ def _split_margin(cin, unit_terms, bias_units):
 # ---- 1. the bf16x3 forward, exactly, at the plan's own size -----------------------------------------------------------
 
 @pytest.mark.parametrize("name", sorted(MODELS))
-def test_split_forward_exact(vx, cuda, name):
+def test_split_forward_exact(vx, cuda, monkeypatch, name):
     """Every layer of the bf16x3 plan through _run(L.fwd_x3, L.pk_hi, ..., lo=(xa_lo, xb_lo, L.pk_lo)), as forward_tape
-    runs it; the first layer on the output of planar_to_ndhwc8_split."""
+    runs it; the first layer on the output of planar_to_ndhwc8_split.  Every model of the exact tier's matrix."""
     vxm, eng, tc = vx
-    kw = MODELS[name]
+    kw, B = MODELS[name].kw, MODELS[name].B
     g = torch.Generator(device=cuda).manual_seed(11 + len(name))
     model = vxm.networks.VxmDense(**kw).to(cuda)
     kj = {}
@@ -105,20 +105,15 @@ def test_split_forward_exact(vx, cuda, name):
             w, k, j = split_weight(p.shape, g)
             p.copy_(w)
             kj[p] = (k, j)
+    check_resolves(vxm, monkeypatch, name, model)
     plan = eng._plan_of(model, True)
     layers = plan.layers
+    nd, kd = plan.nd, (3 if plan.nd == 3 else 1)
     for L in layers:
         k, j = kj[L.w]
         assert torch.equal(L.w_hi, k * 2.0 ** -6) and torch.equal(L.w_lo, j * 2.0 ** -15)
-    size, chans = {0: tuple(kw["inshape"])}, {}
-    for op in plan.ops:
-        if isinstance(op, eng._Layer):
-            size[op.out], chans[op.out] = size[op.b if op.b is not None else op.a], op.cout
-        else:
-            _, s, d = op
-            size[d], chans[d] = tuple(v // 2 for v in size[s]), chans[s]
+    size, chans = plan_sizes(eng, plan, kw["inshape"])
     first, flow = layers[0], layers[-1]
-    B = 1
     # image planes (a + b 2^-9) / 16, b = 0 where a = 0: hi = a / 16 and lo = b 2^-13 exactly (the tie at a = 1, b = -1
     # rounds to even, 2^-4), so the first layer's products are multiples of 2^-19 that fit 24 bits with the bias
     planes = []
@@ -142,7 +137,7 @@ def test_split_forward_exact(vx, cuda, name):
     rows = [("00 images", "planar_to_ndhwc8_split", n_glue, 0.0)]
     for i, L in enumerate(layers):
         bias, D = L.bias.detach(), size[L.out][0]
-        out = eng._run(L.fwd_x3, L.pk_hi, XH[L.a], XH.get(L.b), L.cout, 3, bias, lo=(XL[L.a], XL.get(L.b), L.pk_lo),
+        out = eng._run(L.fwd_x3, L.pk_hi, XH[L.a], XH.get(L.b), L.cout, kd, bias, lo=(XL[L.a], XL.get(L.b), L.pk_lo),
                        up=L.up, slope=L.slope, out_fp32_planar=L is flow)
         if L is first:
             hs, ls = [(img_hi, False)], [(img_lo, False)]
@@ -151,21 +146,21 @@ def test_split_forward_exact(vx, cuda, name):
             hs = [(XH[L.a], L.up)] + ([(XH[L.b], False)] if L.b is not None else [])
             ls = [(XL[L.a], L.up)] + ([(XL[L.b], False)] if L.b is not None else [])
             margin = _split_margin(L.cin, 2 ** 10 + 2 + 1, 2 ** 10 + 1)            # units of 2^-15
-        w3 = torch.cat([L.w_hi, L.w_hi, L.w_lo], 1)                                # [hi, lo, hi] sources
+        w3 = torch.cat([L.w_hi, L.w_hi, L.w_lo], 1).view(L.cout, 3 * L.cin, kd, 3, 3)      # [hi, lo, hi] sources
         if L is flow:
             res = out.permute(0, 2, 3, 4, 1)
-            n = sum(ref.conv(hs + ls + hs, w3, D, finish=lambda y, d0, d1: mism(res[:, d0:d1], ref.epilogue(y, bias, bf16=False))))
+            n = sum(ref.conv(hs + ls + hs, w3, D, nd=nd, finish=lambda y, d0, d1: mism(res[:, d0:d1], ref.epilogue(y, bias, bf16=False))))
         else:
             oh, ol = out
 
             def fin(y, d0, d1):
                 h, lo = split_epilogue(y, bias, L.slope)
                 return mism(oh[:, d0:d1], h) + mism(ol[:, d0:d1], lo)
-            n = sum(ref.conv(hs + ls + hs, w3, D, finish=fin))
+            n = sum(ref.conv(hs + ls + hs, w3, D, nd=nd, finish=fin))
         kind = "one launch" if len(L.fwd_x3[0]) == len(L.fwd_x3[1]) == 1 else "%dx%d blocks" % (len(L.fwd_x3[0]), len(L.fwd_x3[1]))
         rows.append((lname(i, L), "fwd x3 " + kind + (" fp32 planar" if L is flow else ""), n, margin))
         del out
-    assert any(len(L.fwd_x3[0]) * len(L.fwd_x3[1]) > 1 for L in layers) == (name == "doubled")
+    assert any(len(L.fwd_x3[0]) * len(L.fwd_x3[1]) > 1 for L in layers) == MODELS[name].blocked
     _report("bf16x3 forward exact %s" % name, rows)
 
 
@@ -195,28 +190,13 @@ def test_planar_to_ndhwc8_split_exact(vx, cuda, nplanes):
 
 def _split_argmax(hi, lo, nd):
     """one-hot (.., nchild, C) of the first child with the largest hi + lo (fp32 add), and of the first with the largest hi"""
-    ch, cl = _children_nd(hi, nd).float(), _children_nd(lo, nd).float()
+    ch, cl = _children(hi, nd).float(), _children(lo, nd).float()
     v = ch + cl
     one_hot = []
     for t in (v, ch):
         is_max = t == t.max(-2, keepdim=True).values
         one_hot.append(is_max & (is_max.cumsum(-2) == 1))
     return one_hot
-
-
-def _children_nd(x, nd):
-    """(B, D, H, W, C) -> (B, Dc, Hc, Wc, nchild, C), children in the kernels' (kd, kh, kw) order"""
-    if nd == 3:
-        return _children(x)
-    B, D, H, W, C = x.shape
-    return x.reshape(B, D, H // 2, 2, W // 2, 2, C).permute(0, 1, 2, 4, 3, 5, 6).reshape(B, D, H // 2, W // 2, 4, C)
-
-
-def _unchildren_nd(c, nd):
-    if nd == 3:
-        return _unchildren(c)
-    B, D, Hc, Wc, _, C = c.shape
-    return c.reshape(B, D, Hc, Wc, 2, 2, C).permute(0, 1, 2, 4, 3, 5, 6).reshape(B, D, 2 * Hc, 2 * Wc, C)
 
 
 @pytest.mark.parametrize("nd", [3, 2])
@@ -229,10 +209,10 @@ def test_pool_split_exact(vx, cuda, nd):
     hi, lo = ternary(shape, g), (ternary(shape, g).float() * LO).to(torch.bfloat16)
     yh, yl = tc.pool_split((hi, lo), nd)
     first, first_hi = _split_argmax(hi, lo, nd)
-    rh = (_children_nd(hi, nd).float() * first).sum(-2)
-    rl = (_children_nd(lo, nd).float() * first).sum(-2)
+    rh = (_children(hi, nd).float() * first).sum(-2)
+    rl = (_children(lo, nd).float() * first).sum(-2)
     differ = int((first != first_hi).any(-2).sum())
-    v = _children_nd(hi, nd).float() + _children_nd(lo, nd).float()
+    v = _children(hi, nd).float() + _children(lo, nd).float()
     both = int(((v == v.max(-2, keepdim=True).values).sum(-2) > 1).sum())
     n = mism(yh, rh) + mism(yl, rl)
     print("\n[pool_split %d-D, full size] mismatches %d; pooled outputs whose hi argmax differs from the hi + lo one %d, "
@@ -317,9 +297,9 @@ def _expected_unpool(e_hi, e_lo, g_skip, g_pool, nd, slope):
     first, first_hi = _split_argmax(e_hi, e_lo, nd)
     r = first.float() * g_pool.float().unsqueeze(-2)
     if g_skip is not None:
-        r = r + _children_nd(g_skip, nd).float()
-    r = torch.where(_children_nd(e_hi, nd) < 0, r * torch.tensor(slope, dtype=torch.float32, device=r.device), r)
-    return _unchildren_nd(r, nd).to(torch.bfloat16), int((first != first_hi).any(-2).sum())
+        r = r + _children(g_skip, nd).float()
+    r = torch.where(_children(e_hi, nd) < 0, r * torch.tensor(slope, dtype=torch.float32, device=r.device), r)
+    return _unchildren(r, nd).to(torch.bfloat16), int((first != first_hi).any(-2).sum())
 
 
 def _record_pools(monkeypatch, eng, tc):
@@ -359,29 +339,31 @@ def _check_routing(title, calls):
 def test_split_pool_routing_deterministic(vx, cuda, monkeypatch):
     """A first layer that copies image plane 0 (centre tap 1, every other weight and the bias 0) on images 1 + ~2^-10
     noise: every child of the first pool has hi = 1 and lo alone decides which child the forward takes.  The backward
-    must send each pooled gradient to that child."""
+    must send each pooled gradient to that child.  A 3-D model (8 children), then a 2-D one with B = 2 (4 children)."""
     vxm, eng, tc = vx
     monkeypatch.setenv("VXM_B200_CONV_ENGINE", "bf16x3")
-    shape = (32, 48, 64)
-    g = torch.Generator(device=cuda).manual_seed(50)
-    torch.manual_seed(53)
-    model = vxm.networks.VxmDense(inshape=shape).to(cuda)
-    conv0 = model.unet_model.encoder[0][0].main
-    with torch.no_grad():
-        conv0.weight.zero_()
-        conv0.bias.zero_()
-        conv0.weight[:, 0, 1, 1, 1] = 1.0
-    src = 1 + (torch.rand((1, 1) + shape, generator=g, device=cuda) - 0.5) * 2.0 ** -9
-    trg = torch.rand((1, 1) + shape, generator=g, device=cuda)
-    calls = _record_pools(monkeypatch, eng, tc)
-    _, flow = model(src, trg)
-    (flow * torch.randn(flow.shape, generator=g, device=cuda)).sum().backward()
-    torch.cuda.synchronize()
-    hi0 = calls[-1][0]                       # the backward runs the first pool last
-    assert bool((hi0 == 1).all())
-    rows = _check_routing("routing, first layer copies 1 + noise", calls)
-    assert rows[-1][1] > 0
-    assert all(n == 0 for n, _ in rows), rows
+    for shape, B, seed in (((32, 48, 64), 1, 50), ((96, 128), 2, 54)):
+        nd = len(shape)
+        g = torch.Generator(device=cuda).manual_seed(seed)
+        torch.manual_seed(seed + 3)
+        model = vxm.networks.VxmDense(inshape=shape).to(cuda)
+        conv0 = model.unet_model.encoder[0][0].main
+        with torch.no_grad():
+            conv0.weight.zero_()
+            conv0.bias.zero_()
+            conv0.weight[(slice(None), 0) + (1,) * nd] = 1.0
+        src = 1 + (torch.rand((B, 1) + shape, generator=g, device=cuda) - 0.5) * 2.0 ** -9
+        trg = torch.rand((B, 1) + shape, generator=g, device=cuda)
+        with monkeypatch.context() as m:
+            calls = _record_pools(m, eng, tc)
+            _, flow = model(src, trg)
+            (flow * torch.randn(flow.shape, generator=g, device=cuda)).sum().backward()
+            torch.cuda.synchronize()
+        hi0 = calls[-1][0]                       # the backward runs the first pool last
+        assert bool((hi0 == 1).all()) and all(c[4] == nd for c in calls)
+        rows = _check_routing("routing, %d-D first layer copies 1 + noise, B = %d" % (nd, B), calls)
+        assert rows[-1][1] > 0
+        assert all(n == 0 for n, _ in rows), rows
 
 
 def test_split_pool_routing_full_size_step(vx, cuda, monkeypatch):
@@ -410,34 +392,63 @@ def test_split_pool_routing_full_size_step(vx, cuda, monkeypatch):
 
 # ---- 5. the fp32 engine, exactly, at the step's sizes ---------------------------------------------------------------------
 
+# models VXM_B200_CONV_ENGINE=tc runs on f32: feature counts the tensor cores lack, more than 8 image planes
+F32_MODELS = {"ragged": dict(inshape=(96, 112, 128), nb_unet_features=[[16, 24, 24, 24], [24, 24, 24, 24, 24, 12, 12]]),
+              "planes9": dict(inshape=(64, 96, 112), src_feats=5, trg_feats=4)}
+
+
 def _model_convs(name):
-    """Every convolution of the model MODELS[name] in execution order, from the model's own modules: (label, cin, cout,
-    (D, H, W) it runs at, activation).  Encoder level i runs at inshape / 2^i, decoder level j at inshape / 2^(levels - 1 - j)
-    (its convolutions precede the upsampling), the remaining convolutions and the flow head at full size."""
+    """Every convolution of the model MODELS[name] or F32_MODELS[name] in execution order, from the model's own modules:
+    (label, cin, cout, (D, H, W) it runs at (D = 1 in 2-D), B, activation, model name).  Encoder level i runs at
+    inshape / 2^i, decoder level j at inshape / 2^(levels - 1 - j) (its convolutions precede the upsampling), the
+    remaining convolutions and the flow head at full size (half size in a half-resolution U-Net, which skips the last
+    upsampling)."""
     import voxelmorph_b200 as vxm
-    kw = MODELS[name]
+    kw, B = (MODELS[name].kw, MODELS[name].B) if name in MODELS else (F32_MODELS[name], 1)
     inshape = tuple(kw["inshape"])
     model = vxm.networks.VxmDense(**kw)
     unet = model.unet_model
-    assert not unet.half_res
+    top = 1 if unet.half_res else 0
     levels = [(i, convs) for i, convs in enumerate(unet.encoder)] + \
-             [(unet.nb_levels - 1 - j, convs) for j, convs in enumerate(unet.decoder)] + [(0, unet.remaining)]
+             [(unet.nb_levels - 1 - j, convs) for j, convs in enumerate(unet.decoder)] + [(top, unet.remaining)]
     out = []
     for level, convs in levels:
         for blk in convs:
             out.append((level, blk.main, True))
-    out.append((0, model.flow, False))
+    out.append((top, model.flow, False))
     return [("%s %02d %d->%d %s" % (name, i, m.in_channels, m.out_channels, "x".join(str(v >> level) for v in inshape)),
-             m.in_channels, m.out_channels, tuple(v >> level for v in inshape), 1, act) for i, (level, m, act) in enumerate(out)]
+             m.in_channels, m.out_channels, (1,) * (3 - len(inshape)) + tuple(v >> level for v in inshape), B, act, name)
+            for i, (level, m, act) in enumerate(out)]
+
+
+# (cin, cout, shape (D, H, W; D = 1 for 2-D), B, activation): channel counts that end the kernels' blocks early.  Forward
+# output blocks COB 8 / 16 / 32 by cout (dgrad: by cin), input stages CCK 4; weight gradient blocks WCO 16 x WCI 8.
+# H and W are not multiples of the 32 x 16 (forward) and 32 x 8 (weight gradient) tiles.
+RAGGED = [
+    (1, 8, (11, 37, 45), 3, True),        # CCK stage of 1; dgrad: COB 8 of 1; WCI of 1; WCO cut at 8
+    (3, 12, (1, 75, 101), 1, True),       # 2-D; partial COB 16, CCK stage of 3; dgrad: COB 8 of 3
+    (5, 40, (13, 29, 70), 1, True),       # second COB 32 block of 8; WCI of 5; WCO: 16 + 16 + 8
+    (9, 48, (1, 150, 203), 3, True),      # 2-D; second COB 32 block of 16; CCK 4 + 4 + 1; WCI 8 + 1; dgrad: COB 16 of 9
+    (24, 2, (9, 45, 77), 3, True),        # COB 8 of 2; dgrad: COB 32 of 24, CCK stage of 2; WCO cut at 2
+    (40, 24, (1, 83, 99), 1, True),       # 2-D; COB 32 of 24; dgrad: second COB 32 block of 8; WCO 16 + 8
+    (24, 48, (7, 21, 53), 1, True),       # dgrad: COB 32 of 24; WCI 8 x 3; WCO 16 x 3
+    (40, 12, (1, 61, 133), 3, True),      # 2-D; partial COB 16; dgrad: second COB 32 block of 8; WCI 8 x 5
+    (9, 24, (5, 39, 66), 3, True),        # WCI 8 + 1, WCO 16 + 8; dgrad: COB 16 of 9 over a CCK of 24
+    (5, 2, (1, 37, 45), 3, True),         # 2-D; COB 8 of 2, CCK stage of 1 after a full one; dgrad: COB 8 of 5
+    (16, 2, (1, 192, 224), 3, False),     # the 2-D flow head
+]
 
 
 def _f32_cases():
-    # (label, cin, cout, shape (D, H, W; D = 1 with kd = 1 for 2-D), B, activation)
-    return _model_convs("default") + _model_convs("doubled") + [("2-D 32->16 B=2", 32, 16, (1, 192, 224), 2, True)]
+    # (label, cin, cout, shape (D, H, W; D = 1 with kd = 1 for 2-D), B, activation, model or None)
+    return (_model_convs("default") + _model_convs("doubled") + [("2-D 32->16 B=2", 32, 16, (1, 192, 224), 2, True, None)]
+            + _model_convs("2d_halfres") + _model_convs("ragged") + _model_convs("planes9")
+            + [("%s %d->%d %s B=%d" % ("2-D" if D == 1 else "3-D", cin, cout, "x".join(map(str, (D, H, W) if D > 1 else (H, W))), B),
+                cin, cout, (D, H, W), B, act, None) for cin, cout, (D, H, W), B, act in RAGGED])
 
 
 @pytest.mark.parametrize("case", _f32_cases(), ids=lambda c: c[0].replace(" ", "_"))
-def test_f32_conv_exact(vx, cuda, case):
+def test_f32_conv_exact(vx, cuda, monkeypatch, case):
     """vxm_conv3d_fwd_f32 / vxm_conv3d_bwd_f32 through the C ABI: forward (bias, LeakyReLU), dgrad with the LeakyReLU
     mask of a saved activation, weight and bias gradients accumulated onto integer-valued priors (split_reduce_kernel
     adds its 2 * SM split-K partials with +=), all equal to fp64.  Operands: x in {-1, 0, 1} (first layer: / 16),
@@ -445,7 +456,10 @@ def test_f32_conv_exact(vx, cuda, case):
     full-size bias gradient's partial sums would reach a third of 2^24 units)."""
     vxm, _, _ = vx
     lib = vxm._lib.load()
-    name, cin, cout, shape, B, act = case
+    name, cin, cout, shape, B, act, model = case
+    if model in F32_MODELS:
+        monkeypatch.setenv("VXM_B200_CONV_ENGINE", "tc")
+        assert vxm.ops.resolve_engine(vxm.networks.VxmDense(**F32_MODELS[model])) == "f32"
     D, H, W = shape
     kd = 1 if D == 1 else 3
     first = cin <= 8
@@ -489,29 +503,37 @@ def test_f32_conv_exact(vx, cuda, case):
 
 def test_f32_pool_upcat_exact(vx, cuda):
     """maxpool2 (forward and backward: the gradient to the first maximal child) and upsample2_cat (forward and backward)
-    of unet_ops.cu against torch at full resolution, with ternary inputs so that ties are frequent."""
+    of unet_ops.cu against torch at full resolution, with ternary inputs so that ties are frequent: 3-D (1, C, 160, 192,
+    224) and 2-D (8, C, 192, 224), the f32 engine's planar layout."""
     vxm, _, _ = vx
     from voxelmorph_b200 import ops
-    g = torch.Generator(device=cuda).manual_seed(60)
-    x = ternary((1, 16) + FULL, g, torch.float32).requires_grad_(True)
-    y = ops.maxpool2(x)
-    gy = ternary(y.shape, g, torch.float32)
-    y.backward(gy)
-    ch = _children(x.detach().permute(0, 2, 3, 4, 1))
-    is_max = ch == ch.max(4, keepdim=True).values
-    first = is_max & (is_max.cumsum(4) == 1)
-    assert bool((is_max.sum(4) > 1).any())
-    n_pool = mism(y.detach(), F.max_pool3d(x.detach(), 2))
-    n_pool_bwd = mism(x.grad, _unchildren(first.float() * gy.permute(0, 2, 3, 4, 1).unsqueeze(4)).permute(0, 4, 1, 2, 3))
-    a = ternary((1, 32, 80, 96, 112), g, torch.float32).requires_grad_(True)
-    skip = ternary((1, 16) + FULL, g, torch.float32).requires_grad_(True)
-    out = ops.upsample2_cat(a, skip)
-    go = ternary(out.shape, g, torch.float32)
-    out.backward(go)
-    up = a.detach().repeat_interleave(2, 2).repeat_interleave(2, 3).repeat_interleave(2, 4)
-    n_up = mism(out.detach(), torch.cat([up, skip.detach()], 1))
-    n_up_bwd = mism(a.grad, ref.children_sum(go[:, :32].permute(0, 2, 3, 4, 1).double()).float().permute(0, 4, 1, 2, 3)) + \
-        mism(skip.grad, go[:, 32:])
-    print("\n[f32 glue, full size] maxpool2 %d | its backward %d | upsample2_cat %d | its backward %d mismatches"
-          % (n_pool, n_pool_bwd, n_up, n_up_bwd))
-    assert n_pool == n_pool_bwd == n_up == n_up_bwd == 0
+    for nd, B, fine, seed in ((3, 1, FULL, 60), (2, 8, FULL[1:], 61)):
+        g = torch.Generator(device=cuda).manual_seed(seed)
+        coarse = tuple(v // 2 for v in fine)
+
+        def cl(t):            # (B, C, [D,] H, W) -> channels-last (B, D, H, W, C), D = 1 in 2-D
+            return t.permute(0, 2, 3, 4, 1) if nd == 3 else t.permute(0, 2, 3, 1)[:, None]
+
+        def planar(t):        # the inverse of cl
+            return t.permute(0, 4, 1, 2, 3) if nd == 3 else t[:, 0].permute(0, 3, 1, 2)
+        x = ternary((B, 16) + fine, g, torch.float32).requires_grad_(True)
+        y = ops.maxpool2(x)
+        gy = ternary(y.shape, g, torch.float32)
+        y.backward(gy)
+        ch = _children(cl(x.detach()), nd)
+        is_max = ch == ch.max(4, keepdim=True).values
+        first = is_max & (is_max.cumsum(4) == 1)
+        assert bool((is_max.sum(4) > 1).any())
+        n_pool = mism(y.detach(), (F.max_pool3d if nd == 3 else F.max_pool2d)(x.detach(), 2))
+        n_pool_bwd = mism(x.grad, planar(_unchildren(first.float() * cl(gy).unsqueeze(4), nd)))
+        a = ternary((B, 32) + coarse, g, torch.float32).requires_grad_(True)
+        skip = ternary((B, 16) + fine, g, torch.float32).requires_grad_(True)
+        out = ops.upsample2_cat(a, skip)
+        go = ternary(out.shape, g, torch.float32)
+        out.backward(go)
+        up = planar(ref.upsample2(cl(a.detach()), nd))
+        n_up = mism(out.detach(), torch.cat([up, skip.detach()], 1))
+        n_up_bwd = mism(a.grad, planar(ref.children_sum(cl(go[:, :32]).double(), nd).float())) + mism(skip.grad, go[:, 32:])
+        print("\n[f32 glue, full size, %d-D, B = %d] maxpool2 %d | its backward %d | upsample2_cat %d | its backward %d mismatches"
+              % (nd, B, n_pool, n_pool_bwd, n_up, n_up_bwd))
+        assert n_pool == n_pool_bwd == n_up == n_up_bwd == 0
