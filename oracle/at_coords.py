@@ -11,6 +11,8 @@ exactly) and do everything else in float64:
   F.grid_sample(align_corners=True, padding_mode="zeros") defines it, and its adjoints with respect to the
   source and to the coordinates;
 * `coords_fp32`: fl32(p + v), the coordinates the fast warp and VecInt kernels form;
+* `coords_replayed`: the fp32 coordinates of torch's normalise / un-normalise round trip (`spec_np._sample_coords`),
+  which the exact-arithmetic warp and VecInt kernels form;
 * `quantised`: a smooth field whose values are odd multiples of 2^-11 with |v| < 2^7, so that p + v is exact in fp32
   and never integral: every sampler, whatever its coordinate arithmetic, then picks the same trilinear cell;
 * `vecint_step` / `vecint_adjoint`: one scaling-and-squaring step v + v(p + v), and the adjoint of the whole
@@ -104,6 +106,14 @@ def coords_fp32(v):
     return (grid[None] + v).astype(np.float32)
 
 
+def coords_replayed(v, div="true"):
+    """The fp32 sample coordinates of the reference's round trip p + v -> [-1, 1] -> voxel units for a (B, nd, *S) field
+    (spec_np._sample_coords, stacked on axis 1): those of the exact-arithmetic warp / VecInt kernels.  `div` as in
+    spec_np.warp ('true': torch CPU's division, 'recip': torch CUDA's multiply by the reciprocal)."""
+    from . import spec_np
+    return np.stack(spec_np._sample_coords(v, div), axis=1)
+
+
 def quantised(seed, channels, shape, scale):
     """cases.smooth_field(seed, channels, shape, scale) rounded to odd multiples of 2^-11 (|v| < 2^7 asserted): p + v is
     exact in fp32 for any voxel index p < 2^12 and never an integer, so fp64 round-off cannot move a sample across a
@@ -120,11 +130,12 @@ def vecint_step(v):
     return np.asarray(v, np.float64) + sample(v, coords_fp32(v))
 
 
-def vecint_adjoint(states, gout, scale):
-    """d(v_n)/d(vel)^T gout for the chain v_0 = scale * vel, v_{k+1} = v_k + v_k(fl32(p + v_k)), evaluated along the
-    given states v_0 .. v_{n-1} (each (B, nd, *S)) with their fp32 coordinates."""
+def vecint_adjoint(states, gout, scale, coords=coords_fp32):
+    """d(v_n)/d(vel)^T gout for the chain v_0 = scale * vel, v_{k+1} = v_k + v_k(c(v_k)), evaluated along the given
+    states v_0 .. v_{n-1} (each (B, nd, *S)) at the coordinates `coords(v_k)`: fl32(p + v_k) by default, or e.g.
+    `coords_replayed`.  Both have d c / d v = 1 in exact arithmetic, which is what the adjoint uses."""
     g = np.asarray(gout, np.float64)
     for v in reversed(states):
-        gs, gc = sample_adjoint(v, coords_fp32(v), g)
+        gs, gc = sample_adjoint(v, coords(v), g)
         g = g + gs + gc
     return g * scale

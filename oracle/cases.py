@@ -64,3 +64,18 @@ def volume_pair(seed, shape, sigma=3.0):
     flow = smooth_field(seed + 1, len(shape), shape, scale=sigma)
     trg = spec_np.warp(src, flow)
     return src, trg
+
+
+def dice_floor_pair():
+    """(y_true, y_pred) (1, 5, 2, 3) float32 where Dice's clamp decides: per label one (batch, label) pair whose bottom
+    sum is exactly the fp32 floor fl32(1e-5) (y_true = y_pred = [fl32(5e-6), 0, ...]), one a step below it, one a step
+    above it, one ordinary label, and one with both maps empty."""
+    h = F32(5e-6)
+    assert F32(h + h) == F32(1e-5)
+    yt = np.zeros((1, 5, 2, 3), F32)
+    yp = np.zeros_like(yt)
+    for lab, x in enumerate([h, np.nextafter(h, F32(0)), np.nextafter(h, F32(1))]):
+        yt[0, lab, 0, 0] = yp[0, lab, 0, 0] = x
+    yt[0, 3] = [[1, 0, 1], [0.5, 0, 0]]
+    yp[0, 3] = [[0.25, 1, 1], [0, 0.75, 0]]
+    return yt, yp

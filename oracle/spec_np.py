@@ -109,12 +109,15 @@ def warp(src, flow, mode="bilinear", div="true"):
     return out
 
 
-def vecint(vec, nsteps):
-    """Scaling and squaring (reference layers.py:61,64-68)."""
+def vecint(vec, nsteps, div="true", states=None):
+    """Scaling and squaring (reference layers.py:61,64-68).  `div` as in `warp`; a list passed as `states` receives
+    every field the squarings start from (v_0 .. v_{nsteps-1})."""
     assert nsteps >= 0
     vec = (np.asarray(vec, dtype=F32) * F32(1.0 / (2 ** nsteps))).astype(F32)
     for _ in range(nsteps):
-        vec = (vec + warp(vec, vec)).astype(F32)
+        if states is not None:
+            states.append(vec)
+        vec = (vec + warp(vec, vec, div=div)).astype(F32)
     return vec
 
 
@@ -246,14 +249,46 @@ def mse_loss(y_true, y_pred):
     return (d * d).mean()
 
 
-def dice_loss(y_true, y_pred):
+# torch.clamp(t, min=1e-5) on a float32 tensor compares against the scalar rounded to float32
+DICE_FLOOR = float(F32(1e-5))
+
+
+def dice_loss(y_true, y_pred, floor=DICE_FLOOR):
     """losses.py:84-90."""
     a = np.asarray(y_true, np.float64)
     b = np.asarray(y_pred, np.float64)
     ax = tuple(range(2, a.ndim))
     top = 2 * (a * b).sum(axis=ax)
-    bottom = np.maximum((a + b).sum(axis=ax), 1e-5)
+    bottom = np.maximum((a + b).sum(axis=ax), floor)
     return -(top / bottom).mean()
+
+
+def dice_coefs(y_true, y_pred, floor=DICE_FLOOR):
+    """(loss, k1, k2) of `dice_loss` in float64, k1 and k2 shaped (B, L): d/dy_pred = k1 * y_true - k2 and
+    d/dy_true = k1 * y_pred - k2.  The clamp's backward passes the gradient where the bottom sum is >= the floor
+    ([torch] clamp_backward: grad * (self >= min)), the floor included.  Sums are formed one (batch, label) at a
+    time, so full-size one-hot maps need no float64 copy."""
+    B, L = np.shape(y_true)[:2]
+    top, bsum = np.zeros((B, L)), np.zeros((B, L))
+    for b in range(B):
+        for lab in range(L):
+            a = np.asarray(y_true[b, lab], np.float64)
+            p = np.asarray(y_pred[b, lab], np.float64)
+            top[b, lab] = 2 * (a * p).sum()
+            bsum[b, lab] = (a + p).sum()
+    bottom = np.maximum(bsum, floor)
+    n = B * L
+    k1 = -2.0 / n / bottom
+    k2 = np.where(bsum >= floor, -top / (bottom * bottom) / n, 0.0)
+    return -(top / bottom).mean(), k1, k2
+
+
+def dice_grad(y_true, y_pred, floor=DICE_FLOOR):
+    """(loss, d/dy_true, d/dy_pred) of `dice_loss` in float64 (`dice_coefs` broadcast over the volume)."""
+    loss, k1, k2 = dice_coefs(y_true, y_pred, floor)
+    sh = k1.shape + (1,) * (np.ndim(y_true) - 2)
+    k1, k2 = k1.reshape(sh), k2.reshape(sh)
+    return loss, k1 * np.asarray(y_pred, np.float64) - k2, k1 * np.asarray(y_true, np.float64) - k2
 
 
 # --------------------------------------------------------------------------------------
@@ -300,8 +335,11 @@ def upsample2_nearest(x):
     return x
 
 
-def adam_step(p, g, m, v, step, lr=1e-4, b1=0.9, b2=0.999, eps=1e-8):
-    """torch.optim.Adam single-tensor update (scripts/torch/train.py:161,220), float64."""
+def adam_step(p, g, m, v, step, lr=1e-4, b1=0.9, b2=0.999, eps=1e-8, weight_decay=0.0):
+    """torch.optim.Adam single-tensor update (scripts/torch/train.py:161,220), float64.  weight_decay as torch.optim.Adam
+    applies it: g + weight_decay * p (L2, not decoupled)."""
+    if weight_decay:
+        g = g + weight_decay * p
     m = b1 * m + (1 - b1) * g
     v = b2 * v + (1 - b2) * g * g
     bc1 = 1 - b1 ** step

@@ -170,3 +170,36 @@ def test_eval_helpers_known_answers():
     b = np.array([[0, 1, 0], [2, 0, 0]])
     assert np.allclose(spec_np.dice_overlap(a, b), [2 * 1 / 3, 2 * 1 / 3])
     assert np.allclose(spec_np.dice_overlap(a, b, labels=[5]), [0.0])
+
+
+def test_dice_grad_at_the_floor_vs_torch_fp32():
+    """The fp64 Dice oracle against torch's fp32 CPU autograd of the reference's formula where the clamp decides: at
+    the floor the clamp passes the gradient (d/dy = [-0.5, 0.5] / L at the sample, not [-1, 0] / L)."""
+    yt, yp = cases.dice_floor_pair()
+    a, b = t(yt).requires_grad_(True), t(yp).requires_grad_(True)
+    loss = ref_torch.dice_loss(a, b)
+    loss.backward()
+    l64, g_true, g_pred = spec_np.dice_grad(yt, yp)
+    assert abs(loss.item() - l64) <= 1e-7
+    assert abs(l64 - spec_np.dice_loss(yt, yp)) <= 1e-15
+    L = yt.shape[1]
+    np.testing.assert_allclose(g_pred[0, 0, 0, :2], [-0.5 / L, 0.5 / L], rtol=1e-6)    # at the floor: both terms
+    np.testing.assert_allclose(g_pred[0, 1, 0, :2], [-1.0 / L * (2 * float(yt[0, 1, 0, 0]) / spec_np.DICE_FLOOR), 0.0],
+                               rtol=1e-6)                                              # below: the clamp blocks
+    for g32, g64 in ((a.grad, g_true), (b.grad, g_pred)):
+        np.testing.assert_allclose(g32.numpy(), g64, rtol=1e-6, atol=1e-6 * np.abs(g64).max())
+
+
+def test_adam_weight_decay_vs_torch_fp64():
+    rng = np.random.default_rng(1)
+    p = rng.standard_normal(200)
+    m, v = np.zeros(200), np.zeros(200)
+    tp = torch.tensor(p, dtype=torch.float64, requires_grad=True)
+    opt = torch.optim.Adam([tp], lr=3e-3, betas=(0.8, 0.99), eps=1e-6, weight_decay=1e-2)
+    for step in range(1, 6):
+        g = rng.standard_normal(200) * 10.0 ** rng.uniform(-6, 1, 200)
+        g[rng.random(200) < 0.2] = 0
+        tp.grad = torch.tensor(g)
+        opt.step()
+        p, m, v = spec_np.adam_step(p, g, m, v, step, lr=3e-3, b1=0.8, b2=0.99, eps=1e-6, weight_decay=1e-2)
+        np.testing.assert_allclose(tp.detach().numpy(), p, rtol=1e-12, atol=1e-14)

@@ -132,7 +132,8 @@ __global__ void __launch_bounds__(256) dice_bwd_kernel(const float* __restrict__
   float bc = fmaxf(bot, 1e-5f);
   float s = -__ldg(gl) / (float)BL;
   float k1 = s * 2.f / bc;
-  float k2 = bot > 1e-5f ? s * top / (bc * bc) : 0.f;  // clamp passes gradient only above the floor
+  // torch.clamp(min=1e-5) passes the gradient where its input is >= the floor (ATen clamp_backward), the floor included
+  float k2 = bot >= 1e-5f ? s * top / (bc * bc) : 0.f;
   const float* t = yt + (size_t)bl * V;
   float* o = gp + (size_t)bl * V;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < V; i += (size_t)gridDim.x * blockDim.x)
