@@ -135,6 +135,24 @@ int vxm_mse_fwd(const float* y_true, const float* y_pred, float* loss, void* wor
                 void* stream);
 int vxm_mse_bwd(const float* y_true, const float* y_pred, const float* grad_loss,
                 float* grad_pred, size_t n, void* stream);
+/* MSE(image_sigma) of reference voxelmorph/tf/losses.py:112-134: loss[0] = scale * mean (y_true - y_pred)^2 with
+ * scale = 1 / image_sigma^2 (vxm_mse_fwd / _bwd are these with scale 1) */
+int vxm_mse_scaled_fwd(const float* y_true, const float* y_pred, float* loss, void* work, size_t n, double scale,
+                       void* stream);
+int vxm_mse_scaled_bwd(const float* y_true, const float* y_pred, const float* grad_loss, float* grad_pred, size_t n,
+                       double scale, void* stream);
+
+/* ---- KL(prior_lambda) of probabilistic VoxelMorph: reference voxelmorph/tf/losses.py:247-349 ----
+ * params: flow_params (B, 2 nd, D, H, W) (D == 1 for nd == 2), channels [0, nd) the mean mu, [nd, 2 nd) l = log sigma^2.
+ * deg(v) = number of in-volume axial neighbours of v (the conv of ones with _adj_filt, SAME zero padding):
+ *   loss[0] = 0.5 nd (mean_{B,V,nd}(lambda deg e^l - l) + lambda 0.5 / nd sum_axes mean (mu_{x + e_axis} - mu_x)^2),
+ * each mean over that axis's own difference tensor; an axis of size 1 contributes nothing.  Deterministic reduction
+ * through the reduce workspace.  The backward writes the (B, 2 nd, D, H, W) gradient (pointwise in l, the 2 nd-point
+ * Laplacian of mu). */
+int vxm_kl_fwd(const float* params, float* loss, void* work, int B, int D, int H, int W, int nd, float prior_lambda,
+               void* stream);
+int vxm_kl_bwd(const float* params, const float* grad_loss, float* grad_params, int B, int D, int H, int W, int nd,
+               float prior_lambda, void* stream);
 
 /* ---- Dice: reference voxelmorph/torch/losses.py:84-90 ----
  * y_true, y_pred: (B,L,V) with V = D*H*W.  `work`: vxm_dice_workspace_bytes(B*L).
@@ -351,6 +369,20 @@ int vxm_mean_stream_fwd(const float* x, float* mean, float* count, float* out, f
  * gradient that is itself broadcast over the batch */
 int vxm_mean_stream_bwd(const float* grad_out, const float* saved, float* grad_x, int B, size_t n, size_t gout_bstride,
                         void* stream);
+
+/* ---- SampleNormalLogVar of probabilistic VoxelMorph (reference voxelmorph/tf/networks.py:155-165) ----
+ * params: flow_params (B, 2 nd, V) fp32 (mu = channels [0, nd), logvar = [nd, 2 nd)); z (B, nd, V) fp32:
+ *   z = mu + exp(logvar / 2) eps,  eps ~ N(0, 1) from Philox4x32-10 keyed by state[0] (the seed): element
+ *   i = (b nd + c) V + v takes word i mod 4 of the block with counter (lo32(i / 4), hi32(i / 4), lo32(call), hi32(call)),
+ *   Box-Muller on the word pairs (0, 1), (2, 3) with u1 = ((w0 >> 8) + 1) 2^-24, u2 = (w1 >> 8) 2^-24:
+ *   eps0 = sqrt(-2 log u1) cos(2 pi u2), eps1 = sqrt(-2 log u1) sin(2 pi u2).
+ * state (2 int64, device) = (seed, call): the forward writes call to ticket (1 int64, device) and commits call + 1 (work:
+ * the reduce workspace, whose ticket counter orders the commit); no host read.  The backward regenerates eps from
+ * (state[0], *ticket): grad_params[mu] = grad_z, grad_params[logvar] = grad_z eps exp(logvar / 2) / 2. */
+int vxm_sample_normal_logvar_fwd(const float* params, float* z, long long* state, long long* ticket, void* work, int B,
+                                 int nd, size_t V, void* stream);
+int vxm_sample_normal_logvar_bwd(const float* grad_z, const float* params, const long long* state, const long long* ticket,
+                                 float* grad_params, int B, int nd, size_t V, void* stream);
 
 #ifdef __cplusplus
 }

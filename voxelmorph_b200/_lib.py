@@ -16,6 +16,7 @@ c_f = ctypes.c_void_p        # device pointers travel as void*
 c_i = ctypes.c_int
 c_sz = ctypes.c_size_t
 c_fl = ctypes.c_float
+c_d = ctypes.c_double
 
 # name -> (restype, argtypes); mirrors include/vxm_b200.h declaration by declaration
 SIGNATURES = {
@@ -43,6 +44,10 @@ SIGNATURES = {
     "vxm_gradloss_bwd": (c_i, [c_f, c_f, c_f] + [c_i] * 7 + [c_fl, c_f]),
     "vxm_mse_fwd": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_f]),
     "vxm_mse_bwd": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_f]),
+    "vxm_mse_scaled_fwd": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_d, c_f]),
+    "vxm_mse_scaled_bwd": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_d, c_f]),
+    "vxm_kl_fwd": (c_i, [c_f, c_f, c_f] + [c_i] * 5 + [c_fl, c_f]),
+    "vxm_kl_bwd": (c_i, [c_f, c_f, c_f] + [c_i] * 5 + [c_fl, c_f]),
     "vxm_dice_workspace_bytes": (c_sz, [c_i]),
     "vxm_dice_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_i, c_sz, c_f]),
     "vxm_dice_bwd": (c_i, [c_f, c_f, c_f, c_f, c_i, c_sz, c_f]),
@@ -97,6 +102,8 @@ SIGNATURES = {
     "vxm_adam_step_dev": (c_i, [c_f, c_f, c_f, c_f, c_sz, c_f] + [c_fl] * 6 + [c_f]),
     "vxm_mean_stream_fwd": (c_i, [c_f] * 6 + [c_i, c_sz, c_fl, c_i, c_f]),
     "vxm_mean_stream_bwd": (c_i, [c_f, c_f, c_f, c_i, c_sz, c_sz, c_f]),
+    "vxm_sample_normal_logvar_fwd": (c_i, [c_f] * 5 + [c_i, c_i, c_sz, c_f]),
+    "vxm_sample_normal_logvar_bwd": (c_i, [c_f] * 5 + [c_i, c_i, c_sz, c_f]),
 }
 
 _lib = None

@@ -2,7 +2,7 @@
 // kernels.  Reductions are deterministic (fixed block partial order, double accumulation).
 //
 // Algorithmic bytes (fp32): Grad 4*C B/voxel fwd (+ 8*C bwd); MSE 8 B/elem fwd (+ 12 bwd);
-// Dice 8 B/elem fwd (+ 8 bwd).
+// Dice 8 B/elem fwd (+ 8 bwd); KL 4 B/elem of flow_params fwd (+ 8 bwd).
 #include "common.cuh"
 
 namespace vxm {
@@ -64,8 +64,76 @@ __global__ void __launch_bounds__(256) gradloss_bwd_kernel(const float* __restri
   }
 }
 
+// KL of probabilistic VoxelMorph (reference voxelmorph/tf/losses.py:247-349) on flow_params (B, 2 nd, D, H, W): channels
+// [0, nd) the mean mu, [nd, 2 nd) l = log sigma^2.  With deg(v) the number of in-volume axial neighbours of v,
+//   loss = 0.5 / (B V) sum (lambda deg e^l - l)  +  sum_axes c_axis sum (mu_{x + e_axis} - mu_x)^2,
+// c_axis = lambda / (4 * count_axis), count_axis = B nd (n_axis - 1) V / n_axis (0 for an axis of size 1).
+struct KlGeom {
+  int B, nd, D, H, W;
+  size_t HW, DHW;
+  float lam;
+  double cz, cy, cx, cs;
+};
+
+__device__ __forceinline__ int kl_degree(int z, int yy, int x, const KlGeom& g) {
+  return (x > 0) + (x + 1 < g.W) + (yy > 0) + (yy + 1 < g.H) + (z > 0) + (z + 1 < g.D);
+}
+
+// one (b, channel) plane per blockIdx.y (mu or l: uniform per block), 32-bit voxel indices within it
+__global__ void __launch_bounds__(256) kl_fwd_kernel(const float* __restrict__ y, float* __restrict__ loss, KlGeom g,
+                                                     ReduceWork rw) {
+  __shared__ double s_red[32];
+  const int V = (int)g.DHW, HW = (int)g.HW;
+  const float* yp = y + (size_t)blockIdx.y * g.DHW;
+  const bool is_mu = (int)(blockIdx.y % (2 * g.nd)) < g.nd;
+  double accz = 0, accy = 0, accx = 0, accs = 0;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < V; p += gridDim.x * blockDim.x) {
+    int z = p / HW;
+    int r = p - z * HW;
+    int yy = r / g.W, x = r - yy * g.W;
+    float v = __ldg(yp + p);
+    if (is_mu) {
+      if (x + 1 < g.W) accx += pen<2>(__ldg(yp + p + 1) - v);
+      if (yy + 1 < g.H) accy += pen<2>(__ldg(yp + p + g.W) - v);
+      if (z + 1 < g.D) accz += pen<2>(__ldg(yp + p + HW) - v);
+    } else {
+      accs += g.lam * (float)kl_degree(z, yy, x, g) * expf(v) - v;
+    }
+  }
+  double tot = block_sum<double>(accz * g.cz + accy * g.cy + accx * g.cx + accs * g.cs, s_red);
+  finish_reduce(tot, rw, gridDim.x * gridDim.y, blockIdx.y * gridDim.x + blockIdx.x, 1.0, loss, s_red);
+}
+
+__global__ void __launch_bounds__(256) kl_bwd_kernel(const float* __restrict__ y, const float* __restrict__ gl,
+                                                     float* __restrict__ gy, KlGeom g) {
+  const int V = (int)g.DHW, HW = (int)g.HW;
+  const float* yp = y + (size_t)blockIdx.y * g.DHW;
+  float* gp = gy + (size_t)blockIdx.y * g.DHW;
+  const bool is_mu = (int)(blockIdx.y % (2 * g.nd)) < g.nd;
+  const float s = __ldg(gl);
+  const float cz = (float)g.cz, cy = (float)g.cy, cx = (float)g.cx, cs = (float)g.cs;
+  for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < V; p += gridDim.x * blockDim.x) {
+    int z = p / HW;
+    int r = p - z * HW;
+    int yy = r / g.W, x = r - yy * g.W;
+    float v = __ldg(yp + p), acc;
+    if (is_mu) {   // the 2 nd-point Laplacian of mu, each axis scaled by its own count
+      acc = 0.f;
+      if (x > 0) acc += cx * dpen<2>(v - __ldg(yp + p - 1));
+      if (x + 1 < g.W) acc -= cx * dpen<2>(__ldg(yp + p + 1) - v);
+      if (yy > 0) acc += cy * dpen<2>(v - __ldg(yp + p - g.W));
+      if (yy + 1 < g.H) acc -= cy * dpen<2>(__ldg(yp + p + g.W) - v);
+      if (z > 0) acc += cz * dpen<2>(v - __ldg(yp + p - HW));
+      if (z + 1 < g.D) acc -= cz * dpen<2>(__ldg(yp + p + HW) - v);
+    } else {
+      acc = cs * (g.lam * (float)kl_degree(z, yy, x, g) * expf(v) - 1.f);
+    }
+    gp[p] = s * acc;
+  }
+}
+
 __global__ void __launch_bounds__(256) mse_fwd_kernel(const float* __restrict__ a, const float* __restrict__ b,
-                                                      float* __restrict__ loss, size_t n, ReduceWork rw) {
+                                                      float* __restrict__ loss, size_t n, double scale, ReduceWork rw) {
   __shared__ double s_red[32];
   double acc = 0;
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -73,12 +141,13 @@ __global__ void __launch_bounds__(256) mse_fwd_kernel(const float* __restrict__ 
     acc += (double)(d * d);
   }
   double tot = block_sum<double>(acc, s_red);
-  finish_reduce(tot, rw, gridDim.x, blockIdx.x, 1.0 / (double)n, loss, s_red);
+  finish_reduce(tot, rw, gridDim.x, blockIdx.x, scale / (double)n, loss, s_red);
 }
 
 __global__ void __launch_bounds__(256) mse_bwd_kernel(const float* __restrict__ yt, const float* __restrict__ yp,
-                                                      const float* __restrict__ gl, float* __restrict__ gp, size_t n) {
-  float s = __ldg(gl) * (float)(2.0 / (double)n);
+                                                      const float* __restrict__ gl, float* __restrict__ gp, size_t n,
+                                                      double scale) {
+  float s = __ldg(gl) * (float)(2.0 * scale / (double)n);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     gp[i] = s * (__ldg(yp + i) - __ldg(yt + i));
 }
@@ -161,6 +230,33 @@ static int make_grad_geom(int B, int C, int D, int H, int W, int nd, float mult,
   return VXM_OK;
 }
 
+static int make_kl_geom(int B, int D, int H, int W, int nd, float lam, KlGeom* g) {
+  VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0, "kl: non-positive dimension");
+  VXM_REQUIRE(nd == 2 || nd == 3, "kl: nd must be 2 or 3");
+  VXM_REQUIRE(nd == 3 || D == 1, "kl: a 2-D problem must be passed with D == 1");
+  VXM_REQUIRE((size_t)D * H * W < (1u << 31), "kl: at most 2^31 - 1 voxels per volume");
+  VXM_REQUIRE(2 * nd * B <= kMaxReduceBlocks, "kl: at most %d (batch, channel) planes, got %d", kMaxReduceBlocks, 2 * nd * B);
+  g->B = B; g->nd = nd; g->D = D; g->H = H; g->W = W; g->lam = lam;
+  g->HW = (size_t)H * W; g->DHW = g->HW * D;
+  double V = (double)g->DHW;
+  auto coef = [&](int s) { return s > 1 ? (double)lam / (4.0 * B * nd * (s - 1) * (V / s)) : 0.0; };
+  g->cx = coef(W);
+  g->cy = coef(H);
+  g->cz = nd == 3 ? coef(D) : 0.0;
+  g->cs = 0.5 / ((double)B * V);
+  return VXM_OK;
+}
+
+// blocks per plane: about 8 blocks per SM over all planes (fwd: at most kMaxReduceBlocks partials in all)
+static dim3 kl_grid(const KlGeom& g) {
+  int planes = 2 * g.nd * g.B;
+  size_t want = (g.DHW + 256 * 8 - 1) / (256 * 8);
+  int cap = sm_count() * 8 / planes;
+  if (cap > kMaxReduceBlocks / planes) cap = kMaxReduceBlocks / planes;
+  if (cap < 1) cap = 1;
+  return dim3((unsigned)(want < 1 ? 1 : (want > (size_t)cap ? cap : want)), (unsigned)planes);
+}
+
 }  // namespace vxm
 
 using namespace vxm;
@@ -194,15 +290,49 @@ extern "C" int vxm_gradloss_bwd(const float* y, const float* grad_loss, float* g
 
 extern "C" int vxm_mse_fwd(const float* y_true, const float* y_pred, float* loss, void* work, size_t n, void* stream) {
   VXM_REQUIRE(y_true && y_pred && loss && work && n > 0, "mse_fwd: bad argument");
-  mse_fwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, loss, n, as_reduce_work(work));
+  mse_fwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, loss, n, 1.0, as_reduce_work(work));
   return check_launch("mse_fwd");
 }
 
 extern "C" int vxm_mse_bwd(const float* y_true, const float* y_pred, const float* grad_loss, float* grad_pred,
                            size_t n, void* stream) {
   VXM_REQUIRE(y_true && y_pred && grad_loss && grad_pred && n > 0, "mse_bwd: bad argument");
-  mse_bwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, grad_loss, grad_pred, n);
+  mse_bwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, grad_loss, grad_pred, n, 1.0);
   return check_launch("mse_bwd");
+}
+
+extern "C" int vxm_mse_scaled_fwd(const float* y_true, const float* y_pred, float* loss, void* work, size_t n, double scale,
+                                  void* stream) {
+  VXM_REQUIRE(y_true && y_pred && loss && work && n > 0, "mse_scaled_fwd: bad argument");
+  mse_fwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, loss, n, scale, as_reduce_work(work));
+  return check_launch("mse_scaled_fwd");
+}
+
+extern "C" int vxm_mse_scaled_bwd(const float* y_true, const float* y_pred, const float* grad_loss, float* grad_pred,
+                                  size_t n, double scale, void* stream) {
+  VXM_REQUIRE(y_true && y_pred && grad_loss && grad_pred && n > 0, "mse_scaled_bwd: bad argument");
+  mse_bwd_kernel<<<reduce_grid(n), 256, 0, as_stream(stream)>>>(y_true, y_pred, grad_loss, grad_pred, n, scale);
+  return check_launch("mse_scaled_bwd");
+}
+
+extern "C" int vxm_kl_fwd(const float* params, float* loss, void* work, int B, int D, int H, int W, int nd,
+                          float prior_lambda, void* stream) {
+  KlGeom g;
+  int rc = make_kl_geom(B, D, H, W, nd, prior_lambda, &g);
+  if (rc) return rc;
+  VXM_REQUIRE(params && loss && work, "kl_fwd: null pointer");
+  kl_fwd_kernel<<<kl_grid(g), 256, 0, as_stream(stream)>>>(params, loss, g, as_reduce_work(work));
+  return check_launch("kl_fwd");
+}
+
+extern "C" int vxm_kl_bwd(const float* params, const float* grad_loss, float* grad_params, int B, int D, int H, int W,
+                          int nd, float prior_lambda, void* stream) {
+  KlGeom g;
+  int rc = make_kl_geom(B, D, H, W, nd, prior_lambda, &g);
+  if (rc) return rc;
+  VXM_REQUIRE(params && grad_loss && grad_params, "kl_bwd: null pointer");
+  kl_bwd_kernel<<<kl_grid(g), 256, 0, as_stream(stream)>>>(params, grad_loss, grad_params, g);
+  return check_launch("kl_bwd");
 }
 
 extern "C" size_t vxm_dice_workspace_bytes(int BL) { return (size_t)BL * DICE_CHUNKS * 2 * sizeof(double); }

@@ -26,9 +26,11 @@ class _Layer:
     forward and of the dgrad (see _run); `fwd_x3`: the block grid of the split-precision forward; `dgrad_skip`: with a
     polyphase dgrad, the form of the skip part (the dgrad's own form then yields the upsampled part only); `dgrad_img`
     (first convolution only): the form of the dgrad into the image planes, which runs only when an image asks for its
-    gradient (_Plan.image_dgrad_packs)."""
+    gradient (_Plan.image_dgrad_packs).  `srcs`: the parameters the layer's operands are derived from — its own weight, or
+    for the head of a probabilistic model the weights and biases of `flow` and `log_sigma`, which the plan concatenates
+    into the persistent `w` / `bias` of one 2 nd-output convolution."""
     __slots__ = ("w", "bias", "slope", "role", "a", "b", "out", "up", "ca", "cb", "cin", "cout", "fwd", "fwd_x3", "dgrad", "khm",
-                 "dgrad_skip", "dgrad_img", "pk_fwd", "pk_dgrad", "pk_dgrad_skip", "pk_hi", "pk_lo", "w_hi", "w_lo")
+                 "dgrad_skip", "dgrad_img", "pk_fwd", "pk_dgrad", "pk_dgrad_skip", "pk_hi", "pk_lo", "w_hi", "w_lo", "srcs")
 
 
 def _refuse(what):
@@ -49,7 +51,9 @@ def _form(ca, cb, nout, kd, kw, split=None):
 
 def _walk(model):
     """The U-Net and flow head of `model` (a VxmDense) in execution order: _Layer and ("pool", in_id, out_id) entries with
-    shapes and execution forms only (allocates nothing).  Refuses a model some convolution of which no engine path runs."""
+    shapes and execution forms only (allocates nothing).  Refuses a model some convolution of which no engine path runs.
+    A model with a `log_sigma` module (VxmDenseProbabilistic) has a head of 2 nd outputs: `flow` then `log_sigma`, one
+    forward, one dgrad and one weight gradient."""
     unet = model.unet_model
     w0 = unet.encoder[0][0].main.weight
     if w0.dim() not in (4, 5):
@@ -61,15 +65,16 @@ def _walk(model):
     chans = [8]           # channels of every tensor id: the images enter as one bf16 channels-last tensor of 8 channels
     cur, pending_up, skips = 0, None, [None]
 
-    def conv(m, slope, role="inner"):
+    def conv(m, slope, role="inner", extra=None):
         nonlocal cur, pending_up
         L = _Layer()
         L.w, L.bias, L.slope, L.role = m.weight, m.bias, slope, role
+        L.srcs = (m.weight,) if extra is None else (m.weight, m.bias, extra.weight, extra.bias)
         # a convolution after an upsample reads the upsampled previous output, then the skip (a fused upsample + concat)
         L.a, L.b = pending_up if pending_up is not None else (cur, None)
         L.up, pending_up = pending_up is not None, None
         L.ca, L.cb = chans[L.a], (0 if L.b is None else chans[L.b])
-        L.cout, L.cin = m.weight.shape[0], m.weight.shape[1]
+        L.cout, L.cin = m.weight.shape[0] + (0 if extra is None else extra.weight.shape[0]), m.weight.shape[1]
         if m.weight.dim() != w0.dim():
             _refuse("convolutions of different dimensionality")
         if role == "first":
@@ -131,7 +136,7 @@ def _walk(model):
             pending_up = (cur, skips.pop())
     for blk in unet.remaining:
         conv(blk.main, blk.activation.negative_slope)
-    conv(model.flow, None, "flow")        # no activation, fp32 planar output
+    conv(model.flow, None, "flow", getattr(model, "log_sigma", None))        # no activation, fp32 planar output
     return ops
 
 
@@ -157,6 +162,10 @@ class _Plan:
         self.ops = _walk(model)
         self.layers = [L for L in self.ops if isinstance(L, _Layer)]
         self.nd = self.layers[0].w.dim() - 2
+        for L in self.layers:
+            if len(L.srcs) > 1:           # the 2 nd-output head: persistent operands, refilled by refresh
+                L.w = torch.empty((L.cout,) + tuple(L.w.shape[1:]), dtype=torch.float32, device=L.w.device)
+                L.bias = torch.empty(L.cout, dtype=torch.float32, device=L.w.device)
         self.slope = {L.out: float(L.slope) for L in self.layers if L.slope is not None}     # convolution output id -> slope
         bf16, x3 = [], []
         for L in self.layers:
@@ -176,11 +185,16 @@ class _Plan:
         self.img_table, self.img_stamp = None, None
 
     def weight_ptrs(self):
-        return tuple(L.w.data_ptr() for L in self.layers)
+        return tuple(p.data_ptr() for L in self.layers for p in L.srcs)
 
     def refresh(self, split):
-        stamp = (_weights_epoch, tuple(L.w._version for L in self.layers))
+        stamp = (_weights_epoch, tuple(p._version for L in self.layers for p in L.srcs))
         if stamp != self.stamps[0]:
+            for L in self.layers:
+                if len(L.srcs) > 1:       # device copies: graph-capturable like the pack launch
+                    fw, fb, lw, lb = L.srcs
+                    torch.cat([fw.detach(), lw.detach()], out=L.w)
+                    torch.cat([fb.detach(), lb.detach()], out=L.bias)
             self.bf16.refresh()
             self.stamps[0] = stamp
         if split and stamp != self.stamps[1]:
@@ -342,6 +356,7 @@ def backward_tape(ctx, g_flow, image_grad=False):
     gskip = {}    # encoder-output id -> raw skip gradient
     grads = {}
     folded = []   # (layer, gw2d, gb2d): 2-D weight gradients of the kd-folded layers, mapped back after the flush
+    heads = []    # (layer, gw, gb): weight gradient of a 2 nd-output head, split between its modules after the flush
     for L in reversed(plan.ops):
         if not isinstance(L, _Layer):
             _, src, dst = L
@@ -370,6 +385,8 @@ def backward_tape(ctx, g_flow, image_grad=False):
             else:
                 batch.add(xa, None, g_in, gwf, gbf, 3 * L.cin, L.cout, 1, False, False)
             folded.append((L, gwf, gbf))
+        elif len(L.srcs) > 1:
+            heads.append((L,) + tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, batch=batch))
         elif _flat_grads(L):
             tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, out_w=L.w.grad, out_b=None if L.bias is None else L.bias.grad,
                           batch=batch)
@@ -411,6 +428,15 @@ def backward_tape(ctx, g_flow, image_grad=False):
             grads[L.w] = gw.contiguous()
             if L.bias is not None:
                 grads[L.bias] = gb.contiguous()
+    for L, gw, gb in heads:
+        fw, fb, lw, lb = L.srcs
+        k = fw.shape[0]
+        gw = gw.squeeze(2) if nd == 2 else gw
+        for p, g in ((fw, gw[:k]), (fb, gb[:k]), (lw, gw[k:]), (lb, gb[k:])):
+            if getattr(p, "_vxm_flat_grad", False) and p.grad is not None and p.grad.is_contiguous():
+                p.grad.add_(g)
+            else:
+                grads[p] = g.contiguous()
     return grads
 
 
@@ -486,8 +512,10 @@ class _UnetFlowFn(torch.autograd.Function):
 
 
 def unet_flow(model, source, target, split=False):
-    """flow = model.flow(model.unet_model(cat(source, target))) on the tensor-core engine.  split=False: bf16 operands
+    """flow = model.flow(model.unet_model(cat(source, target))) on the tensor-core engine (for a model with `log_sigma`:
+    cat(flow(x), log_sigma(x)), the probabilistic model's flow_params).  split=False: bf16 operands
     (throughput mode); split=True: bf16x3 split precision in the forward (flow within 1e-4 of the fp32 reference), the
     backward uses bf16 operands in both modes."""
-    params = [p for p in list(model.unet_model.parameters()) + list(model.flow.parameters())]
+    head = [model.flow] + ([model.log_sigma] if hasattr(model, "log_sigma") else [])
+    params = list(model.unet_model.parameters()) + [p for m in head for p in m.parameters()]
     return _UnetFlowFn.apply(model, source, target, bool(split), *params)

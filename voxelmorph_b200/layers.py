@@ -274,3 +274,44 @@ class MeanStream(nn.Module):
 
     def forward(self, x):
         return _MeanStreamFn.apply(x, self.mean, self.count, self.cap, self.training)
+
+
+class _SampleNormalLogVarFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, params, state):
+        _lib.require_cuda(params, what="SampleNormalLogVar")
+        params = _lib.contig(params)
+        B, C, D, H, W, nd = _dims(params)
+        if C != 2 * nd:
+            raise _lib.VxmError("SampleNormalLogVar: expected 2 * %d channels (mean, log variance), got %d" % (nd, C))
+        if not state.is_cuda or state.dtype != torch.int64 or state.numel() != 2 or not state.is_contiguous():
+            raise _lib.VxmError("SampleNormalLogVar: the noise state must be a contiguous (seed, call) int64 CUDA tensor")
+        z = torch.empty((B, nd) + tuple(params.shape[2:]), dtype=torch.float32, device=params.device)
+        ticket = torch.empty(1, dtype=torch.int64, device=params.device)
+        _lib.check(_lib.load().vxm_sample_normal_logvar_fwd(_lib.ptr(params), _lib.ptr(z), _lib.ptr(state), _lib.ptr(ticket),
+                                                            _lib.ptr(_lib.reduce_workspace(params.device)), B, nd, D * H * W,
+                                                            _lib.stream_ptr()), "vxm_sample_normal_logvar_fwd")
+        ctx.save_for_backward(params)
+        ctx.state, ctx.ticket = state, ticket
+        return z
+
+    @staticmethod
+    def backward(ctx, gz):
+        (params,) = ctx.saved_tensors
+        B, C, D, H, W, nd = _dims(params)
+        gz = _lib.contig(gz)
+        gp = torch.empty_like(params)
+        _lib.check(_lib.load().vxm_sample_normal_logvar_bwd(_lib.ptr(gz), _lib.ptr(params), _lib.ptr(ctx.state), _lib.ptr(ctx.ticket),
+                                                            _lib.ptr(gp), B, nd, D * H * W, _lib.stream_ptr()),
+                   "vxm_sample_normal_logvar_bwd")
+        return gp, None
+
+
+def sample_normal_logvar(params, state):
+    """z = mu + exp(logvar / 2) eps with eps ~ N(0, 1) (neurite's SampleNormalLogVar, which the reference's probabilistic
+    VxmDense draws its field with, voxelmorph/tf/networks.py:155-165), for params (B, 2 nd, *vol) = cat(mu, logvar).
+
+    eps comes from a counter-based generator (Philox4x32-10, include/vxm_b200.h) keyed by state = (seed, call), an int64
+    device tensor: each call draws the stream of the current `call` and advances it by one on the device, and its backward
+    regenerates that same eps instead of storing it."""
+    return _SampleNormalLogVarFn.apply(params, state)

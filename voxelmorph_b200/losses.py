@@ -1,5 +1,6 @@
 """NCC / MSE / Dice / Grad losses with the reference's surface
-(reference voxelmorph/torch/losses.py): plain classes whose bound `.loss(y_true, y_pred)`
+(reference voxelmorph/torch/losses.py), and the KL loss and sigma-weighted MSE of the probabilistic
+model (reference voxelmorph/tf/losses.py): plain classes whose bound `.loss(y_true, y_pred)`
 returns a 0-d tensor supporting `.item()`, `*`, `+`, `.backward()`.
 Each loss is one fused sm_90a kernel (plus a fused backward) from libvxm_b200.so.
 """
@@ -77,16 +78,22 @@ class NCC:
 
 class _MseFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, y_true, y_pred):
+    def forward(ctx, y_true, y_pred, scale):
         _lib.require_cuda(y_true, y_pred, what="MSE")
         if tuple(y_true.shape) != tuple(y_pred.shape):
             y_true, y_pred = torch.broadcast_tensors(y_true, y_pred)
         a, b = _lib.contig(y_true), _lib.contig(y_pred)
         lib = _lib.load()
         loss = _scalar(a.device)
-        _lib.check(lib.vxm_mse_fwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(loss), _lib.ptr(_lib.reduce_workspace(a.device)),
-                                   a.numel(), _lib.stream_ptr()), "vxm_mse_fwd")
+        ws = _lib.reduce_workspace(a.device)
+        if scale == 1.0:
+            _lib.check(lib.vxm_mse_fwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(loss), _lib.ptr(ws), a.numel(), _lib.stream_ptr()),
+                       "vxm_mse_fwd")
+        else:
+            _lib.check(lib.vxm_mse_scaled_fwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(loss), _lib.ptr(ws), a.numel(), scale,
+                                              _lib.stream_ptr()), "vxm_mse_scaled_fwd")
         ctx.save_for_backward(a, b)
+        ctx.scale = scale
         return loss
 
     @staticmethod
@@ -95,17 +102,26 @@ class _MseFn(torch.autograd.Function):
         gl = gl.contiguous().float()
         gp = torch.empty_like(b)
         lib = _lib.load()
-        _lib.check(lib.vxm_mse_bwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(gl), _lib.ptr(gp), a.numel(), _lib.stream_ptr()),
-                   "vxm_mse_bwd")
+        if ctx.scale == 1.0:
+            _lib.check(lib.vxm_mse_bwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(gl), _lib.ptr(gp), a.numel(), _lib.stream_ptr()),
+                       "vxm_mse_bwd")
+        else:
+            _lib.check(lib.vxm_mse_scaled_bwd(_lib.ptr(a), _lib.ptr(b), _lib.ptr(gl), _lib.ptr(gp), a.numel(), ctx.scale,
+                                              _lib.stream_ptr()), "vxm_mse_scaled_bwd")
         gt = -gp if ctx.needs_input_grad[0] else None
-        return gt, gp
+        return gt, gp, None
 
 
 class MSE:
-    """Mean squared error loss (reference losses.py:70-76)."""
+    """Mean squared error loss (reference losses.py:70-76); with `image_sigma`, the sigma-weighted form of the reference's
+    TensorFlow side, 1 / image_sigma^2 * mean((y_true - y_pred)^2) (voxelmorph/tf/losses.py:112-134), which
+    train.py --use-probs sets through --legacy-image-sigma."""
+
+    def __init__(self, image_sigma=1.0):
+        self.image_sigma = image_sigma
 
     def loss(self, y_true, y_pred):
-        return _MseFn.apply(y_true, y_pred)
+        return _MseFn.apply(y_true, y_pred, 1.0 / float(self.image_sigma) ** 2)
 
 
 class _DiceFn(torch.autograd.Function):
@@ -195,3 +211,50 @@ class Grad:
             p = 2
         mult = 1.0 if self.loss_mult is None else float(self.loss_mult)
         return _GradFn.apply(y_pred, p, mult)
+
+
+class _KlFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, params, prior_lambda):
+        _lib.require_cuda(params, what="KL")
+        params = _lib.contig(params)
+        B, C, D, H, W, nd = _dims(params)
+        if C != 2 * nd:
+            raise _lib.VxmError("KL: expected flow_params with 2 * %d channels (mean, log sigma), got %d" % (nd, C))
+        loss = _scalar(params.device)
+        _lib.check(_lib.load().vxm_kl_fwd(_lib.ptr(params), _lib.ptr(loss), _lib.ptr(_lib.reduce_workspace(params.device)),
+                                          B, D, H, W, nd, prior_lambda, _lib.stream_ptr()), "vxm_kl_fwd")
+        ctx.save_for_backward(params)
+        ctx.cfg = (B, D, H, W, nd, prior_lambda)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        (params,) = ctx.saved_tensors
+        B, D, H, W, nd, prior_lambda = ctx.cfg
+        gl = gl.contiguous().float()
+        gp = torch.empty_like(params)
+        _lib.check(_lib.load().vxm_kl_bwd(_lib.ptr(params), _lib.ptr(gl), _lib.ptr(gp), B, D, H, W, nd, prior_lambda,
+                                          _lib.stream_ptr()), "vxm_kl_bwd")
+        return gp, None
+
+
+class KL:
+    """Kullback-Leibler divergence of probabilistic flows (reference voxelmorph/tf/losses.py:247-349), on the NCDHW
+    `flow_params` of networks.VxmDenseProbabilistic: channels [0, nd) the mean mu, [nd, 2 nd) l = log sigma^2.
+
+        loss = 0.5 nd (mean_{B,V,nd}(prior_lambda D e^l - l) + prior_lambda 0.5 / nd sum_i mean((mu_{x+e_i} - mu_x)^2))
+
+    with D the number of in-volume axial neighbours of each voxel (the reference's degree matrix) and each mean over axis
+    i's own difference tensor; an axis of size 1 has no differences and contributes nothing (the reference's mean of an
+    empty tensor would be NaN).  `y_true` is ignored; `flow_vol_shape`, if given, must be y_pred's spatial shape."""
+
+    def __init__(self, prior_lambda, flow_vol_shape=None):
+        self.prior_lambda = prior_lambda
+        self.flow_vol_shape = flow_vol_shape
+
+    def loss(self, y_true, y_pred):
+        if self.flow_vol_shape is not None and tuple(int(s) for s in self.flow_vol_shape) != tuple(y_pred.shape[2:]):
+            raise _lib.VxmError("KL: flow_vol_shape %s does not match flow_params of spatial shape %s"
+                                % (tuple(self.flow_vol_shape), tuple(y_pred.shape[2:])))
+        return _KlFn.apply(y_pred, float(self.prior_lambda))

@@ -210,16 +210,23 @@ class VxmDense(LoadableModel):
         """(pos_flow, neg_flow, preint_flow): the U-Net's field brought to the integration resolution (`preint_flow`,
         what train.py regularises), integrated and brought back to full resolution (`pos_flow`, what warps the moving
         image; `neg_flow` its inverse when bidir).  reference networks.py:253-276."""
+        return self._integrate(self._head(source, target))
+
+    def _head(self, source, target):
+        """The U-Net and its head: the field `flow` predicts (a VxmDenseProbabilistic: cat(flow, log_sigma))."""
         engine = ops.resolve_engine(self)
         if engine in ('bf16', 'bf16x3'):
             # tensor-core engine: Unet + flow head as one hand-written forward/backward (engine_bf16.py)
             from . import engine_bf16
-            flow_field = engine_bf16.unet_flow(self, source, target, split=(engine == 'bf16x3'))
-        else:
-            x = ops.upsample_free_cat(source, target)
-            x = self.unet_model(x)
-            flow_field = self.flow(x)
+            return engine_bf16.unet_flow(self, source, target, split=(engine == 'bf16x3'))
+        x = ops.upsample_free_cat(source, target)
+        x = self.unet_model(x)
+        if hasattr(self, 'log_sigma'):
+            return torch.cat([self.flow(x), self.log_sigma(x)], dim=1)
+        return self.flow(x)
 
+    def _integrate(self, flow_field):
+        """(pos_flow, neg_flow, preint_flow) of a field at the U-Net's resolution (see flows)."""
         pos_flow = flow_field
         if self.resize:
             pos_flow = self.resize(pos_flow)
@@ -247,6 +254,83 @@ class VxmDense(LoadableModel):
 
         if not registration:
             return (y_source, y_target, preint_flow) if self.bidir else (y_source, preint_flow)
+        return y_source, pos_flow
+
+
+def rank_seed(seed, rank):
+    """The noise seed of data-parallel rank `rank` for a model constructed with `seed`: rank 0 keeps it, every other rank
+    gets a splitmix64 mix of (seed, rank), so that replicas built from one torch seed draw independent noise."""
+    if rank == 0:
+        return int(seed)
+    m = (1 << 64) - 1
+    z = (int(seed) + (int(rank) * 0x9E3779B97F4A7C15)) & m
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & m
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & m
+    return (z ^ (z >> 31)) & ((1 << 63) - 1)
+
+
+class VxmDenseProbabilistic(VxmDense):
+    """Probabilistic diffeomorphic VoxelMorph (Dalca et al., MICCAI 2018 / MedIA 2019): VxmDense with a second head,
+    `log_sigma`, next to `flow`, as the reference's TensorFlow VxmDense builds it with use_probs=True
+    (voxelmorph/tf/networks.py:155-165, 230-232).  The reference's torch VxmDense refuses use_probs, and so does this
+    package's; this class takes VxmDense's constructor arguments bar use_probs.
+
+    `log_sigma` = Conv(final_nf, nd, 3, padding=1), weight ~ N(0, 1e-10), bias -10.  flow_params = cat(mu, l) (B, 2 nd,
+    *vol) with mu = flow(x) and l = log_sigma(x) = log sigma^2 (at half resolution with unet_half_res, as in TF).
+
+    Training form (registration=False): z = mu + exp(l / 2) eps, eps ~ N(0, 1) — the formula of neurite's
+    SampleNormalLogVar, which agrees with the KL loss reading exp(log_sigma) as the variance (voxelmorph/tf/losses.py:340)
+    — goes through resize, VecInt, resize and the warp exactly as VxmDense's field does; returns (y_source, flow_params),
+    or (y_source, y_target, flow_params) when bidir (neg_flow = -z, the same draw).  Attach losses.KL to flow_params.
+
+    Registration form (registration=True): the mean mu is integrated and nothing is sampled, the papers' use of the model
+    at test time.  This departs deliberately from the TF graph, whose sampling layer has no training switch.
+
+    Noise: eps is drawn on the device (layers.sample_normal_logvar) from the non-persistent int64 buffer
+    `noise_state` = (seed, call); `seed` is drawn from torch's default CPU generator at construction (torch.manual_seed
+    makes runs reproducible; under data parallelism each rank mixes its rank in, see rank_seed), and every training
+    forward advances `call` on the device, so CUDA-graph replays draw fresh noise.  The buffer stays out of checkpoints:
+    the state-dict keys are VxmDense's plus log_sigma.weight and log_sigma.bias."""
+
+    @store_config_args
+    def __init__(self, inshape, nb_unet_features=None, nb_unet_levels=None, unet_feat_mult=1,
+                 nb_unet_conv_per_level=1, int_steps=7, int_downsize=2, bidir=False,
+                 src_feats=1, trg_feats=1, unet_half_res=False):
+        config = self.config
+        super().__init__(inshape, nb_unet_features, nb_unet_levels, unet_feat_mult, nb_unet_conv_per_level, int_steps,
+                         int_downsize, bidir, False, src_feats, trg_feats, unet_half_res)
+        self.config = config             # (VxmDense's decorator recorded its own arguments)
+        ndims = len(inshape)
+        self.log_sigma = _conv_cls(ndims)(self.unet_model.final_nf, ndims, kernel_size=3, padding=1)
+        self.log_sigma.weight = nn.Parameter(Normal(0, 1e-10).sample(self.log_sigma.weight.shape))
+        self.log_sigma.bias = nn.Parameter(torch.full(self.log_sigma.bias.shape, -10.0))
+        seed = int(torch.randint(0, 2 ** 63 - 1, (1,), dtype=torch.int64))
+        self.register_buffer("noise_state", torch.tensor([seed, 0], dtype=torch.int64), persistent=False)
+
+    def _maybe_attach_dp(self):
+        first = not self._dp_checked
+        dp = super()._maybe_attach_dp()
+        if first and dp is not None:
+            with torch.no_grad():
+                self.noise_state[0] = rank_seed(int(self.noise_state[0]), dp.rank)
+        return dp
+
+    def forward(self, source, target, registration=False):
+        self._maybe_attach_dp()
+        if registration and not self.training and self.registration_no_grad and torch.is_grad_enabled():
+            with torch.no_grad():
+                return self.forward(source, target, registration=True)
+        flow_params = self._head(source, target)
+        nd = flow_params.shape[1] // 2
+        if registration:
+            field = flow_params[:, :nd]
+        else:
+            field = layers.sample_normal_logvar(flow_params, self.noise_state)
+        pos_flow, neg_flow, _ = self._integrate(field)
+        y_source = self.transformer(source, pos_flow)
+        y_target = self.transformer(target, neg_flow) if self.bidir else None
+        if not registration:
+            return (y_source, y_target, flow_params) if self.bidir else (y_source, flow_params)
         return y_source, pos_flow
 
 
