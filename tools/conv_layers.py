@@ -13,8 +13,8 @@ V = FULL[0] * FULL[1] * FULL[2]
 FLOPS = {}          # layer name -> useful FLOPs of the launch (none for the layout kernels)
 
 
-def flops(name, cin, cout):
-    FLOPS[name] = 2 * 27 * cin * cout * V
+def flops(name, cin, cout, v=V):
+    FLOPS[name] = 2 * 27 * cin * cout * v
 
 
 def timeit(fn, n=7):
@@ -85,6 +85,11 @@ def build():
         cin = 2 if cx == 8 else cx
         L[name] = (lambda xx=xx, g=g, cin=cin, cout=cout, up=up: tc.conv_wgrad(xx, None, g, cin, cout, 3, up=up))
         flops(name, cin, cout)
+    # dec3's upsampled source at half resolution (the rates of the upsampled wgrads count the fine form's FLOPs; the
+    # coarse form, VXM_B200_POLYPHASE=1, does a third of them)
+    xx, g = rnd(tuple(s // 2 for s in HALF), 32), rnd(HALF, 32)
+    L["dec3_wgrad_a x32^ g32 (half res)"] = lambda: tc.conv_wgrad(xx, None, g, 32, 32, 3, up=True)
+    flops("dec3_wgrad_a x32^ g32 (half res)", 32, 32, V // 8)
     # kd-folded variants of the two layers with 2 / 3 real channels on one side
     planes2 = [torch.rand((1, 1) + FULL, device=dev) for _ in range(2)]
     planes3 = [torch.randn((1, 1) + FULL, device=dev) for _ in range(3)]

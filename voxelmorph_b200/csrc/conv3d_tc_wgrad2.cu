@@ -301,6 +301,285 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
   }
 }
 
+// ---- weight gradient of a nearest-x2 upsampled 32-channel source, on the coarse voxels ---------------------------------
+// With u = up(x) and tap offset t in {-1, 0, +1} per axis,
+//     gw[t][ci][co] = sum_v u[v + t][ci] gz[v][co] = sum_c x[c + s(t)][ci] G_a(t)[c][co],
+// where per axis t = 0 -> (E, s = 0), t = +1 -> (O, s = 0), t = -1 -> (O, s = -1), E[c] = g[2c] + g[2c+1] and
+// O[c] = g[2c-1] + g[2c] (c = 0 .. Dc; fine voxels outside the volume are zero, as is x[-1] and x[Dc]).  So 8 coarse
+// pair-summed gradients G_{ad ah aw} (a = O or E per axis) replace the fine gz: a quarter of the fine form's K.
+// The loader warpgroup streams the fine gz slices through a 3-slice shared-memory ring (cp.async; slice 2s+1 serves
+// coarse slices s and s+1), forms G from it (fp32 sums), splits each value into bf16 hi + lo (G = hi + lo to ~2^-17
+// relative, so the result differs from the fine form by fp32 re-association only) and writes 16 swizzled slabs per
+// coarse slice; the x slabs are coarse, staged as in wgrad2_kernel.  MMA warpgroup k owns the depth tap kd = k
+// ((O, -1), (E, 0), (O, 0)) and three accumulators, one per kh ((O, -1), (E, 0), (O, 0): the A window one tile row
+// lower for s = 0).  Each is m64n64: M = (sw, ci) is a Toeplitz view of the x slab (two M atoms one row apart: x[w-1],
+// x[w]), N = (aw, co) the O and E slabs; (sw = -1, E) is padding, so 3/4 of the MMA work is useful.  hi and lo are two
+// MMAs into the same accumulator.  Per coarse voxel: 2 x 36864 MACs instead of the fine form's 8 x 27648 (1/3).
+constexpr int PTH = 2, PTU = 31;                                 // coarse tile: 2 rows x 31 columns (+1 zero column)
+constexpr int PXROWS = (PTH + 1) * TWR, PXR = PXROWS + 8;        // x slab: rows h0-1 .. h0+PTH-1, + 8 zero rows
+// G slab: rows h0 .. h0+PTH-1.  The MMAs read one row past a slab: row 0 of the next slab (or of the zero tail after
+// the last), which is always zero (column w0 - 1 belongs to the previous tile).
+constexpr int PGROWS = PTH * TWR;
+constexpr uint32_t PXSLAB = PXR * 64, PGSLAB = PGROWS * 64, PGSTAGE = 16 * PGSLAB;
+// fine gz slice of a tile: rows 2h0-1 .. 2(h0+PTH)-1, columns 2w0-3 .. 2(w0+PTU)-1, 32 channels (16-byte chunks, unswizzled)
+constexpr int PFROWS = 2 * PTH + 1, PFCOLS = 2 * TWR + 1, PFCHUNKS = PFROWS * PFCOLS * 4;
+constexpr uint32_t PFSLICE = PFCHUNKS * 16;
+constexpr int PNGS = 2, PNSLOT = 4, PMAXSLOT = 8, PNTHREADS = 512;   // warps 0-11: MMA warpgroups (kd = 0, 1, 2), 12-15: loader
+constexpr size_t PSMEM = (size_t)PNGS * PGSTAGE + 512 + (size_t)PNSLOT * PXSLAB + 3 * PFSLICE + 512 + 128 * 8 * sizeof(float);
+
+struct Wgrad2PolyArgs {
+  const __nv_bfloat16* x; int xpitch;        // coarse (B, Dc, Hc, Wc, xpitch), channels [0, 32) used
+  const __nv_bfloat16* gz; int Cg, gpitch;   // fine (B, D, H, W, gpitch), channels [0, Cg) used, Cg <= 32
+  float* partial;                            // [grid][27][32][32]
+  float* bias_partial;                       // [grid][32] or null
+  int B, D, H, W, Dc, Hc, Wc;
+  int tiles_h, tiles_w, dchunk, nchunks, nitems, nslot;
+};
+
+// G slab of (hi/lo, ad, ah, aw), index 0 = O, 1 = E per axis
+__host__ __device__ constexpr int poly_slab(int hl, int ad, int ah, int aw) { return ((hl * 2 + ad) * 2 + ah) * 2 + aw; }
+
+__global__ void __launch_bounds__(PNTHREADS, 1) wgrad2_poly_kernel(const Wgrad2PolyArgs a) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const int NS = a.nslot;
+  uint8_t* s_g = smem;
+  uint8_t* s_x = s_g + PNGS * PGSTAGE + 512;                  // after the G stages' zero tail
+  uint8_t* s_f = s_x + (size_t)NS * PXSLAB;                   // fine gz ring: slice f in slot f mod 3
+  uint64_t* bars = reinterpret_cast<uint64_t*>(s_f + 3 * PFSLICE);
+  uint64_t* xfull = bars;
+  uint64_t* xempty = bars + PMAXSLOT;
+  uint64_t* gfull = bars + 2 * PMAXSLOT;
+  uint64_t* gempty = gfull + PNGS;
+  float* s_bsum = reinterpret_cast<float*>(bars) + 128;       // [128 loader threads][8]
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  // zero rows past every slab (never written by the loader) start as zeros
+  for (uint32_t i = threadIdx.x * 16u; i < (uint32_t)(PNGS * PGSTAGE + 512 + NS * PXSLAB); i += PNTHREADS * 16u)
+    *reinterpret_cast<uint4*>(smem + i) = make_uint4(0u, 0u, 0u, 0u);
+  fence_proxy_async();
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < NS; ++i) { mbar_init(&xfull[i], 128); mbar_init(&xempty[i], 12); }
+    for (int i = 0; i < PNGS; ++i) { mbar_init(&gfull[i], 128); mbar_init(&gempty[i], 12); }
+    fence_barrier_init();
+  }
+  __syncthreads();
+  const int HW_tiles = a.tiles_h * a.tiles_w;
+  const bool has_work = blockIdx.x < a.nitems;
+
+  if (warp >= 12) {
+    // ================================ LOADER (128 threads) ================================
+    const int lt = threadIdx.x - 12 * 32;
+    const int c8 = lt & 3;                      // this thread's 8 channels, for every unit it handles
+    uint32_t xslot = 0, xphase = 1, gslot = 0, gphase = 1;
+    float* bsum = s_bsum + lt * 8;              // this thread's bias sums (shared memory: the loader has no registers to spare)
+#pragma unroll
+    for (int e = 0; e < 8; ++e) bsum[e] = 0.f;
+    const bool cok = c8 * 8 < a.Cg;
+    for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
+      const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
+      const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
+      const int h0 = ht * PTH, w0 = wt * PTU, d0 = ch * a.dchunk, d1 = min(d0 + a.dchunk, a.Dc + 1);
+      constexpr int KX = PXROWS * 4 / 128;
+      int soff[KX];
+      uint32_t doff[KX];
+#pragma unroll
+      for (int k = 0; k < KX; ++k) {
+        const int row = (lt + k * 128) >> 2;
+        const int h = h0 - 1 + row / TWR, w = w0 - 1 + row % TWR;
+        doff[k] = swz((uint32_t)row * 64u + (uint32_t)c8 * 16u, 64);
+        soff[k] = (h >= 0 && h < a.Hc && w >= 0 && w < a.Wc) ? (h * a.Wc + w) * a.xpitch + c8 * 8 : -1;
+      }
+      // fine slice f into its ring slot (one cp.async group per call, empty when not needed)
+      auto load_fine = [&](int f, bool need) {
+        if (need) {
+          uint8_t* dst = s_f + (size_t)((f + 3) % 3) * PFSLICE;
+          const bool fok = f >= 0 && f < a.D;
+          for (int idx = lt; idx < PFCHUNKS; idx += 128) {
+            const int r = idx / (PFCOLS * 4), rem = idx - r * (PFCOLS * 4), col = rem >> 2, cc = rem & 3;
+            const int fh = 2 * h0 - 1 + r, fw = 2 * w0 - 3 + col;
+            const bool ok = fok && fh >= 0 && fh < a.H && fw >= 0 && fw < a.W && cc * 8 < a.Cg;
+            cp_async16(dst + (size_t)idx * 16, ok ? a.gz + ((((size_t)b * a.D + f) * a.H + fh) * a.W + fw) * a.gpitch + cc * 8 : a.gz,
+                       ok ? 16u : 0u);
+          }
+        }
+        cp_async_commit();
+      };
+      load_fine(2 * d0 - 1, true);
+      load_fine(2 * d0, true);
+      load_fine(2 * d0 + 1, true);
+      for (int s = d0 - 1; s < d1; ++s) {
+        // ---- coarse x slab of slice s ----
+        mbar_wait(&xempty[xslot], xphase);
+        uint8_t* slab = s_x + (size_t)xslot * PXSLAB;
+        const bool dok = s >= 0 && s < a.Dc;
+        const __nv_bfloat16* base = a.x + ((size_t)b * a.Dc + (dok ? s : 0)) * a.Hc * a.Wc * a.xpitch;
+#pragma unroll
+        for (int k = 0; k < KX; ++k) {
+          const bool ok = dok && soff[k] >= 0;
+          cp_async16(slab + doff[k], ok ? base + soff[k] : a.x, ok ? 16u : 0u);
+        }
+        cp_async_arrive_noinc(&xfull[xslot]);
+        if (++xslot == (uint32_t)NS) { xslot = 0; xphase ^= 1; }
+        if (s < d0) continue;
+        // ---- the 16 G slabs of coarse slice s ----
+        mbar_wait(&gempty[gslot], gphase);
+        uint8_t* st = s_g + (size_t)gslot * PGSTAGE;
+        // one depth parity per pass (ad = 0: O, fine slices 2s-1, 2s; ad = 1: E, 2s, 2s+1): 32 live sums.  Before a
+        // pass, all but the most recent fine load group have landed: the pass's two slices (the newest is the next one)
+#pragma unroll 1
+        for (int ad = 0; ad < 2; ++ad) {
+          cp_async_wait<1>();
+          named_bar(1, 128);
+#pragma unroll 1
+          for (int u = lt >> 2; u < PGROWS; u += 32) {
+            const int i = u / TWR, j = u % TWR;
+            float g[2][2][8];                   // [ah][aw][channel], fp32 pair sums
+#pragma unroll
+            for (int q = 0; q < 32; ++q) (&g[0][0][0])[q] = 0.f;
+            if (j > 0 && cok) {
+#pragma unroll
+              for (int kd = 0; kd < 2; ++kd) {
+                const int fd = 2 * s - 1 + ad + kd;
+                if (fd < 0 || fd >= a.D) continue;
+                const uint8_t* fs = s_f + (size_t)((fd + 3) % 3) * PFSLICE;
+#pragma unroll
+                for (int kh = 0; kh < 3; ++kh) {
+                  float f[3][8];
+#pragma unroll
+                  for (int kw = 0; kw < 3; ++kw) {
+                    const uint4 q = *reinterpret_cast<const uint4*>(fs + (size_t)((((2 * i + kh) * PFCOLS) + 2 * j + kw) * 4 + c8) * 16);
+                    const __nv_bfloat162* hq = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                      const float2 v = __bfloat1622float2(hq[e]);
+                      f[kw][2 * e] = v.x; f[kw][2 * e + 1] = v.y;
+                    }
+                  }
+                  // fine tap k of an axis feeds O (k = 0, 1) and E (k = 1, 2)
+#pragma unroll
+                  for (int ah = 0; ah < 2; ++ah) {
+                    if (ah == 0 ? kh == 2 : kh == 0) continue;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                      g[ah][0][e] += f[0][e] + f[1][e];
+                      g[ah][1][e] += f[1][e] + f[2][e];
+                    }
+                  }
+                }
+              }
+              if (ad == 1)
+#pragma unroll
+                for (int e = 0; e < 8; ++e) bsum[e] += g[1][1][e];   // every fine voxel lies in exactly one E box
+            }
+            const uint32_t roff = swz((uint32_t)u * 64u + (uint32_t)c8 * 16u, 64);
+#pragma unroll
+            for (int ah = 0; ah < 2; ++ah)
+#pragma unroll
+              for (int aw = 0; aw < 2; ++aw) {
+                uint32_t hi[4], lo[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float v0 = g[ah][aw][2 * e], v1 = g[ah][aw][2 * e + 1];
+                  const __nv_bfloat162 h2 = __floats2bfloat162_rn(v0, v1);
+                  const float2 hf = __bfloat1622float2(h2);
+                  hi[e] = *reinterpret_cast<const uint32_t*>(&h2);
+                  lo[e] = pack_bf16x2(v0 - hf.x, v1 - hf.y);
+                }
+                *reinterpret_cast<uint4*>(st + (size_t)poly_slab(0, ad, ah, aw) * PGSLAB + roff) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                *reinterpret_cast<uint4*>(st + (size_t)poly_slab(1, ad, ah, aw) * PGSLAB + roff) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+              }
+          }
+          // every loader thread is done with slice 2s-1+ad: its slot takes slice 2s+2+ad (needed by slice s+1)
+          named_bar(1, 128);
+          load_fine(2 * s + 2 + ad, s + 1 < d1);
+        }
+        fence_proxy_async();                    // generic-proxy stores -> the wgmma (async proxy) reads
+        mbar_arrive(&gfull[gslot]);
+        if (++gslot == PNGS) { gslot = 0; gphase ^= 1; }
+      }
+    }
+    if (a.bias_partial) {
+      // bias partial of this CTA: fixed-order reduction over the 32 loader threads of each channel group
+      named_bar(1, 128);
+      if (lt < 32) {
+        float sum = 0.f;
+        for (int r = 0; r < 32; ++r) sum += s_bsum[(4 * r + (lt >> 3)) * 8 + (lt & 7)];
+        a.bias_partial[(size_t)blockIdx.x * 32 + lt] = has_work ? sum : 0.f;
+      }
+    }
+  } else {
+    // ================================ MMA WARPGROUPS ================================
+    const int wg = warp >> 2;                   // = kd: (O, -1), (E, 0), (O, 0)
+    const int t = threadIdx.x & 127;
+    const int ad = wg == 1 ? 1 : 0;
+    float acc[3][32];
+    if (has_work) {
+      const uint32_t x_u32 = smem_u32(s_x), g_u32 = smem_u32(s_g);
+      uint32_t wslot = 0, wphase = 0, hslot = 0, gs = 0, gph = 0, acc0 = 0;
+      for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
+        const int ch = (item / HW_tiles) % a.nchunks;
+        const int nd = min(ch * a.dchunk + a.dchunk, a.Dc + 1) - ch * a.dchunk;
+        for (int j = 0; j < nd; ++j) {
+          for (int q = 0; q < (j == 0 ? 2 : 1); ++q) {
+            mbar_wait(&xfull[wslot], wphase);
+            if (++wslot == (uint32_t)NS) { wslot = 0; wphase ^= 1; }
+          }
+          mbar_wait(&gfull[gs], gph);
+          const uint32_t cur = hslot + 1 == (uint32_t)NS ? 0 : hslot + 1;   // slab of slice s; hslot: slice s - 1
+          const uint32_t a_base = x_u32 + (wg == 0 ? hslot : cur) * PXSLAB;
+          const uint32_t b_base = g_u32 + gs * PGSTAGE + 64u;                // G row k + 1 pairs with x rows k, k + 1
+          wg_fence();
+#pragma unroll
+          for (int s3 = 0; s3 < 3; ++s3) {      // kh: (O, -1), (E, 0), (O, 0)
+            const int ah = s3 == 1 ? 1 : 0;
+            const uint64_t adesc0 = make_desc_mn_swz<64>(a_base + (s3 == 0 ? 0u : (uint32_t)TWR * 64u), 64u);
+#pragma unroll
+            for (int i = 0; i < PGROWS / 16; ++i)
+#pragma unroll
+              for (int hl = 0; hl < 2; ++hl) {
+                const uint64_t adesc = adesc0 + (uint64_t)((16 * i * 64) >> 4);
+                const uint64_t bdesc = make_desc_mn_swz<64>(b_base + (uint32_t)poly_slab(hl, ad, ah, 0) * PGSLAB + 16u * i * 64u, PGSLAB);
+                Wgmma<64, 1, 1>::mma(acc[s3], adesc, bdesc, (i == 0 && hl == 0) ? acc0 : 1u);
+              }
+          }
+          wg_commit();
+          wg_wait<0>();
+          if (lane == 0) {
+            mbar_arrive(&xempty[hslot]);
+            mbar_arrive(&gempty[gs]);
+          }
+          acc0 = 1u;
+          hslot = cur;
+          if (++gs == PNGS) { gs = 0; gph ^= 1; }
+        }
+        if (lane == 0) mbar_arrive(&xempty[hslot]);
+        if (++hslot == (uint32_t)NS) hslot = 0;
+      }
+    }
+    float* part = a.partial + (size_t)blockIdx.x * 27 * 32 * 32;
+    if (!has_work) {
+      for (int i = threadIdx.x; i < 27 * 32 * 32; i += 384) part[i] = 0.f;
+    } else {
+      // fragment (row m, column n): m = (sw, ci), n = (aw, co); kw = 0 for (sw = -1, O), 2 for (0, O), 1 for (0, E)
+      const int w4 = t >> 5, qr = lane >> 2, pc = lane & 3;
+#pragma unroll
+      for (int s3 = 0; s3 < 3; ++s3)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int m = 16 * w4 + 8 * i + qr, sw = m >> 5, ci = m & 31;
+#pragma unroll
+          for (int jn = 0; jn < 8; ++jn) {
+            const int n = 8 * jn + 2 * pc, aw = n >> 5, co = n & 31;
+            if (sw == 0 && aw == 1) continue;
+            const int kw = aw == 1 ? 1 : (sw == 0 ? 0 : 2);
+            const int tap = (wg * 3 + s3) * 3 + kw;
+            *reinterpret_cast<float2*>(part + ((size_t)tap * 32 + ci) * 32 + co) = make_float2(acc[s3][4 * jn + 2 * i], acc[s3][4 * jn + 2 * i + 1]);
+          }
+        }
+    }
+  }
+}
+
 // gw[co][ci_off + ci][tap] (+)= sum_cta partial[cta][tap][ci][co]   (fixed order -> deterministic).  Block = 64 elements
 // x 4 quarters of the CTA range: threads follow the partial layout (co fastest) so the reads coalesce, and the four
 // quarter sums (combined in fixed order through shared memory) keep 4x more loads in flight than one serial loop.
@@ -392,11 +671,88 @@ bool wgrad2_supported(int Ca, int Cb, int Cg) {
   return (Ca == 0 || chan_ok(Ca)) && (Cb == 0 || chan_ok(Cb)) && Ca + Cb > 0 && chan_ok(Cg);
 }
 
+// depth chunking: balance the persistent CTAs (waves of nsm items) against the `halo` slabs every chunk re-loads
+static int wgrad2_dchunk(int D, long long tiles, int nsm, double halo) {
+  int best_nch = 1;
+  double best_cost = 1e300;
+  for (int nch = 1; nch <= 32 && nch <= D; ++nch) {
+    const int dc = (D + nch - 1) / nch;
+    const long long items = tiles * ((D + dc - 1) / dc);
+    const long long waves = (items + nsm - 1) / nsm;
+    const double cost = (double)waves * (dc + halo);
+    if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
+  }
+  return (D + best_nch - 1) / best_nch;
+}
+
+// Partials of `grid` CTAs of T x G x GOUT floats at `partial` (bias partials at `bias_partial`): record the deferred
+// reduction, or reduce now.
+static int wgrad2_finish(float* partial, float* bias_partial, int grid, int T, int G, int GOUT, float* grad_w, float* grad_b, int Cout_real,
+                         int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer, int co_off) {
+  const int per_cta = T * G * GOUT;
+  if (defer) {
+    defer->partial = partial; defer->gw = grad_w; defer->bias_partial = bias_partial; defer->gb = grad_b;
+    defer->ncta = grid; defer->T = T; defer->G = G; defer->GOUT = GOUT; defer->Cout = Cout_real; defer->Cin_total = Cin_total;
+    defer->ci_off = ci_off; defer->ci_cnt = ci_cnt; defer->accumulate = accumulate; defer->blk_begin = (per_cta + 63) / 64;   // block count, turned into an offset by the flush
+    defer->co_off = co_off;
+    return VXM_OK;
+  }
+  wgrad2_reduce_kernel<<<(per_cta + 63) / 64, 256, 0, st>>>(partial, grad_w, grid, T, G, GOUT, Cout_real, Cin_total, ci_off, ci_cnt,
+                                                              bias_partial, grad_b, accumulate);
+  return check_launch("conv3d_tc_wgrad2_reduce");
+}
+
+// The coarse form (wgrad2_poly_kernel) serves every 3-D launch whose source is a 32-channel nearest-x2 upsampled slice
+// against a 32-channel gz slice, on even fine extents; VXM_B200_POLYPHASE=0 keeps the fine kernel (A/B switch).
+static bool wgrad2_poly_ok(int Cx, int up, int Cg, int kd, int D, int H, int W) {
+  const char* e = getenv("VXM_B200_POLYPHASE");
+  if (e && e[0] == '0' && e[1] == 0) return false;
+  return up && kd == 3 && Cx == 32 && Cg == 32 && D % 2 == 0 && H % 2 == 0 && W % 2 == 0;
+}
+
+static int wgrad2_poly_launch(const void* x, int x_pitch, const void* gz, int Cg, int g_pitch, float* grad_w, float* grad_b, void* work, int B,
+                              int D, int H, int W, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st,
+                              ReduceDesc* defer, size_t* work_used, int co_off) {
+  Wgrad2PolyArgs a{};
+  a.x = (const __nv_bfloat16*)x; a.xpitch = x_pitch;
+  a.gz = (const __nv_bfloat16*)gz; a.Cg = Cg; a.gpitch = g_pitch;
+  a.B = B; a.D = D; a.H = H; a.W = W; a.Dc = D / 2; a.Hc = H / 2; a.Wc = W / 2;
+  // G has Dc + 1 (Hc + 1, Wc + 1) coarse positions per axis: O[Dc] pairs the last fine voxel with the zero past it
+  a.tiles_h = (a.Hc + PTH) / PTH; a.tiles_w = (a.Wc + PTU) / PTU;
+  const int nsm = conv_ctas();
+  const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
+  a.dchunk = wgrad2_dchunk(a.Dc + 1, tiles, nsm, 0.5);
+  a.nchunks = (a.Dc + a.dchunk) / a.dchunk;
+  a.nitems = (int)(tiles * a.nchunks);
+  int grid = a.nitems < nsm ? a.nitems : nsm;
+  if (grid > 256) grid = 256;
+  a.partial = (float*)work;
+  if (defer) {
+    const size_t npart = (size_t)grid * 27 * 32 * 32;
+    a.bias_partial = grad_b ? (float*)work + npart : nullptr;
+    *work_used = (npart + (grad_b ? (size_t)grid * 32 : 0)) * sizeof(float);
+    *work_used = (*work_used + 255) & ~(size_t)255;
+  } else {
+    a.bias_partial = grad_b ? (float*)work + (size_t)256 * 27 * 64 * 32 : nullptr;
+  }
+  a.nslot = PNSLOT;
+  const size_t smem = PSMEM;
+  VXM_CUDA(cudaFuncSetAttribute(wgrad2_poly_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  wgrad2_poly_kernel<<<grid, PNTHREADS, smem, st>>>(a);
+  int rc = check_launch("conv3d_tc_wgrad2_poly");
+  if (rc) return rc;
+  return wgrad2_finish(a.partial, a.bias_partial, grid, 27, 32, 32, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, st, defer,
+                       co_off);
+}
+
 // one source tensor (C channels, optionally nearest-x2 upsampled) against gz; weights [ci_off, ci_off + ci_cnt) of Cin_total
 int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
                   int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer,
                   size_t* work_used, bool khm, int x_pitch, int g_pitch, int co_off) {
   VXM_REQUIRE(defer || co_off == 0, "conv3d_tc_wgrad2: gz slices need the deferred reduction");
+  if (!khm && wgrad2_poly_ok(Cx, up, Cg, kd, D, H, W))
+    return wgrad2_poly_launch(x, x_pitch ? x_pitch : Cx, gz, Cg, g_pitch ? g_pitch : Cg, grad_w, grad_b, work, B, D, H, W, Cout_real, Cin_total,
+                              ci_off, ci_cnt, accumulate, st, defer, work_used, co_off);
   Wgrad2Args a{};
   a.x = (const __nv_bfloat16*)x; a.Cx = Cx; a.up = up; a.upd = (up && kd == 3) ? 1 : 0;
   a.gz = (const __nv_bfloat16*)gz; a.Cg = Cg;
@@ -411,16 +767,8 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
   const int nsm = conv_ctas();
   // depth chunking: balance the persistent CTAs (waves of nsm items) against the 2 halo slabs every chunk re-loads
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
-  int best_nch = 1;
-  double best_cost = 1e300;
-  for (int nch = 1; nch <= 32 && nch <= D; ++nch) {
-    const int dc = (D + nch - 1) / nch;
-    const long long items = tiles * ((D + dc - 1) / dc);
-    const long long waves = (items + nsm - 1) / nsm;
-    const double cost = (double)waves * (dc + (kd == 3 ? 2.5 : 0.5));
-    if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
-  }
-  a.dchunk = (D + best_nch - 1) / best_nch; a.nchunks = (D + a.dchunk - 1) / a.dchunk;
+  a.dchunk = wgrad2_dchunk(D, tiles, nsm, kd == 3 ? 2.5 : 0.5);
+  a.nchunks = (D + a.dchunk - 1) / a.dchunk;
   a.nitems = (int)(tiles * a.nchunks);
   int grid = a.nitems < nsm ? a.nitems : nsm;
   if (grid > 256) grid = 256;
@@ -458,17 +806,8 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
   } else if (kd == 3) VXM_W2_G(3); else VXM_W2_G(1);
   int rc = check_launch("conv3d_tc_wgrad2");
   if (rc) return rc;
-  const int T = kd * 9, per_cta = T * G * GOUT;
-  if (defer) {
-    defer->partial = a.partial; defer->gw = grad_w; defer->bias_partial = a.bias_partial; defer->gb = grad_b;
-    defer->ncta = grid; defer->T = T; defer->G = G; defer->GOUT = GOUT; defer->Cout = Cout_real; defer->Cin_total = Cin_total;
-    defer->ci_off = ci_off; defer->ci_cnt = ci_cnt; defer->accumulate = accumulate; defer->blk_begin = (per_cta + 63) / 64;   // block count, turned into an offset by the flush
-    defer->co_off = co_off;
-    return VXM_OK;
-  }
-  wgrad2_reduce_kernel<<<(per_cta + 63) / 64, 256, 0, st>>>(a.partial, grad_w, grid, T, G, GOUT, Cout_real, Cin_total, ci_off, ci_cnt,
-                                                              a.bias_partial, grad_b, accumulate);
-  return check_launch("conv3d_tc_wgrad2_reduce");
+  return wgrad2_finish(a.partial, a.bias_partial, grid, kd * 9, G, GOUT, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, st,
+                       defer, co_off);
 }
 
 }  // namespace tcw
