@@ -384,6 +384,27 @@ int vxm_sample_normal_logvar_fwd(const float* params, float* z, long long* state
 int vxm_sample_normal_logvar_bwd(const float* grad_z, const float* params, const long long* state, const long long* ticket,
                                  float* grad_params, int B, int nd, size_t V, void* stream);
 
+/* ---- Phenotype decoder of ConditionalTemplateCreation (reference voxelmorph/tf/networks.py:856-983): Dense(V F, 'elu')
+ * and neurite's conv_dec with no levels (one 1x1 convolution F -> F, bias, linear) as one launch each way ----
+ * pheno (B, P), W (P, F, V), bias (F, V), like_w (F, F, [1, 1, 1]) (output channel g, input channel f), like_b (F),
+ * out (B, F, V), all fp32 device memory owned by the caller; V = prod(vol) (2-D and 3-D alike), 1 <= P <= 16,
+ * 1 <= F <= 32:
+ *   pre[b,f,v] = bias[f,v] + sum_p pheno[b,p] W[p,f,v],  h = pre > 0 ? pre : expm1(pre),
+ *   out[b,g,v] = like_b[g] + sum_f like_w[g,f] h[b,f,v]            (out overwritten)
+ * The backward recomputes pre and h (no activation is stored) and gives, with g_pre = (like_w^T grad_out) (h < 0 ? h + 1 : 1):
+ *   grad_W[p,f,v] = sum_b pheno[b,p] g_pre[b,f,v],  grad_bias[f,v] = sum_b g_pre[b,f,v],
+ *   grad_like_w[g,f] = sum_{b,v} grad_out[b,g,v] h[b,f,v],  grad_like_b[g] = sum_{b,v} grad_out[b,g,v];
+ * accumulate = 1 adds them to the four gradient buffers, 0 overwrites them (a batch larger than the kernel's register
+ * chunk, 64 / F entries rounded down to 1, 2 or 4, is added to grad_W and grad_bias one chunk at a time).  No gradient is
+ * formed for pheno.  Sums run in a fixed order: results are bit-reproducible.  work:
+ * vxm_pheno_decoder_workspace_bytes(F) bytes, zero before its first use; the call leaves it reusable. */
+size_t vxm_pheno_decoder_workspace_bytes(int F);
+int vxm_pheno_decoder_fwd(const float* pheno, const float* W, const float* bias, const float* like_w, const float* like_b,
+                          float* out, int B, int P, int F, size_t V, void* stream);
+int vxm_pheno_decoder_bwd(const float* grad_out, const float* pheno, const float* W, const float* bias, const float* like_w,
+                          float* grad_W, float* grad_bias, float* grad_like_w, float* grad_like_b, void* work, int B, int P,
+                          int F, size_t V, int accumulate, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

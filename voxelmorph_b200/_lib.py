@@ -104,6 +104,9 @@ SIGNATURES = {
     "vxm_mean_stream_bwd": (c_i, [c_f, c_f, c_f, c_i, c_sz, c_sz, c_f]),
     "vxm_sample_normal_logvar_fwd": (c_i, [c_f] * 5 + [c_i, c_i, c_sz, c_f]),
     "vxm_sample_normal_logvar_bwd": (c_i, [c_f] * 5 + [c_i, c_i, c_sz, c_f]),
+    "vxm_pheno_decoder_workspace_bytes": (c_sz, [c_i]),
+    "vxm_pheno_decoder_fwd": (c_i, [c_f] * 6 + [c_i, c_i, c_i, c_sz, c_f]),
+    "vxm_pheno_decoder_bwd": (c_i, [c_f] * 10 + [c_i, c_i, c_i, c_sz, c_i, c_f]),
 }
 
 _lib = None

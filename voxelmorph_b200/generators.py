@@ -26,7 +26,7 @@ from collections import OrderedDict
 import numpy as np
 
 __all__ = ["VolumeCache", "load_volfile", "volgen", "scan_to_scan", "scan_to_atlas", "semisupervised", "template_creation",
-           "Prefetcher"]
+           "conditional_template_creation", "Prefetcher"]
 
 
 def _cuda_ready():
@@ -302,6 +302,24 @@ def template_creation(vol_names, bidir=False, batch_size=1, zeros_dtype=np.float
         invols = [scan]
         outvols = [scan, zeros, zeros, zeros] if bidir else [scan, zeros, zeros]
         yield (invols, outvols)
+
+
+def conditional_template_creation(vol_names, atlas, attributes, batch_size=1, np_var='vol', pad_shape=None,
+                                  add_feat_axis=True, zeros_dtype=np.float32, cache=None):
+    """Conditional template creation; arguments, yields and random draws as reference generators.py:222-253:
+    ([pheno, atlas, vols], [vols, zeros, zeros, zeros]) with pheno (batch_size, P) the rows of `attributes` (a dict keyed
+    by the entries of `vol_names`, e.g. pyutils.load_pheno_csv's) for the drawn volumes, atlas (1, *vol, C) repeated over
+    the batch, zeros (batch_size, *vol, nd).  Volumes come through the decode-once cache; every array is float32."""
+    atlas = np.asarray(atlas)
+    zeros = _zero_flow(batch_size, atlas.shape[1:-1], zeros_dtype)
+    atlas = np.repeat(atlas.astype(np.float32, copy=False), batch_size, axis=0)
+    cache = _default_cache if cache is None else cache
+    opts = dict(pad_shape=pad_shape, add_feat_axis=add_feat_axis)
+    while True:
+        indices = np.random.randint(len(vol_names), size=batch_size)   # same draw as generators.py:241
+        pheno = np.stack([attributes[vol_names[i]] for i in indices], axis=0).astype(np.float32)
+        vols = _batch([cache.get(vol_names[i], np_var, **opts) for i in indices])
+        yield ([pheno, atlas, vols], [vols, zeros, zeros, zeros])
 
 
 def semisupervised(vol_names, seg_names, labels, atlas_file=None, downsize=2, prob_dtype=np.float32, zeros_dtype=np.float32, cache=None):

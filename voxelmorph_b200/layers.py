@@ -315,3 +315,106 @@ def sample_normal_logvar(params, state):
     device tensor: each call draws the stream of the current `call` and advances it by one on the device, and its backward
     regenerates that same eps instead of storing it."""
     return _SampleNormalLogVarFn.apply(params, state)
+
+
+_pd_ws = {}
+
+
+def _pheno_decoder_workspace(device, F):
+    """Per (device, stream, F) scratch of the decoder backward: zeroed once, the kernel leaves its ticket counter zero."""
+    key = (device.index, torch.cuda.current_stream(device).cuda_stream, int(F))
+    ws = _pd_ws.get(key)
+    if ws is None:
+        ws = torch.zeros(int(_lib.load().vxm_pheno_decoder_workspace_bytes(int(F))), dtype=torch.uint8, device=device)
+        _pd_ws[key] = ws
+    return ws
+
+
+def _flat_grad(p):
+    """p's .grad when it is a contiguous view of FusedAdam's flat gradient buffer (optim.FlatParams marks them)."""
+    return p.grad if getattr(p, "_vxm_flat_grad", False) and p.grad is not None and p.grad.is_contiguous() else None
+
+
+class _PhenoDecoderFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, pheno, weight, bias, like_weight, like_bias):
+        _lib.require_cuda(pheno, weight, bias, like_weight, like_bias, what="PhenoDecoder")
+        pheno = _lib.contig(pheno)
+        P, F = weight.shape[0], weight.shape[1]
+        vol = tuple(weight.shape[2:])
+        if pheno.dim() != 2 or pheno.shape[1] != P or tuple(bias.shape) != (F,) + vol \
+                or like_weight.numel() != F * F or like_weight.shape[0] != F or tuple(like_bias.shape) != (F,):
+            raise _lib.VxmError("PhenoDecoder: pheno %s does not match weight %s, bias %s, like_weight %s, like_bias %s"
+                                % (tuple(pheno.shape), tuple(weight.shape), tuple(bias.shape), tuple(like_weight.shape),
+                                   tuple(like_bias.shape)))
+        if not (weight.is_contiguous() and bias.is_contiguous() and like_weight.is_contiguous()):
+            raise _lib.VxmError("PhenoDecoder: the parameters must be contiguous")
+        B, V = pheno.shape[0], bias[0].numel()
+        out = torch.empty((B, F) + vol, dtype=torch.float32, device=pheno.device)
+        _lib.check(_lib.load().vxm_pheno_decoder_fwd(_lib.ptr(pheno), _lib.ptr(weight), _lib.ptr(bias), _lib.ptr(like_weight),
+                                                     _lib.ptr(like_bias), _lib.ptr(out), B, P, F, V, _lib.stream_ptr()),
+                   "vxm_pheno_decoder_fwd")
+        ctx.save_for_backward(pheno, weight, bias, like_weight, like_bias)
+        ctx.cfg = (B, P, F, V)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        pheno, weight, bias, like_weight, like_bias = ctx.saved_tensors
+        B, P, F, V = ctx.cfg
+        gout = _lib.contig(gout)
+        params = (weight, bias, like_weight, like_bias)
+        flat = [_flat_grad(p) for p in params]
+        # like the tensor-core engine's weight gradients: straight into FusedAdam's flat buffer when every parameter has
+        # its view there, and autograd then receives none; otherwise fresh tensors for autograd to accumulate
+        accumulate = all(g is not None for g in flat)
+        outs = flat if accumulate else [torch.empty_like(p) for p in params]
+        _lib.check(_lib.load().vxm_pheno_decoder_bwd(_lib.ptr(gout), _lib.ptr(pheno), _lib.ptr(weight), _lib.ptr(bias),
+                                                     _lib.ptr(like_weight), *[_lib.ptr(g) for g in outs],
+                                                     _lib.ptr(_pheno_decoder_workspace(gout.device, F)), B, P, F, V,
+                                                     int(accumulate), _lib.stream_ptr()), "vxm_pheno_decoder_bwd")
+        if accumulate:
+            return None, None, None, None, None
+        return (None,) + tuple(outs)
+
+
+class PhenoDecoder(nn.Module):
+    """The phenotype decoder of ConditionalTemplateCreation (reference voxelmorph/tf/networks.py:905-915): a Dense layer
+    from P subject attributes to a full-resolution F-channel image with ELU, then neurite's conv_dec with no levels, one
+    1x1 convolution F -> F with bias and no activation.  For pheno (B, P):
+
+        pre = bias + sum_p pheno[:, p] weight[p],  h = ELU(pre),  out = like_bias + like_weight * h  (1x1 convolution)
+
+    out is (B, F, *inshape).  `weight` is stored (P, F, *inshape) and `bias` (F, *inshape), so the output is channels-first
+    with no transpose.  A Keras Dense kernel (P, V F) and bias (V F,) (V = prod(inshape), F fastest, as Keras' Reshape to
+    (*inshape, F) reads them) map onto it by reshaping to (P, *inshape, F) and (*inshape, F) and moving F to axis 1 and 0:
+    see `from_keras`.  Initialisation is Keras': glorot-uniform kernels (the Dense's fans P and V F, the 1x1
+    convolution's F and F), zero biases.
+
+    Forward and backward are one kernel launch each (csrc/pheno_decoder.cu); no activation is kept, the backward recomputes
+    it.  When every parameter's .grad is a view of FusedAdam's flat buffer the gradients are accumulated there directly.
+    No gradient is formed for pheno.  Limits: 1 <= P <= 16, 1 <= F <= 32."""
+
+    def __init__(self, P, F, inshape):
+        super().__init__()
+        inshape = tuple(int(s) for s in inshape)
+        V = int(math.prod(inshape))
+        nd = len(inshape)
+        lim = math.sqrt(6.0 / (P + V * F))
+        self.weight = nn.Parameter(torch.empty((P, F) + inshape).uniform_(-lim, lim))
+        self.bias = nn.Parameter(torch.zeros((F,) + inshape))
+        lim = math.sqrt(6.0 / (2 * F))
+        self.like_weight = nn.Parameter(torch.empty((F, F) + (1,) * nd).uniform_(-lim, lim))
+        self.like_bias = nn.Parameter(torch.zeros(F))
+
+    @staticmethod
+    def from_keras(kernel, bias, inshape):
+        """(weight, bias) of this layout from a Keras Dense kernel (P, V F) and bias (V F,)."""
+        kernel, bias = torch.as_tensor(kernel), torch.as_tensor(bias)
+        inshape = tuple(inshape)
+        w = kernel.reshape((kernel.shape[0],) + inshape + (-1,)).movedim(-1, 1)
+        b = bias.reshape(inshape + (-1,)).movedim(-1, 0)
+        return w.contiguous(), b.contiguous()
+
+    def forward(self, pheno):
+        return _PhenoDecoderFn.apply(pheno, self.weight, self.bias, self.like_weight, self.like_bias)

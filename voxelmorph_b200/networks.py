@@ -455,3 +455,97 @@ class TemplateCreation(LoadableModel):
     # the transform from source to target and its application to an image, through the inner VxmDense
     register = VxmDenseSemiSupervisedSeg.register
     apply_transform = VxmDenseSemiSupervisedSeg.apply_transform
+
+
+def _glorot_conv_(conv):
+    """Keras' default initialisation of a convolution: glorot-uniform kernel (fans = taps x channels), zero bias."""
+    taps = int(np.prod(conv.weight.shape[2:]))
+    lim = float(np.sqrt(6.0 / (taps * (conv.weight.shape[0] + conv.weight.shape[1]))))
+    with torch.no_grad():
+        conv.weight.uniform_(-lim, lim)
+        conv.bias.zero_()
+    return conv
+
+
+class ConditionalTemplateCreation(LoadableModel):
+    """VoxelMorph network to learn a conditional template: one atlas for every set of subject attributes (Dalca et al.,
+    "Learning Conditional Deformable Templates with Convolutional Networks", NeurIPS 2019).
+
+    The torch backend of the reference has no such class; the semantics are those of its TensorFlow model
+    (voxelmorph/tf/networks.py:856-983).  For pheno (B, P), atlas (B or 1, atlas_feats, *inshape) and image
+    (B, src_feats, *inshape):
+
+        x0 = pheno_decoder(pheno)                 Dense(prod(inshape) F, 'elu') and neurite's conv_dec with no levels
+                                                  (a 1x1 convolution F -> F, linear): layers.PhenoDecoder
+        x_i = extra_convs[i](x_{i-1})             extra_conv_layers convolutions F -> F, 3^n, no activation
+        atlas_t = atlas + atlas_gen(x)            F -> atlas_feats, 3^n, weight and bias ~ N(0, 1e-7)
+        pos_flow, neg_flow = vxm_model.flows(atlas_t, image)     bidirectional VxmDense, atlas_t moving
+        outputs = (y_source, mean_stream(neg_flow), pos_flow, pos_flow)   or (y_source, pos_flow, pos_flow) without
+                                                  the mean stream; registration=True: (y_source, pos_flow)
+
+    with F = conv_nb_features.  The warp of the image by neg_flow (TF's unused y_target) is not computed.  Keras'
+    initialisation is kept: glorot-uniform kernels and zero biases in the decoder and the extra convolutions.  The extra
+    convolutions and atlas_gen run on the fp32 CUDA-core kernels whatever the U-Net's engine.
+
+    Checkpoint keys: `pheno_decoder.*`, `extra_convs.{i}.*`, `atlas_gen.*`, `vxm_model.*` and the mean stream's buffers
+    `mean_stream.mean` / `mean_stream.count`.  `template(pheno, atlas)` returns the conditional atlas (TF's pheno_model).
+    Not implemented (NotImplementedError): conv_nb_levels > 0, templcondsi, a conv_image_shape other than
+    (*inshape, conv_nb_features) and conv_size other than 3.  `kwargs` are forwarded to the inner VxmDense."""
+
+    @store_config_args
+    def __init__(self, inshape, pheno_input_shape, nb_unet_features=None, src_feats=1, atlas_feats=None,
+                 conv_image_shape=None, conv_size=3, conv_nb_levels=0, conv_nb_features=32, extra_conv_layers=3,
+                 use_mean_stream=True, mean_cap=100, templcondsi=False, templcondsi_init=None, **kwargs):
+        super().__init__()
+        inshape = tuple(int(s) for s in inshape)
+        ndims = len(inshape)
+        F = int(conv_nb_features)
+        if atlas_feats is None:
+            atlas_feats = src_feats
+        if templcondsi:
+            raise NotImplementedError("ConditionalTemplateCreation: templcondsi is not implemented (the TF branch reads an "
+                                      "undefined tensor and cannot run either)")
+        if conv_nb_levels > 0:
+            raise NotImplementedError("ConditionalTemplateCreation: conv_nb_levels > 0 (a conv_dec U-Net in the atlas "
+                                      "generator) is not implemented; use conv_nb_levels=0")
+        if conv_image_shape is not None and tuple(conv_image_shape) != inshape + (F,):
+            raise NotImplementedError("ConditionalTemplateCreation: conv_image_shape must be (*inshape, conv_nb_features) "
+                                      "= %s, got %s" % (inshape + (F,), tuple(conv_image_shape)))
+        if conv_size != 3:
+            raise NotImplementedError("ConditionalTemplateCreation: conv_size must be 3 (the convolution kernels are 3^n), "
+                                      "got %r" % (conv_size,))
+        P = int(np.prod(pheno_input_shape))
+        self.pheno_decoder = layers.PhenoDecoder(P, F, inshape)
+        Conv = _conv_cls(ndims)
+        self.extra_convs = nn.ModuleList([_glorot_conv_(Conv(F, F, 3, padding=1)) for _ in range(extra_conv_layers)])
+        self.atlas_gen = Conv(F, atlas_feats, 3, padding=1)
+        self.atlas_gen.weight = nn.Parameter(Normal(0, 1e-7).sample(self.atlas_gen.weight.shape))
+        self.atlas_gen.bias = nn.Parameter(Normal(0, 1e-7).sample(self.atlas_gen.bias.shape))
+        self.vxm_model = VxmDense(inshape, nb_unet_features, bidir=True, src_feats=atlas_feats, trg_feats=src_feats, **kwargs)
+        self.mean_stream = layers.MeanStream((ndims,) + inshape, cap=mean_cap) if use_mean_stream else None
+
+    def _atlas(self, pheno, atlas):
+        x = self.pheno_decoder(pheno)
+        for conv in self.extra_convs:
+            x = conv(x)
+        return atlas + self.atlas_gen(x)
+
+    def template(self, pheno, atlas):
+        """The conditional atlas atlas + atlas_gen(...) for attributes `pheno` (B, P), without autograd."""
+        with torch.no_grad():
+            return self._atlas(pheno, atlas)
+
+    def forward(self, pheno, atlas, image, registration=False):
+        from . import dist as vdist
+        if vdist.env_world()[0] > 1:
+            raise _lib.VxmError("ConditionalTemplateCreation does not run data parallel yet: each rank would keep its own "
+                                "mean stream, and the atlas generator lies outside the inner model's gradient exchange; "
+                                "train it on one GPU (WORLD_SIZE=1)")
+        atlas_t = self._atlas(pheno, atlas)
+        pos_flow, neg_flow, _ = self.vxm_model.flows(atlas_t, image)
+        y_source = self.vxm_model.transformer(atlas_t, pos_flow)
+        if registration:
+            return y_source, pos_flow
+        if self.mean_stream is None:
+            return y_source, pos_flow, pos_flow
+        return y_source, self.mean_stream(neg_flow), pos_flow, pos_flow
