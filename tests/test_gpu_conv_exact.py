@@ -79,7 +79,9 @@ def _report(title, rows):
 # kw: the VxmDense arguments (every size divisible by 2^levels); B: the batch; tc: the engine VXM_B200_CONV_ENGINE=tc runs
 # the model on; blocked: whether its bf16x3 plan has channel-blocked launches.  "doubled" (64 channels) runs on f32 under
 # 'tc' and is checked here for VXM_B200_CONV_ENGINE=bf16 / bf16x3 set explicitly.
-Case = collections.namedtuple("Case", "kw B tc blocked")
+# probs: a VxmDenseProbabilistic, whose head is one 2 nd-output convolution (flow, then log_sigma); its U-Net layers are those of
+# the VxmDense case of the same arguments, so only the head is checked
+Case = collections.namedtuple("Case", "kw B tc blocked probs", defaults=(False,))
 MODELS = {
     "default": Case(dict(inshape=(160, 192, 224)), 1, "bf16x3", False),
     "doubled": Case(dict(inshape=(64, 96, 112), nb_unet_features=DOUBLED), 1, "f32", True),
@@ -91,7 +93,15 @@ MODELS = {
     "2d": Case(dict(inshape=(192, 224)), 8, "bf16x3", False),
     "2d_doubled": Case(dict(inshape=(160, 192), nb_unet_features=DOUBLED), 2, "f32", True),
     "2d_halfres": Case(dict(inshape=(176, 240), unet_half_res=True), 3, "bf16x3", False),
+    "probs": Case(dict(inshape=(160, 192, 224)), 1, "bf16x3", False, True),
+    "probs_2d": Case(dict(inshape=(192, 224)), 8, "bf16x3", False, True),
+    "probs_halfres": Case(dict(inshape=(160, 192, 224), unet_half_res=True), 2, "bf16x3", False, True),
 }
+
+
+def build_model(vxm, name):
+    cls = vxm.networks.VxmDenseProbabilistic if MODELS[name].probs else vxm.networks.VxmDense
+    return cls(**MODELS[name].kw)
 
 
 def plan_sizes(eng, plan, inshape):
@@ -115,20 +125,51 @@ def check_resolves(vxm, monkeypatch, name, model):
     monkeypatch.delenv("VXM_B200_CONV_ENGINE")
 
 
-# "split+unfolded" changes a form only in 3-D (polyphase and kd folding are 3-D forms)
-@pytest.mark.parametrize("name,forms", [(n, f) for n in sorted(MODELS) for f in ("polyphase+kdfold", "split+unfolded")
-                                        if f == "polyphase+kdfold" or len(MODELS[n].kw["inshape"]) == 3])
-def test_plan_launches_exact(vx, cuda, monkeypatch, name, forms):
-    """Forward, dgrad and weight gradient of every layer of the plan through the engine's own calls (_run, WgradBatch), with
-    the arguments forward_tape / backward_tape pass.  "split+unfolded" (VXM_B200_POLYPHASE=0, VXM_B200_KDFOLD=0) runs the
-    layers whose form that changes."""
-    vxm, eng, tc = vx
-    kw, B = MODELS[name].kw, MODELS[name].B
-    g = torch.Generator(device=cuda).manual_seed(1 + len(name))
-    model = vxm.networks.VxmDense(**kw).to(cuda)
+def quantise(model, g):
     with torch.no_grad():
         for p in model.parameters():
             p.copy_(qweight(p.shape, g))
+
+
+def tape_operands(eng, tc, plan, inshape, B, g):
+    """The exact tier's operands of a plan: image planes (B, 1, D, H, W) and their channels-last cat, the ternary bf16
+    tensor X[i] of every tensor id but the flow's (X[0]: the images as the first convolution reads them), the ternary
+    output gradient G of every convolution but the head, and the head's gradient planes with their channels-last cat"""
+    size, chans = plan_sizes(eng, plan, inshape)
+    first, flow = plan.layers[0], plan.layers[-1]
+    planes = [ternary((B, 1) + size[0], g, torch.float32) * PLANE for _ in range(first.cin)]
+    images = torch.cat(planes, 1).permute(0, 2, 3, 4, 1)
+    X = {i: ternary((B,) + size[i] + (c,), g) for i, c in chans.items() if i != flow.out}
+    X[0] = tc.planar_fold_kd(planes, 8) if first.fwd == "fold" else tc.planar_to_ndhwc8(planes)
+    G = {L.out: ternary((B,) + size[L.out] + (L.cout,), g) for L in plan.layers if L is not flow}
+    gplanes = [ternary((B, 1) + size[flow.out], g, torch.float32) * PLANE for _ in range(flow.cout)]
+    gflow = torch.cat(gplanes, 1).permute(0, 2, 3, 4, 1)
+    return size, planes, images, X, G, gplanes, gflow
+
+
+def check_head_plan(model, plan):
+    """the plan facts of a probabilistic model's head: one 2 nd-output convolution that is never kd-folded, derived from
+    four parameters, whose persistent operands are cat(flow, log_sigma) bit for bit"""
+    flow = plan.layers[-1]
+    assert flow.role == "flow" and flow.cout == 2 * plan.nd and flow.dgrad != "fold"
+    assert len(flow.srcs) == 4 and flow.srcs[0] is model.flow.weight and flow.srcs[3] is model.log_sigma.bias
+    assert torch.equal(flow.w, torch.cat([model.flow.weight.detach(), model.log_sigma.weight.detach()]))
+    assert torch.equal(flow.bias, torch.cat([model.flow.bias.detach(), model.log_sigma.bias.detach()]))
+
+
+# "split+unfolded" changes a form only in 3-D (polyphase and kd folding are 3-D forms); a probabilistic head runs the same
+# form in both settings, and its U-Net layers are checked by the VxmDense cases
+@pytest.mark.parametrize("name,forms", [(n, f) for n in sorted(MODELS) for f in ("polyphase+kdfold", "split+unfolded")
+                                        if f == "polyphase+kdfold" or (len(MODELS[n].kw["inshape"]) == 3 and not MODELS[n].probs)])
+def test_plan_launches_exact(vx, cuda, monkeypatch, name, forms):
+    """Forward, dgrad and weight gradient of every layer of the plan through the engine's own calls (_run, WgradBatch), with
+    the arguments forward_tape / backward_tape pass.  "split+unfolded" (VXM_B200_POLYPHASE=0, VXM_B200_KDFOLD=0) runs the
+    layers whose form that changes.  A probabilistic model: its 2 nd-output head only."""
+    vxm, eng, tc = vx
+    kw, B = MODELS[name].kw, MODELS[name].B
+    g = torch.Generator(device=cuda).manual_seed(1 + len(name))
+    model = build_model(vxm, name).to(cuda)
+    quantise(model, g)
     check_resolves(vxm, monkeypatch, name, model)
     monkeypatch.setenv("VXM_B200_POLYPHASE", "1")
     monkeypatch.setenv("VXM_B200_KDFOLD", "1")
@@ -139,21 +180,18 @@ def test_plan_launches_exact(vx, cuda, monkeypatch, name, forms):
     plan = eng._plan_of(model, False)
     layers = plan.layers
     nd, kd = plan.nd, (3 if plan.nd == 3 else 1)
-    only = {i for i, (L, L0) in enumerate(zip(layers, base)) if forms == "polyphase+kdfold" or L.fwd != L0.fwd or L.dgrad != L0.dgrad}
+    if MODELS[name].probs:
+        check_head_plan(model, plan)
+        only = {len(layers) - 1}
+    else:
+        only = {i for i, (L, L0) in enumerate(zip(layers, base)) if forms == "polyphase+kdfold" or L.fwd != L0.fwd or L.dgrad != L0.dgrad}
     assert only
     if forms == "polyphase+kdfold":
         assert (layers[0].fwd == "fold") == (nd == 3 and layers[0].cin == 2)
         if name == "default":
             assert sum(1 for L in layers if L.dgrad_skip is not None) == 4 and layers[-1].dgrad == "fold"
-    size, chans = plan_sizes(eng, plan, kw["inshape"])
     first, flow = layers[0], layers[-1]
-    planes = [ternary((B, 1) + size[0], g, torch.float32) * PLANE for _ in range(first.cin)]
-    images = torch.cat(planes, 1).permute(0, 2, 3, 4, 1)
-    X = {i: ternary((B,) + size[i] + (c,), g) for i, c in chans.items() if i != flow.out}
-    X[0] = tc.planar_fold_kd(planes, 8) if first.fwd == "fold" else tc.planar_to_ndhwc8(planes)
-    G = {L.out: ternary((B,) + size[L.out] + (L.cout,), g) for L in layers if L is not flow}
-    gplanes = [ternary((B, 1) + size[flow.out], g, torch.float32) * PLANE for _ in range(flow.cout)]
-    gflow = torch.cat(gplanes, 1).permute(0, 2, 3, 4, 1)
+    size, planes, images, X, G, gplanes, gflow = tape_operands(eng, tc, plan, kw["inshape"], B, g)
     for L in layers:
         assert bool(((L.w * 64).abs() <= 8).all()) and bool(((L.bias * 64).abs() <= 8).all())
 
@@ -269,6 +307,95 @@ def test_plan_launches_exact(vx, cuda, monkeypatch, name, forms):
                 rw, rb = prior[0] + rw, prior[1] + rb
             rows.append((lname(i, layers[i]), form, mism(gw.reshape(rw.shape), rw) + mism(gb, rb), margin))
     _report("exact %s %s" % (name, forms), rows)
+
+
+@pytest.mark.parametrize("name", ["probs", "probs_2d"])
+def test_head_split_exact(vx, cuda, monkeypatch, name):
+    """backward_tape over the exact tier's operands and a quantised head gradient: the 2 nd-output head's weight and bias
+    gradients reach flow.weight, flow.bias, log_sigma.weight and log_sigma.bias as the [:nd] / [nd:] slices of the fp64
+    sums, through autograd's dict; with the parameters re-pointed into FlatParams, into the four .grad views on top of
+    integer-valued priors, and autograd gets nothing for them."""
+    vxm, eng, tc = vx
+    kw, B = MODELS[name].kw, MODELS[name].B
+    g = torch.Generator(device=cuda).manual_seed(70 + len(name))
+    model = build_model(vxm, name).to(cuda)
+    quantise(model, g)
+    plan = eng._plan_of(model, False)
+    check_head_plan(model, plan)
+    nd, kd = plan.nd, (3 if plan.nd == 3 else 1)
+    flow = plan.layers[-1]
+    _, _, _, X, _, gplanes, gflow = tape_operands(eng, tc, plan, kw["inshape"], B, g)
+    g_flow = torch.cat(gplanes, 1)
+    if nd == 2:
+        g_flow = g_flow.squeeze(2)         # as forward_tape returns a 2-D flow
+    gw, gb = ref.wgrad([(X[flow.a], False)], gflow, kd, nd=nd)
+    aw, ab = ref.wgrad([(X[flow.a], False)], gflow, kd, absolute=True, nd=nd)
+    margin = max(float(aw.max()) / PLANE, float(ab.max()) / PLANE / 2) / 2 ** 24
+    heads = [model.flow.weight, model.flow.bias, model.log_sigma.weight, model.log_sigma.bias]
+    want = [gw[:nd].float(), gb[:nd].float(), gw[nd:].float(), gb[nd:].float()]
+    want = [w.reshape(p.shape) for w, p in zip(want, heads)]
+    rows = []
+    grads = eng.backward_tape(dict(plan=plan, tensors=X, split=False, pool_lows={}), g_flow)
+    for p, w, what in zip(heads, want, ("flow.weight", "flow.bias", "log_sigma.weight", "log_sigma.bias")):
+        rows.append((what, "head split", mism(grads[p], w), margin))
+    fp = vxm.optim.FlatParams(list(model.parameters()))
+    fp.grad.copy_(torch.randint(-4, 5, (fp.numel,), generator=g, device=cuda).float())
+    priors = [p.grad.clone() for p in heads]
+    views = [p.grad for p in heads]
+    grads = eng.backward_tape(dict(plan=plan, tensors=X, split=False, pool_lows={}), g_flow)
+    assert not any(p in grads for p in heads)
+    assert all(p.grad is v for p, v in zip(heads, views))
+    for p, w, prior, what in zip(heads, want, priors, ("flow.weight", "flow.bias", "log_sigma.weight", "log_sigma.bias")):
+        rows.append((what, "flat view accumulated", mism(p.grad, prior + w), margin))
+    _report("head split %s" % name, rows)
+
+
+# every model of the matrix, both engines; "default" with source.requires_grad, so that the image dgrad runs as well
+FLAT_CASES = [(n, s) for n in sorted(MODELS) for s in (False, True)]
+
+
+@pytest.mark.parametrize("name,split", FLAT_CASES, ids=["%s-%s" % (n, "bf16x3" if s else "bf16") for n, s in FLAT_CASES])
+def test_flat_grads_equal_autograd(vx, cuda, name, split):
+    """unet_flow on ordinary weights and images, backward with one fixed flow gradient (no VecInt or warp atomics), once
+    with plain parameters (autograd) and once with FusedAdam's FlatParams views zeroed by zero_grad: every parameter's
+    gradient bit-identical, written in place into the flat buffer (the kd-folded first layer and flow head through their
+    unfolded views, the 2 nd-output head through its split, 2-D layers through the squeeze), and the image gradient
+    unchanged."""
+    vxm, eng, _ = vx
+    kw, B = MODELS[name].kw, MODELS[name].B
+    torch.manual_seed(90 + len(name))
+    model = build_model(vxm, name).to(cuda)
+    g = torch.Generator(device=cuda).manual_seed(91 + len(name))
+    with torch.no_grad():
+        for m in (model.flow, getattr(model, "log_sigma", None)):
+            if m is not None:
+                m.weight.copy_(torch.randn(m.weight.shape, generator=g, device=cuda) * 0.05)
+    inshape = tuple(kw["inshape"])
+    S = torch.rand((B, kw.get("src_feats", 1)) + inshape, generator=g, device=cuda)
+    T = torch.rand((B, kw.get("trg_feats", 1)) + inshape, generator=g, device=cuda)
+    image_grad = name == "default"
+    params = list(model.parameters())
+    gflow = []
+
+    def run():
+        src = S.clone().requires_grad_(image_grad)
+        out = eng.unet_flow(model, src, T, split=split)
+        if not gflow:
+            gflow.append(torch.randn(out.shape, generator=g, device=cuda))
+        out.backward(gflow[0])
+        return out.detach(), [p.grad.clone() for p in params], src.grad
+
+    f1, g1, s1 = run()
+    assert all(bool(t.any()) for t in g1)
+    fp = vxm.optim.FlatParams(params)
+    fp.zero_grad()
+    views = [p.grad for p in params]
+    f2, g2, s2 = run()
+    assert all(p.grad is v for p, v in zip(params, views))         # accumulated in place: autograd got nothing
+    assert torch.equal(f1, f2)
+    bad = [n for (n, _), a, b in zip(model.named_parameters(), g1, g2) if not torch.equal(a, b)]
+    assert not bad, bad
+    assert (s1 is None) == (not image_grad) and (s1 is None or torch.equal(s1, s2))
 
 
 # ---- b. the glue kernels of the full-size backward ------------------------------------------------------------------

@@ -22,7 +22,7 @@ import torch
 import torch.nn.functional as F
 
 import conv_exact_ref as ref
-from test_gpu_conv_exact import CAPS, MODELS, _children, _unchildren, check_resolves, mism, plan_sizes, ternary
+from test_gpu_conv_exact import CAPS, MODELS, _children, _unchildren, build_model, check_head_plan, check_resolves, mism, plan_sizes, ternary
 
 pytestmark = pytest.mark.gpu
 
@@ -94,11 +94,12 @@ def _split_margin(cin, unit_terms, bias_units):
 @pytest.mark.parametrize("name", sorted(MODELS))
 def test_split_forward_exact(vx, cuda, monkeypatch, name):
     """Every layer of the bf16x3 plan through _run(L.fwd_x3, L.pk_hi, ..., lo=(xa_lo, xb_lo, L.pk_lo)), as forward_tape
-    runs it; the first layer on the output of planar_to_ndhwc8_split.  Every model of the exact tier's matrix."""
+    runs it; the first layer on the output of planar_to_ndhwc8_split.  Every model of the exact tier's matrix (of a
+    probabilistic one, the 2 nd-output head, whose hi / lo parts come from the concatenated fp32 head)."""
     vxm, eng, tc = vx
     kw, B = MODELS[name].kw, MODELS[name].B
     g = torch.Generator(device=cuda).manual_seed(11 + len(name))
-    model = vxm.networks.VxmDense(**kw).to(cuda)
+    model = build_model(vxm, name).to(cuda)
     kj = {}
     with torch.no_grad():
         for p in model.parameters():
@@ -109,6 +110,10 @@ def test_split_forward_exact(vx, cuda, monkeypatch, name):
     plan = eng._plan_of(model, True)
     layers = plan.layers
     nd, kd = plan.nd, (3 if plan.nd == 3 else 1)
+    if MODELS[name].probs:
+        check_head_plan(model, plan)
+        fw, _, lw, _ = layers[-1].srcs
+        kj[layers[-1].w] = tuple(torch.cat([a, b]) for a, b in zip(kj[fw], kj[lw]))
     for L in layers:
         k, j = kj[L.w]
         assert torch.equal(L.w_hi, k * 2.0 ** -6) and torch.equal(L.w_lo, j * 2.0 ** -15)
@@ -136,6 +141,8 @@ def test_split_forward_exact(vx, cuda, monkeypatch, name):
 
     rows = [("00 images", "planar_to_ndhwc8_split", n_glue, 0.0)]
     for i, L in enumerate(layers):
+        if MODELS[name].probs and L is not flow:
+            continue
         bias, D = L.bias.detach(), size[L.out][0]
         out = eng._run(L.fwd_x3, L.pk_hi, XH[L.a], XH.get(L.b), L.cout, kd, bias, lo=(XL[L.a], XL.get(L.b), L.pk_lo),
                        up=L.up, slope=L.slope, out_fp32_planar=L is flow)
@@ -439,10 +446,32 @@ RAGGED = [
 ]
 
 
+# ConditionalTemplateCreation's generator convolutions (extra_convs F -> F, atlas_gen F -> atlas_feats, no activation, at
+# full resolution): (inshape, B, conv_nb_features F, atlas_feats).  F = 32 is the default, F = 4 the setting of
+# tools/cond_template_step.py
+COND_GEN = [((160, 192, 224), 1, 32, 1), ((160, 192, 224), 1, 4, 1), ((192, 224), 8, 32, 2)]
+
+
+def _cond_gen_convs():
+    """the generator convolutions, read off a ConditionalTemplateCreation's own modules (built at a small size of the same
+    dimensionality: channel counts do not depend on it, and the phenotype decoder holds prod(inshape) F weights per
+    attribute).  The extra convolutions are identical, so the first one stands for all of them."""
+    import voxelmorph_b200 as vxm
+    out = []
+    for inshape, B, F, af in COND_GEN:
+        m = vxm.networks.ConditionalTemplateCreation((16,) * len(inshape), (1,), conv_nb_features=F, atlas_feats=af)
+        assert len({(c.in_channels, c.out_channels) for c in m.extra_convs}) == 1
+        shape = (1,) * (3 - len(inshape)) + tuple(inshape)
+        for what, c in (("extra_convs", m.extra_convs[0]), ("atlas_gen", m.atlas_gen)):
+            out.append(("cond F=%d %s %d->%d %s B=%d" % (F, what, c.in_channels, c.out_channels, "x".join(map(str, inshape)), B),
+                        c.in_channels, c.out_channels, shape, B, False, None))
+    return out
+
+
 def _f32_cases():
     # (label, cin, cout, shape (D, H, W; D = 1 with kd = 1 for 2-D), B, activation, model or None)
     return (_model_convs("default") + _model_convs("doubled") + [("2-D 32->16 B=2", 32, 16, (1, 192, 224), 2, True, None)]
-            + _model_convs("2d_halfres") + _model_convs("ragged") + _model_convs("planes9")
+            + _model_convs("2d_halfres") + _model_convs("ragged") + _model_convs("planes9") + _cond_gen_convs()
             + [("%s %d->%d %s B=%d" % ("2-D" if D == 1 else "3-D", cin, cout, "x".join(map(str, (D, H, W) if D > 1 else (H, W))), B),
                 cin, cout, (D, H, W), B, act, None) for cin, cout, (D, H, W), B, act in RAGGED])
 
