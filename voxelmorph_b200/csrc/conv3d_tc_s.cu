@@ -58,13 +58,19 @@ __device__ __forceinline__ uint64_t make_desc_kmajor_swz(uint32_t saddr, uint32_
   return d | desc_swizzle(width);
 }
 
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 // HT = 8: one slab step feeds TWO 4-row accumulators (one per epilogue group), halving the per-step issue / barrier
 // overhead that bounds the thin layers and cutting the halo re-reads from 1.5x to 1.25x.
 // ACC: the split-precision epilogue (acc_in / out_mode 2, 3) is compiled in; the plain kernels (ACC = false) keep the
 // round-1 epilogue — with the extra live registers the 32-channel variants spilled and lost up to 1.8x.
 // EPI: epilogue specialisation.  0 = generic run-time epilogue; 1 = forward (bias + LeakyReLU with
 // 0 <= slope <= 1, bf16 channels-last, all COUT channels real); 2 = dgrad (LeakyReLU derivative from the saved activation);
-// 3 = raw sums with an optional channel split at a multiple of 16 (single-pass dgrad of a concat layer).
+// 3 = raw sums with an optional channel split at a multiple of 16 (single-pass dgrad of a concat layer); 4 = fp32 planar
+// (B, Cout, D, H, W) output of the first a.Cout channels, optional bias, LeakyReLU iff slope >= 0 (the flow head, the
+// image dgrad).  1, 2 and 4 exist for KD = 1 as well (kd-folded layers, 2-D models), for up to 32 outputs.
 // OP: the bf16 outputs and the mask are one channel block of a wider tensor (pitch a.opitch, no out2); the channel-blocked
 // execution of the layers whose weights do not fit shared memory in one piece (64 -> 64, 128 -> 64, ...).
 // PD: polyphase forms of a layer that reads a nearest-x2 upsampled source (3-D, EPI != 0).  Along each axis the upsampled
@@ -85,6 +91,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
   static_assert(PD == 0 || (KD == 3 && EPI != 0 && !ACC && !OP), "polyphase forms: 3-D, specialised epilogue");
   static_assert(PD != 1 || G1 > 0, "the polyphase forward merges channel group 0 and keeps group 1");
   static_assert(PD != 2 || (G1 == 0 && COUT == 32 && HT == 8 && EPI == 2), "the coarse dgrad: 32 -> 32 channels, 8-row tiles");
+  static_assert(EPI != 4 || (PD == 0 && !ACC && !OP && COUT <= 32), "the fp32 planar epilogue drains in the fragment layout");
+  static_assert(KD == 3 || EPI == 0 || (EPI != 3 && COUT <= 32), "KD = 1: fragment-layout epilogues 1, 2, 4 only");
   constexpr int SROWS = (HT + 2) * WT;
   constexpr int NH = PD == 2 ? 1 : HT / 4;                // tile events per slab step (PD 2: 4 coarse rows = 128 rows)
   constexpr int NEVEN = (HT + 3) / 2;                     // PD 2: even slab rows, staged first
@@ -226,6 +234,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
     // wgmma chain of sub-tile `sub` of tile half hb of the step whose kd window starts at ring slot `hslot`; `par`: parity
     // of the output slice (PD 1)
     constexpr int NKD = PD == 2 ? 4 : KD;            // slabs of the kd window
+    // (issues and commits the chain; the caller waits for it)
     auto mma = [&](uint32_t hslot, int hb, int sub, float (&acc)[NF][NN / 2], int par) {
       uint64_t adesc0_kd[NKD], adesc1_kd[NKD];
       uint32_t sl = hslot;
@@ -264,7 +273,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         }
       }
       wg_commit();
-      wg_wait<0>();
     };
     // columns [c, c + 16) of the chain's accumulators in row form (see chan for the 16 this thread receives)
     auto readout = [&](float (&acc)[NF][NN / 2], int c, uint32_t (&r)[16]) {
@@ -318,6 +326,21 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
       constexpr int XPAIR = NF * 2 * COUT;                       // floats per warp pair and buffer half: P0 of 15, P2 of 16
       static_assert(2 * 2 * XPAIR <= ACC_STAGE_FLOATS, "seam exchange fits the stage buffer");
       uint32_t xpar = 0;
+      // Ordered hand-off of the tensor pipe (fragment drain): group g issues the chain of its tile event e only after the
+      // other group has issued event e - 1 (named barrier 7 + g, 256 threads: the waiting group's bar.sync and the other
+      // group's bar.arrive right after its wg_commit).  Issued in event order, the chains complete in event order, so one
+      // group drains while the other's chain is on the tensor pipe instead of both draining at once.  Group 1 opens the
+      // first turn; a group arrives after event e only if event e + 1 exists, so every barrier phase gets exactly one
+      // arrival and one sync (the next arrival on a barrier needs a turn that only its completion grants).
+      constexpr bool ORD = !ROWS;
+      [[maybe_unused]] uint32_t nev = 0;                         // tile events of this CTA
+      if constexpr (ORD) {
+        for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
+          const int d0 = ((item / HW_tiles) % a.nchunks) * a.dchunk;
+          nev += (uint32_t)(min(d0 + a.dchunk, Dout) - d0) * NH;
+        }
+        if (grp == 1) named_bar_arrive(7, 256);                 // (event 0 exists: every CTA has an item)
+      }
       for (int item = blockIdx.x; item < a.nitems; item += gridDim.x) {
         const int wt = item % a.tiles_w, ht = (item / a.tiles_w) % a.tiles_h;
         const int ch = (item / HW_tiles) % a.nchunks, b = item / (HW_tiles * a.nchunks);
@@ -336,6 +359,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
               if (wp + 8 * i >= 1 && wp + 8 * i <= WUSE && w + 8 * i < a.W && hbase + 4 * hb + 2 * blk < Ho)
                 okm |= 1u << (4 * hb + 2 * blk + i);
         size_t vbase = (((size_t)b * Dout + d0) * Ho + hbase) * Wo + (size_t)(long long)w;
+        // EPI 4: channel c of voxel v (channels-last index) sits at v + (b (Cout - 1) + c) D H W in the planar output
+        [[maybe_unused]] const size_t DHWp = (size_t)Dout * HWp, pbase = (size_t)b * (a.Cout - 1) * DHWp;
         for (int j = 0; j < nd; ++j) {
           const uint32_t js = PD == 2 ? 2u * j : (uint32_t)j;   // ring index of the window's first slab
           observe(cnt_base + js + (PD == 2 ? 3u : (KD == 3 ? 2u : 0u)));
@@ -377,7 +402,11 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                   if (rvalid) ld_global_nc_v8(a.mask + rvox * COUT + chan(i), mrow[i]);
               }
               float acc[NF][NN / 2];
+              [[maybe_unused]] const uint32_t e = ecnt - 1;      // this tile event
+              if constexpr (ORD) named_bar(7 + grp, 256);        // event e - 1 is issued
               mma(hslot, hb, sub, acc, (d0 + j) & 1);
+              if (ORD && e + 1 < nev) named_bar_arrive(8 - grp, 256);   // event e + 1 may issue
+              wg_wait<0>();
               if constexpr (ROWS) {
                 const bool valid = rvalid;
                 const size_t vox = rvox;
@@ -440,6 +469,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                 if constexpr (COUT != 16) load_mask(f);
 #pragma unroll
                 for (int jj = 0; jj < COUT / 8; ++jj) {
+                  if (EPI == 4 && 8 * jj >= a.Cout) break;       // (uniform) no real channel from here on
                   const int c0 = 8 * jj + 2 * p;
                   float v[2][2];                                 // [i][e]: channel c0 + e of column w' + 8 i
 #pragma unroll
@@ -468,12 +498,33 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
                         const float x = v[i][e] + (a.bias ? __ldg(a.bias + c0 + e) : 0.f);
                         v[i][e] = fmaxf(x, x * slope);           // LeakyReLU for 0 <= slope <= 1
                       }
-                    } else if constexpr (EPI == 2) {             // sign bits of the saved bf16 activations
+                    } else if constexpr (EPI == 2 && KD == 3) {  // sign bits of the saved bf16 activations
                       const uint32_t mw = mreg[f][i][jj];
                       if (mw & 0x8000u) v[i][0] *= slope;
                       if (mw & 0x80000000u) v[i][1] *= slope;
+                    } else if constexpr (EPI == 2) {
+                      // KD = 1 keeps the generic epilogue's arithmetic: + 0 (no bias), then the derivative where the saved
+                      // bf16 activation compares below zero (a saved -0.0 or NaN does not)
+                      const uint32_t mw = mreg[f][i][jj];
+                      v[i][0] += 0.f;
+                      v[i][1] += 0.f;
+                      if (__uint_as_float(mw << 16) < 0.f) v[i][0] *= slope;
+                      if (__uint_as_float(mw & 0xffff0000u) < 0.f) v[i][1] *= slope;
+                    } else if constexpr (EPI == 4) {
+#pragma unroll
+                      for (int e = 0; e < 2; ++e) {
+                        float x = v[i][e] + (a.bias && c0 + e < a.Cout ? __ldg(a.bias + c0 + e) : 0.f);
+                        if (slope >= 0.f) x = x >= 0.f ? x : x * slope;
+                        v[i][e] = x;
+                      }
                     }
-                    if (okm >> (4 * hb + 2 * blk + i) & 1u) {
+                    if constexpr (EPI == 4) {
+                      if (okm >> (4 * hb + 2 * blk + i) & 1u) {
+                        float* o = reinterpret_cast<float*>(a.out) + vox_of(blk, i) + pbase + (size_t)c0 * DHWp;
+                        if (c0 < a.Cout) o[0] = v[i][0];
+                        if (c0 + 1 < a.Cout) o[DHWp] = v[i][1];
+                      }
+                    } else if (okm >> (4 * hb + 2 * blk + i) & 1u) {
                       const size_t vox = vox_of(blk, i);
                       __nv_bfloat16* dst = (EPI == 3 && c0 >= c1) ? reinterpret_cast<__nv_bfloat16*>(a.out2) + vox * (COUT - c1) + (c0 - c1)
                                                                   : reinterpret_cast<__nv_bfloat16*>(a.out) + vox * (OP ? a.opitch : c1) + c0;
@@ -527,6 +578,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) conv_tcs_kernel(const __grid_cons
         const int c1 = a.out2 ? a.csplit : a.Cout;          // channels [0,c1) -> out, [c1,Cout) -> out2
         float acc[NF][NN / 2];
         mma(hslot, hb, sub, acc, 0);
+        wg_wait<0>();
         // 16 output channels at a time: the kw = 0, 1, 2 partial sums, shuffle-combined across lanes, stored
 #pragma unroll
         for (int i = 0; i < NCH; ++i) {
@@ -1007,14 +1059,17 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   cudaStream_t st = as_stream(stream);
   if (poly != 2 && plan_tma(a, g0, g1, HTv) != 0) return VXM_ERR_CUDA;   // (the coarse dgrad permutes its slab rows)
   const bool acc_epi = acc_in != nullptr || out_mode >= 2;
-  // epilogue specialisation: 3-D, bf16 channels-last output, every padded channel real
+  // epilogue specialisation: bf16 channels-last output with every padded channel real (EPI 1-3; KD = 1: 1 and 2, up to
+  // 32 outputs), or the fp32 planar output (EPI 4, up to 32 padded outputs, one 16- or 32-channel input group)
   int epi = 0;
   {
     const char* e = getenv("VXM_B200_TCS_EPI");       // "0": generic epilogue everywhere (A/B switch)
-    const bool plain = kd == 3 && out_mode == 0 && !acc_epi && Cout == coutp && !(e && e[0] == '0');
+    const bool spec = !acc_epi && !(e && e[0] == '0');
+    const bool plain = spec && out_mode == 0 && Cout == coutp && (kd == 3 || coutp <= 32);
     if (plain && !out2 && !mask && slope >= 0.f && slope <= 1.f) epi = 1;
     else if (plain && !out2 && mask && !bias) epi = 2;
-    else if (plain && !mask && !bias && slope < 0.f && (!out2 || csplit % 16 == 0)) epi = 3;
+    else if (plain && kd == 3 && !mask && !bias && slope < 0.f && (!out2 || csplit % 16 == 0)) epi = 3;
+    else if (spec && out_mode == 1 && !out2 && coutp <= 32 && g0 <= 32 && g1 == 0) epi = 4;
     if (poly) epi = poly;               // the polyphase forms exist with their specialised epilogue only
   }
 #define VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, ACC_, E_, ...)                                                                  \
@@ -1031,12 +1086,17 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
     else if (epi == 3) VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 3, true);                                                      \
     else VXM_TCS_LAUNCH_E(3, G0_, G1_, 32, 4, false, 0, true);                                                                    \
   } while (0)
+// which specialised instantiations exist (the others' dead branches name the generic one): EPI 1 / 2 with KD = 1 up to 32
+// outputs, EPI 4 up to 32 outputs over one 16- or 32-channel group
+#define VXM_TCS_KD1(KD_, CO_) ((KD_) == 3 || (CO_) <= 32)
+#define VXM_TCS_PL(G0_, G1_, CO_) ((CO_) <= 32 && (G0_) <= 32 && (G1_) == 0)
 #define VXM_TCS_LAUNCH(KD_, G0_, G1_, CO_, HT_)                                                                                   \
   do {                                                                                                                            \
     if (acc_epi) VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, true, 0);                                                              \
-    else if (KD_ == 3 && epi == 1) VXM_TCS_LAUNCH_E(3, G0_, G1_, CO_, HT_, false, 1);                                             \
-    else if (KD_ == 3 && epi == 2) VXM_TCS_LAUNCH_E(3, G0_, G1_, CO_, HT_, false, 2);                                             \
+    else if (VXM_TCS_KD1(KD_, CO_) && epi == 1) VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, false, VXM_TCS_KD1(KD_, CO_) ? 1 : 0);  \
+    else if (VXM_TCS_KD1(KD_, CO_) && epi == 2) VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, false, VXM_TCS_KD1(KD_, CO_) ? 2 : 0);  \
     else if (KD_ == 3 && epi == 3) VXM_TCS_LAUNCH_E(3, G0_, G1_, CO_, HT_, false, 3);                                             \
+    else if (VXM_TCS_PL(G0_, G1_, CO_) && epi == 4) VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, false, VXM_TCS_PL(G0_, G1_, CO_) ? 4 : 0); \
     else VXM_TCS_LAUNCH_E(KD_, G0_, G1_, CO_, HT_, false, 0);                                                                     \
   } while (0)
 #define VXM_TCS_G8(KD_, CO_)                                                  \
