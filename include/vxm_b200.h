@@ -405,6 +405,28 @@ int vxm_pheno_decoder_bwd(const float* grad_out, const float* pheno, const float
                           float* grad_W, float* grad_bias, float* grad_like_w, float* grad_like_b, void* work, int B, int P,
                           int F, size_t V, int accumulate, void* stream);
 
+/* ---- HyperMorph (reference voxelmorph/tf/networks.py:1192-1231): the hypernetwork and the U-Net weights it generates ----
+ * Hypernetwork: hyp (P), nb_layers Dense layers of U units with ReLU, weights in torch.nn.Linear's (out, in) layout:
+ * weights[0] (U, P), weights[l > 0] (U, U), biases[l] (U).  `weights`, `biases`, `grad_weights` and `grad_biases` are
+ * HOST arrays of nb_layers device pointers.  1 <= P <= 16, 1 <= U <= 256, 1 <= nb_layers <= 8.
+ *   pre (nb_layers, U): every layer's pre-activation (kept for the backward),  h (U) = relu(pre[nb_layers - 1])
+ * The backward turns grad_h (U) into the gradient of every weight and bias (TF's ReluGrad: pre > 0); none for hyp.
+ * Generated weights: A (U, N) row-major, a (N), W (N), all fp32 device memory:
+ *   W[j] = a[j] + sum_k h[k] A[k,j]                                                         (W overwritten)
+ *   grad_A[k,j] = h[k] grad_W[j],  grad_a[j] = grad_W[j],  grad_h[k] = sum_j A[k,j] grad_W[j]  (grad_h overwritten)
+ * accumulate = 1 adds the parameter gradients to their buffers (a rounded product, then a rounded sum: what autograd's
+ * accumulation computes), 0 overwrites them.  Sums run in a fixed order: results are bit-reproducible.  work:
+ * vxm_hyper_workspace_bytes(U, N) bytes of scratch (no initial value needed); 0 for sizes the kernels refuse. */
+size_t vxm_hyper_workspace_bytes(int U, size_t N);
+int vxm_hyper_mlp_fwd(const float* hyp, const float* const* weights, const float* const* biases, float* pre, float* h,
+                      int P, int U, int nb_layers, void* stream);
+int vxm_hyper_mlp_bwd(const float* grad_h, const float* hyp, const float* const* weights, const float* pre,
+                      float* const* grad_weights, float* const* grad_biases, int P, int U, int nb_layers, int accumulate,
+                      void* stream);
+int vxm_hyper_weights_fwd(const float* h, const float* A, const float* a, float* W, int U, size_t N, void* stream);
+int vxm_hyper_weights_bwd(const float* h, const float* A, const float* grad_W, float* grad_A, float* grad_a,
+                          float* grad_h, void* work, int U, size_t N, int accumulate, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -107,6 +107,11 @@ SIGNATURES = {
     "vxm_pheno_decoder_workspace_bytes": (c_sz, [c_i]),
     "vxm_pheno_decoder_fwd": (c_i, [c_f] * 6 + [c_i, c_i, c_i, c_sz, c_f]),
     "vxm_pheno_decoder_bwd": (c_i, [c_f] * 10 + [c_i, c_i, c_i, c_sz, c_i, c_f]),
+    "vxm_hyper_workspace_bytes": (c_sz, [c_i, c_sz]),
+    "vxm_hyper_mlp_fwd": (c_i, [c_f] * 5 + [c_i, c_i, c_i, c_f]),
+    "vxm_hyper_mlp_bwd": (c_i, [c_f] * 6 + [c_i, c_i, c_i, c_i, c_f]),
+    "vxm_hyper_weights_fwd": (c_i, [c_f] * 4 + [c_i, c_sz, c_f]),
+    "vxm_hyper_weights_bwd": (c_i, [c_f] * 7 + [c_i, c_sz, c_i, c_f]),
 }
 
 _lib = None

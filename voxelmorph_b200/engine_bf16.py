@@ -5,7 +5,9 @@
 channels-last bf16 glue kernels: every activation between the fp32 input images and the fp32 flow field is a
 bf16 (B,D,H,W,C) tensor, the concat / upsample / bias / LeakyReLU / LeakyReLU-derivative are fused into the
 convolution kernels, and the backward pass (dgrad, wgrad, pooling and skip routing) is written out by hand —
-torch autograd only sees one node.  Parameters stay the module's own fp32 `nn.Parameter`s.
+torch autograd only sees one node.  Parameters stay the module's own fp32 `nn.Parameter`s, except in a model whose U-Net
+weights are generated (HyperVxmDense): its convolutions hold plain views of one persistent flat buffer, and the backward
+returns their gradient as one flat tensor of the same layout.
 """
 import torch
 
@@ -69,7 +71,10 @@ def _walk(model):
         nonlocal cur, pending_up
         L = _Layer()
         L.w, L.bias, L.slope, L.role = m.weight, m.bias, slope, role
-        L.srcs = (m.weight,) if extra is None else (m.weight, m.bias, extra.weight, extra.bias)
+        if not isinstance(m.weight, torch.nn.Parameter):
+            # a generated weight (a view of the model's flat buffer): the plan keeps no autograd history of it
+            L.w, L.bias = m.weight.detach(), m.bias.detach()
+        L.srcs = (L.w,) if extra is None else (m.weight, m.bias, extra.weight, extra.bias)
         # a convolution after an upsample reads the upsampled previous output, then the skip (a fused upsample + concat)
         L.a, L.b = pending_up if pending_up is not None else (cur, None)
         L.up, pending_up = pending_up is not None, None
@@ -183,6 +188,7 @@ class _Plan:
         self.ptrs = self.weight_ptrs()
         self.stamps = [None, None]
         self.img_table, self.img_stamp = None, None
+        self.gen_ptr = None               # the generated weights' buffer (_plan_of)
 
     def weight_ptrs(self):
         return tuple(p.data_ptr() for L in self.layers for p in L.srcs)
@@ -220,12 +226,16 @@ class _Plan:
         return self.img_table.packs[0]
 
 
-def _plan_of(model, split):
+def _plan_of(model, split, generated=None):
     """The model's plan with its operands refreshed (built lazily; rebuilt when the parameters moved, e.g. after
-    .to(device) or FlatParams)."""
+    .to(device) or FlatParams, or when `generated`, the flat buffer the U-Net's weights are views of, did).  The
+    refresh stamp counts bump_weights_epoch calls, which the weight generation makes: generated weights repack on every
+    step, and a captured step records the pack launch."""
     plan = model.__dict__.get("_vxm_pack_plan")
-    if plan is None or plan.ptrs != plan.weight_ptrs():
+    gen_ptr = None if generated is None else generated.data_ptr()
+    if plan is None or plan.ptrs != plan.weight_ptrs() or plan.gen_ptr != gen_ptr:
         plan = _Plan(model)
+        plan.gen_ptr = gen_ptr
         object.__setattr__(model, "_vxm_pack_plan", plan)
     plan.refresh(split)
     return plan
@@ -289,16 +299,17 @@ def _flat_grads(L):
                for p in (L.w, L.bias) if p is not None)
 
 
-def forward_tape(model, source, target, split=False):
+def forward_tape(model, source, target, split=False, generated=None):
     """Runs Unet + flow head, returns (flow fp32 (B,nd,*vol), tape).  `split`: split-precision (bf16x3) forward — every
     activation is a (hi, lo) bf16 pair and every layer three tensor-core passes; the tape keeps the hi parts, which is
     what the (bf16-operand) backward reads, and the lo parts of the pool inputs, so that the backward routes each pool
-    gradient to the child the pool chose on hi + lo."""
+    gradient to the child the pool chose on hi + lo.  `generated`: the flat buffer the U-Net's weights are views of
+    (HyperVxmDense), whose gradient backward_tape then returns under the key "generated"."""
     nd = source.dim() - 2
     kd = 3 if nd == 3 else 1
     _lib.require_cuda(source, target, what="VxmDense")
     source, target = _lib.contig(source), _lib.contig(target)
-    plan = _plan_of(model, split)
+    plan = _plan_of(model, split, generated)
     planes = [source[:, i:i + 1] for i in range(source.shape[1])] + [target[:, i:i + 1] for i in range(target.shape[1])]
     first = plan.layers[0]
     if nd != plan.nd or len(planes) != first.cin:
@@ -336,7 +347,8 @@ def forward_tape(model, source, target, split=False):
             tensors[L.out] = out
     if nd == 2:
         flow = flow.squeeze(2)
-    return flow, dict(plan=plan, tensors=tensors, split=split, pool_lows=pool_lows)
+    return flow, dict(plan=plan, tensors=tensors, split=split, pool_lows=pool_lows,
+                      generated=None if generated is None else generated.detach())
 
 
 def backward_tape(ctx, g_flow, image_grad=False):
@@ -357,6 +369,15 @@ def backward_tape(ctx, g_flow, image_grad=False):
     grads = {}
     folded = []   # (layer, gw2d, gb2d): 2-D weight gradients of the kd-folded layers, mapped back after the flush
     heads = []    # (layer, gw, gb): weight gradient of a 2 nd-output head, split between its modules after the flush
+    base = ctx.get("generated")
+    dW = None if base is None else torch.zeros(base.numel(), dtype=torch.float32, device=dev)
+    gen = {}      # layer -> (weight, bias) views of dW at the layer's place in the generated layout
+    if dW is not None:
+        for L in plan.layers:
+            if L.role != "flow":
+                ow, ob = [(t.data_ptr() - base.data_ptr()) // base.element_size() for t in (L.w, L.bias)]
+                gen[L] = (dW[ow:ow + L.w.numel()].view(L.w.shape), dW[ob:ob + L.cout])
+        grads["generated"] = dW
     for L in reversed(plan.ops):
         if not isinstance(L, _Layer):
             _, src, dst = L
@@ -385,6 +406,9 @@ def backward_tape(ctx, g_flow, image_grad=False):
             else:
                 batch.add(xa, None, g_in, gwf, gbf, 3 * L.cin, L.cout, 1, False, False)
             folded.append((L, gwf, gbf))
+        elif L in gen:
+            # generated weights: accumulated into the zeroed flat gradient at their own place, no per-layer tensors
+            tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, out_w=gen[L][0], out_b=gen[L][1], batch=batch)
         elif len(L.srcs) > 1:
             heads.append((L,) + tc.conv_wgrad(xa, xb, g_in, L.cin, L.cout, kd, up=L.up, batch=batch))
         elif _flat_grads(L):
@@ -420,7 +444,10 @@ def backward_tape(ctx, g_flow, image_grad=False):
     batch.flush()     # one launch reduces every layer's per-CTA partials (fixed order: deterministic)
     for L, gwf, gbf in folded:
         gw, gb = (unfold_grad_first(gwf, L.cout, L.cin), gbf) if L.role == "first" else unfold_grad_flow(gwf, gbf, nd, L.cin)
-        if _flat_grads(L):
+        if L in gen:
+            gen[L][0].add_(gw)
+            gen[L][1].add_(gb)
+        elif _flat_grads(L):
             L.w.grad.add_(gw)
             if L.bias is not None:
                 L.bias.grad.add_(gb)
@@ -482,8 +509,8 @@ def unfold_grad_flow(gwf, gbf, nd, cin):
 
 class _UnetFlowFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, model, source, target, split, *params):
-        flow, tape = forward_tape(model, source, target, split=split)
+    def forward(ctx, model, source, target, split, generated, *params):
+        flow, tape = forward_tape(model, source, target, split=split, generated=generated)
         ctx.tape = tape
         ctx.params = params
         ctx.model_ref = model
@@ -508,14 +535,15 @@ class _UnetFlowFn(torch.autograd.Function):
                 g_source = g_img[:, :ctx.src_feats]
             if ctx.image_grads[1]:
                 g_target = g_img[:, ctx.src_feats:]
-        return (None, g_source, g_target, None) + tuple(grads.get(p) for p in ctx.params)
+        return (None, g_source, g_target, None, grads.get("generated")) + tuple(grads.get(p) for p in ctx.params)
 
 
-def unet_flow(model, source, target, split=False):
+def unet_flow(model, source, target, split=False, generated=None):
     """flow = model.flow(model.unet_model(cat(source, target))) on the tensor-core engine (for a model with `log_sigma`:
     cat(flow(x), log_sigma(x)), the probabilistic model's flow_params).  split=False: bf16 operands
     (throughput mode); split=True: bf16x3 split precision in the forward (flow within 1e-4 of the fp32 reference), the
-    backward uses bf16 operands in both modes."""
+    backward uses bf16 operands in both modes.  `generated` (HyperVxmDense): the flat tensor the U-Net's weights are
+    views of; its gradient is formed as one flat tensor of the same layout."""
     head = [model.flow] + ([model.log_sigma] if hasattr(model, "log_sigma") else [])
     params = list(model.unet_model.parameters()) + [p for m in head for p in m.parameters()]
-    return _UnetFlowFn.apply(model, source, target, bool(split), *params)
+    return _UnetFlowFn.apply(model, source, target, bool(split), generated, *params)

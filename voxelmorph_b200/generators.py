@@ -26,7 +26,7 @@ from collections import OrderedDict
 import numpy as np
 
 __all__ = ["VolumeCache", "load_volfile", "volgen", "scan_to_scan", "scan_to_atlas", "semisupervised", "template_creation",
-           "conditional_template_creation", "Prefetcher"]
+           "conditional_template_creation", "hypermorph", "Prefetcher"]
 
 
 def _cuda_ready():
@@ -398,3 +398,17 @@ class Prefetcher:
 
     def close(self):
         self._stop.set()
+
+
+def hypermorph(base_generator, oversample_rate=0.2):
+    """HyperMorph's hyperparameter extension of any generator (reference scripts/tf/train_hypermorph.py:107-121): yields
+    ((*inputs, hyp), outputs) for every (inputs, outputs) of `base_generator`, hyp of shape (1, 1) float32.  lambda is
+    drawn as the script's random_hyperparam draws it — np.random.rand() < oversample_rate picks np.random.choice([0, 1]),
+    otherwise np.random.rand() — before next(base_generator).  The draw is made once per batch, not once per batch entry
+    as in the script: HyperVxmDense takes one lambda per step, shared by the batch.  At batch size 1 (the script's
+    default) the sequence of np.random draws is the script's."""
+    while True:
+        lam = np.random.choice([0, 1]) if np.random.rand() < oversample_rate else np.random.rand()
+        hyp = np.full((1, 1), lam, dtype=np.float32)
+        inputs, outputs = next(base_generator)
+        yield (tuple(inputs) + (hyp,), outputs)

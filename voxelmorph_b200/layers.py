@@ -418,3 +418,137 @@ class PhenoDecoder(nn.Module):
 
     def forward(self, pheno):
         return _PhenoDecoderFn.apply(pheno, self.weight, self.bias, self.like_weight, self.like_bias)
+
+
+def _ptr_array(tensors):
+    """A host array of device pointers (the hypernetwork entry points take one per layer)."""
+    import ctypes
+    arr = (ctypes.c_void_p * len(tensors))(*[t.data_ptr() for t in tensors])
+    return arr, ctypes.cast(arr, ctypes.c_void_p)
+
+
+class _HyperWeightsFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, hyp, out, kernel, bias, *mlp):
+        _lib.require_cuda(hyp, out, kernel, bias, *mlp, what="HyperWeights")
+        U, N = kernel.shape
+        L = len(mlp) // 2
+        P = mlp[0].shape[1]
+        if tuple(hyp.shape) != (1, P):
+            raise _lib.VxmError("HyperWeights: hyp must have shape (1, %d) — one set of hyperparameters per step, shared by "
+                                "every image of the batch; got %s" % (P, tuple(hyp.shape)))
+        if not all(t.is_contiguous() for t in (out, kernel, bias) + mlp) or tuple(bias.shape) != (N,) \
+                or tuple(out.shape) != (N,):
+            raise _lib.VxmError("HyperWeights: the parameters must be contiguous, hyper_kernel (U, N), hyper_bias and the "
+                                "generated buffer (N,)")
+        hyp = _lib.contig(hyp)
+        lib = _lib.load()
+        pre = torch.empty((L, U), dtype=torch.float32, device=hyp.device)
+        h = torch.empty(U, dtype=torch.float32, device=hyp.device)
+        wa, wp = _ptr_array(mlp[0::2])
+        ba, bp = _ptr_array(mlp[1::2])
+        _lib.check(lib.vxm_hyper_mlp_fwd(_lib.ptr(hyp), wp, bp, _lib.ptr(pre), _lib.ptr(h), P, U, L, _lib.stream_ptr()),
+                   "vxm_hyper_mlp_fwd")
+        _lib.check(lib.vxm_hyper_weights_fwd(_lib.ptr(h), _lib.ptr(kernel), _lib.ptr(bias), _lib.ptr(out), U, N,
+                                             _lib.stream_ptr()), "vxm_hyper_weights_fwd")
+        # the U-Net's weights changed behind torch's version counters: the tensor-core engine's packed copies refresh
+        from . import engine_bf16
+        engine_bf16.bump_weights_epoch()
+        ctx.save_for_backward(hyp, pre, h, kernel, bias, *mlp)
+        ctx.cfg = (P, U, L, N)
+        return out.detach()
+
+    @staticmethod
+    def backward(ctx, dW):
+        hyp, pre, h, kernel, bias, *mlp = ctx.saved_tensors
+        P, U, L, N = ctx.cfg
+        dW = _lib.contig(dW)
+        params = [kernel, bias] + mlp
+        flat = [_flat_grad(p) for p in params]
+        # as PhenoDecoder: straight into FusedAdam's flat buffer when every parameter has its view there (autograd then
+        # receives none), otherwise fresh tensors for autograd to accumulate
+        accumulate = all(g is not None for g in flat)
+        outs = flat if accumulate else [torch.empty_like(p) for p in params]
+        lib = _lib.load()
+        dh = torch.empty(U, dtype=torch.float32, device=dW.device)
+        work = torch.empty(int(lib.vxm_hyper_workspace_bytes(U, N)), dtype=torch.uint8, device=dW.device)
+        _lib.check(lib.vxm_hyper_weights_bwd(_lib.ptr(h), _lib.ptr(kernel), _lib.ptr(dW), _lib.ptr(outs[0]), _lib.ptr(outs[1]),
+                                             _lib.ptr(dh), _lib.ptr(work), U, N, int(accumulate), _lib.stream_ptr()),
+                   "vxm_hyper_weights_bwd")
+        wa, wp = _ptr_array(mlp[0::2])
+        ga, gp = _ptr_array(outs[2::2])
+        gba, gbp = _ptr_array(outs[3::2])
+        _lib.check(lib.vxm_hyper_mlp_bwd(_lib.ptr(dh), _lib.ptr(hyp), wp, _lib.ptr(pre), gp, gbp, P, U, L, int(accumulate),
+                                         _lib.stream_ptr()), "vxm_hyper_mlp_bwd")
+        if accumulate:
+            return (None,) * (4 + len(mlp))
+        return (None, None) + tuple(outs)
+
+
+def hyper_layout(shapes):
+    """Offsets of the flat generated layout: [(weight offset, bias offset)] for convolutions of weight shapes `shapes`,
+    each stored as [weight, bias] in the given (execution) order, and the total N."""
+    offs, n = [], 0
+    for s in shapes:
+        k = int(math.prod(s))
+        offs.append((n, n + k))
+        n += k + int(s[0])
+    return offs, n
+
+
+class HyperWeights(nn.Module):
+    """HyperMorph's hypernetwork and the weights it generates (Hoopes et al., IPMI 2021 / MELBA 2022; reference
+    voxelmorph/tf/networks.py:1192-1231 with neurite's HyperConvFromDense).  For hyp (1, P):
+
+        h = relu(Dense_{L-1}(... relu(Dense_0(hyp))))            hypernet.{i}: nn.Linear, U units each
+        Wflat = hyper_bias + h @ hyper_kernel                      hyper_kernel (U, N), hyper_bias (N)
+
+    `shapes` are the generated convolutions' weight shapes in the U-Net's execution order; Wflat holds each as
+    [weight, bias] (hyper_layout), and `views(wflat)` returns them as (weight, bias) tensors.  Wflat is written by the
+    device into one persistent buffer (`wflat`, not a checkpoint entry), so every step's weights sit at the same
+    addresses: the tensor-core engine's packing descriptors and a captured CUDA graph stay valid.  Consequently the
+    generated weights of a forward are valid until the next forward: run a backward before the next forward.
+
+    Initialisation (the package's choice; neurite's HyperConvFromDense initialiser is not restated): the Dense layers as
+    Keras initialises them, glorot-uniform kernels and zero biases; each convolution's block of hyper_kernel
+    glorot-uniform over the fans (U, 27 Cin Cout) for its weight part and (U, Cout) for its bias part; hyper_bias zero.
+
+    Forward and backward are two launches each (csrc/hyper.cu); when every parameter's .grad is a view of FusedAdam's
+    flat buffer the gradients are accumulated there directly.  hyp receives no gradient.  Limits: 1 <= P <= 16,
+    U <= 256, 1 <= nb_layers <= 8."""
+
+    def __init__(self, shapes, nb_hyp_params=1, nb_hyp_layers=6, nb_hyp_units=128):
+        super().__init__()
+        P, L, U = int(nb_hyp_params), int(nb_hyp_layers), int(nb_hyp_units)
+        if not (1 <= P <= 16 and 1 <= U <= 256 and 1 <= L <= 8):
+            raise ValueError("HyperWeights: nb_hyp_params must be 1 to 16, nb_hyp_units 1 to 256 and nb_hyp_layers 1 to 8; "
+                             "got %d, %d, %d" % (P, U, L))
+        self.shapes = [tuple(int(d) for d in s) for s in shapes]
+        self.offsets, N = hyper_layout(self.shapes)
+        self.hypernet = nn.ModuleList()
+        for i in range(L):
+            lin = nn.Linear(P if i == 0 else U, U)
+            lim = math.sqrt(6.0 / (lin.in_features + lin.out_features))
+            with torch.no_grad():
+                lin.weight.uniform_(-lim, lim)
+                lin.bias.zero_()
+            self.hypernet.append(lin)
+        kernel = torch.empty(U, N)
+        for s, (ow, ob) in zip(self.shapes, self.offsets):
+            taps = int(math.prod(s[2:]))
+            lim = math.sqrt(6.0 / (U + taps * s[0] * s[1]))
+            kernel[:, ow:ob].uniform_(-lim, lim)
+            lim = math.sqrt(6.0 / (U + s[0]))
+            kernel[:, ob:ob + s[0]].uniform_(-lim, lim)
+        self.hyper_kernel = nn.Parameter(kernel)
+        self.hyper_bias = nn.Parameter(torch.zeros(N))
+        self.register_buffer("wflat", torch.zeros(N), persistent=False)
+
+    def forward(self, hyp):
+        """Wflat (N,) for hyp (1, P), differentiable with respect to every parameter of this module."""
+        mlp = [p for lin in self.hypernet for p in (lin.weight, lin.bias)]
+        return _HyperWeightsFn.apply(hyp, self.wflat, self.hyper_kernel, self.hyper_bias, *mlp)
+
+    def views(self, wflat):
+        """[(weight, bias)] views of a flat layout, in the order of `shapes`."""
+        return [(wflat[ow:ob].view(s), wflat[ob:ob + s[0]]) for s, (ow, ob) in zip(self.shapes, self.offsets)]

@@ -258,3 +258,12 @@ class KL:
             raise _lib.VxmError("KL: flow_vol_shape %s does not match flow_params of spatial shape %s"
                                 % (tuple(self.flow_vol_shape), tuple(y_pred.shape[2:])))
         return _KlFn.apply(y_pred, float(self.prior_lambda))
+
+
+def hyper_loss(hyp, image_loss, reg_loss):
+    """HyperMorph's loss (reference scripts/tf/train_hypermorph.py:159-177): (1 - lam) image_loss + lam reg_loss with
+    lam = hyp[0, 0], formed on the device from the (1, 1) hyp tensor (no host synchronisation, so a captured step takes
+    the lambda of each replay's hyp).  lam receives no gradient.  The script's terms are image_loss = MSE(image_sigma=0.05)
+    or NCC and reg_loss = Grad('l2', loss_mult=int_downsize) of the pre-integration flow."""
+    lam = hyp.detach().reshape(-1)[0]
+    return (1.0 - lam) * image_loss + lam * reg_loss

@@ -549,3 +549,82 @@ class ConditionalTemplateCreation(LoadableModel):
         if self.mean_stream is None:
             return y_source, pos_flow, pos_flow
         return y_source, self.mean_stream(neg_flow), pos_flow, pos_flow
+
+
+class HyperVxmDense(VxmDense):
+    """HyperMorph: VxmDense whose U-Net convolution weights are generated from the regularisation weight(s) by a
+    hypernetwork, so that one model serves every lambda (Hoopes et al., "HyperMorph: Amortized Hyperparameter Learning
+    for Image Registration", IPMI 2021 / MELBA 2022; reference voxelmorph/tf/networks.py:1192-1231, trained by
+    scripts/tf/train_hypermorph.py).  The torch backend of the reference has no such class; this one restates the TF
+    model over this package's VxmDense (zero-fill sampler, int_downsize, torch NCC):
+
+        h = hypernet(hyp)                                 nb_hyp_layers Dense(nb_hyp_units, relu) layers, hyp (1, P)
+        W_l, b_l = views of hyper_bias + h @ hyper_kernel every U-Net convolution (encoder, decoder, remaining), in
+                                                          execution order, each [weight, bias]: layers.HyperWeights
+        the U-Net with those weights (LeakyReLU(0.2) as before), then the flow head — a plain convolution with its own
+        parameters `flow.*` — and VxmDense's integration, resize and warp.
+
+    forward(source, target, hyp, registration=False) returns what VxmDense.forward returns.  One set of hyperparameters
+    per step: hyp must have shape (1, P), and its weights are shared by every image of the batch (the engines' launches
+    take one weight set; at batch size 1, the reference script's default, this is the script's behaviour).  Attach
+    losses.hyper_loss to weigh the image and smoothness terms by lambda.  Parameters: `hyper.hypernet.{i}.weight/bias`,
+    `hyper.hyper_kernel` (U, N), `hyper.hyper_bias` (N) and `flow.*`; the U-Net holds none of its own (N = 326 032 for
+    the default features).  The generated weights live in one persistent buffer: run each forward's backward before the
+    next forward.  use_probs is not implemented.  kwargs are VxmDense's."""
+
+    @store_config_args
+    def __init__(self, inshape, nb_hyp_params=1, nb_hyp_layers=6, nb_hyp_units=128, **kwargs):
+        config = self.config
+        if kwargs.get("use_probs", False):
+            raise NotImplementedError("HyperVxmDense: use_probs (a flow-variance head) is not implemented")
+        super().__init__(inshape, **kwargs)
+        self.config = config             # (VxmDense's decorator recorded its own arguments)
+        unet = self.unet_model
+        self._convs = [blk.main for convs in list(unet.encoder) + list(unet.decoder) for blk in convs] + \
+                      [blk.main for blk in unet.remaining]
+        self.hyper = layers.HyperWeights([tuple(c.weight.shape) for c in self._convs], nb_hyp_params, nb_hyp_layers,
+                                         nb_hyp_units)
+        for c in self._convs:
+            del c.weight, c.bias
+        object.__setattr__(self, "_wflat", None)
+        self._assign(self.hyper.wflat)
+
+    def _apply(self, fn, *args, **kwargs):
+        out = super()._apply(fn, *args, **kwargs)
+        self._assign(self.hyper.wflat)   # the generated buffer moved (.to, .cuda): re-point the U-Net at it
+        return out
+
+    def _assign(self, wflat):
+        """Point every U-Net convolution at its (weight, bias) views of `wflat`."""
+        object.__setattr__(self, "_wflat", wflat)
+        for c, (w, b) in zip(self._convs, self.hyper.views(wflat)):
+            c.weight, c.bias = w, b
+
+    def _head(self, source, target):
+        engine = ops.resolve_engine(self)
+        if engine in ('bf16', 'bf16x3'):
+            from . import engine_bf16
+            return engine_bf16.unet_flow(self, source, target, split=(engine == 'bf16x3'), generated=self._wflat)
+        return super()._head(source, target)
+
+    def forward(self, source, target, hyp, registration=False):
+        P = self.hyper.hypernet[0].in_features
+        if hyp.dim() != 2 or tuple(hyp.shape) != (1, P):
+            raise _lib.VxmError("HyperVxmDense: hyp must have shape (1, %d), one set of hyperparameters per step shared "
+                                "by the whole batch (per-image values are not supported); got %s" % (P, tuple(hyp.shape)))
+        self._maybe_attach_dp()
+        if registration and not self.training and self.registration_no_grad and torch.is_grad_enabled():
+            with torch.no_grad():
+                return self.forward(source, target, hyp, registration=True)
+        self._assign(self.hyper(hyp))
+        try:
+            pos_flow, neg_flow, preint_flow = self.flows(source, target)
+        finally:
+            # back to plain views of the buffer: the module keeps no autograd history from one step to the next (a kept
+            # graph would also keep its AccumulateGrad nodes, bound to the stream they were made on, into a capture)
+            self._assign(self.hyper.wflat)
+        y_source = self.transformer(source, pos_flow)
+        y_target = self.transformer(target, neg_flow) if self.bidir else None
+        if not registration:
+            return (y_source, y_target, preint_flow) if self.bidir else (y_source, preint_flow)
+        return y_source, pos_flow
