@@ -53,8 +53,8 @@ KERNEL_CASES = {
 }
 
 
-def _hyper_module(vxm, cuda, name, seed=0):
-    shapes, P, U, L = KERNEL_CASES[name]
+def _hyper_module(vxm, cuda, name, seed=0, cases=KERNEL_CASES):
+    shapes, P, U, L = cases[name]
     if isinstance(shapes, str):
         shapes = _shapes(vxm, DEFAULT_FEATS if shapes == "default" else WIDE_FEATS)
     torch.manual_seed(seed)
@@ -80,8 +80,13 @@ def _run(mod, hyp, dW):
 @pytest.mark.parametrize("name", sorted(KERNEL_CASES))
 def test_kernels_vs_fp64(vxm, cuda, name):
     mod, hyp, dW = _hyper_module(vxm, cuda, name)
-    got = _run(mod, hyp, dW)
-    P, U, L = KERNEL_CASES[name][1:]
+    check_vs_fp64(mod, hyp, dW, _run(mod, hyp, dW), name)
+
+
+def check_vs_fp64(mod, hyp, dW, got, name):
+    """got = [Wflat, then every parameter's gradient] against fp64 autograd, each within its counted bound"""
+    L = len(mod.hypernet)
+    P, U = mod.hypernet[0].in_features, mod.hypernet[0].out_features
     prm = [p.detach().double().requires_grad_(True) for p in mod.parameters()]
     mlp = [(prm[2 + 2 * i], prm[3 + 2 * i]) for i in range(L)]
     A, a = prm[0], prm[1]
@@ -225,11 +230,22 @@ def _loss(vxm, hyp, outs, T):
 @pytest.mark.parametrize("name", sorted(STEP))
 @pytest.mark.parametrize("eng_name", ["f32", "bf16x3", "bf16"])
 def test_hyper_step_vs_oracle(vxm, cuda, engine, eng_name, name):
+    check_step_vs_oracle(vxm, cuda, engine, eng_name, name)
+
+
+def check_step_vs_oracle(vxm, cuda, engine, eng_name, name, flat=False):
+    """One step's flow, moved image, loss and every parameter gradient against fp64 autograd (STEP_TOL), then the
+    registration form.  flat: the parameters are FusedAdam's views, zeroed, as in training — the gradients are read from
+    the flat buffer.  Returns the model and the optimizer (None unless flat)."""
     engine(eng_name)
     kw = STEP[name]
     model, cfg = _hyper_model(vxm, kw)
     sd = {k: v.clone() for k, v in model.state_dict().items()}
     model = model.to(cuda).train()
+    opt = None
+    if flat:
+        opt = vxm.optim.FusedAdam(model.parameters(), lr=1e-3)
+        opt.zero_grad()
     s, tr = cases.volume_pair(41, kw["inshape"], sigma=1.5)
     S_c, T_c = t(s), t(tr)
     hyp = torch.tensor([[0.3]])
@@ -262,6 +278,7 @@ def test_hyper_step_vs_oracle(vxm, cuda, engine, eng_name, name):
     e_reg, e_pos = relmax(y_reg.cpu(), reg[0]), relmax(pos.cpu(), reg[1])
     print("[hyper registration %s %s] moved %.2e pos_flow %.2e" % (eng_name, name, e_reg, e_pos))
     assert e_reg <= tol["moved"] and e_pos <= tol["fp"]
+    return model, opt
 
 
 def test_two_lambdas_give_different_flows(vxm, cuda, engine):

@@ -79,12 +79,15 @@ UNETS = {
     "probs": ("VxmDenseProbabilistic", dict(inshape=(96, 128, 160)), 1),
     "probs_2d": ("VxmDenseProbabilistic", dict(inshape=(192, 224)), 8),
     "template": ("TemplateCreation", dict(inshape=(96, 128, 160)), 1),
+    "hyper": ("HyperVxmDense", dict(inshape=(96, 128, 160)), 1),
+    "hyper_2d": ("HyperVxmDense", dict(inshape=(192, 224)), 8),
 }
 
 
 def _unet_run(vxm, cuda, name):
     """a fresh model (fixed weights, a head of ordinary size), its U-Net and head on images that ask for their gradient,
-    backward with a fixed flow gradient: [flow, every parameter's gradient, the source image's gradient]"""
+    backward with a fixed flow gradient: [flow, every parameter's gradient, the source image's gradient].  A
+    HyperVxmDense's parameters include the hypernetwork's, reached through the generated weights' flat gradient."""
     cls, kw, B = UNETS[name]
     torch.manual_seed(3)
     model = getattr(vxm.networks, cls)(**kw)
@@ -98,6 +101,8 @@ def _unet_run(vxm, cuda, name):
     planes = net.unet_model.encoder[0][0].main.in_channels
     S = torch.rand((B, 1) + kw["inshape"], generator=g, device=cuda).requires_grad_(True)
     T = torch.rand((B, planes - 1) + kw["inshape"], generator=g, device=cuda)
+    if cls == "HyperVxmDense":            # the generated weights (hypernetwork and weight generation) for one lambda
+        net._assign(net.hyper(torch.tensor([[0.4]], device=cuda)))
     out = net._head(S, T)
     out.backward(torch.randn(out.shape, generator=g, device=cuda))
     torch.cuda.synchronize()
@@ -255,6 +260,25 @@ def k_decoder(vxm, g):
     return out + [fp.grad.clone()], []
 
 
+def k_hyper(vxm, g):
+    """the hypernetwork and weight generation forward (pre, h and the generated buffer), the backward into fresh tensors
+    (autograd; dh and its partial workspace) and into FusedAdam's flat views behind a 1-float pad (unaligned, 4-byte
+    loads; 16-byte loads for the fresh tensors, N = 14 736), U = 37 (the unrolled rows' tail)"""
+    mod = vxm.layers.HyperWeights([(16, 2, 3, 3, 3), (32, 16, 3, 3, 3)], 3, 4, 37).to(g.device)
+    with torch.no_grad():
+        for p in mod.parameters():
+            p.copy_(_randn(g, p.shape, 0.3))
+    hyp, gout = _rand(g, (1, 3)), _randn(g, mod.hyper_bias.shape)
+    w = mod(hyp)
+    out = [w.detach().clone()]
+    w.backward(gout)
+    out += [p.grad for p in mod.parameters()]
+    fp = vxm.optim.FlatParams([torch.nn.Parameter(torch.zeros(1, device=g.device))] + list(mod.parameters()))
+    fp.zero_grad()
+    mod(hyp).backward(gout)
+    return out + [fp.grad.clone()], []
+
+
 def k_jacdet(vxm, g):
     out = []
     for shape in ((2, 3, 40, 48, 56), (8, 2, 96, 112)):
@@ -268,7 +292,7 @@ KERNELS = {
     "ncc9": lambda vxm, g: k_ncc(vxm, g, [((1, 1, 80, 96, 112), None), ((8, 1, 96, 112), None)]),
     "ncc_generic": lambda vxm, g: k_ncc(vxm, g, [((2, 1, 45, 70, 121), (5, 9, 7)), ((3, 1, 64, 80), (5, 5))]),
     "grad": k_grad, "mse": k_mse, "dice": k_dice, "kl": k_kl, "sampler": k_sampler, "mean_stream": k_mean_stream,
-    "decoder": k_decoder, "jacdet": k_jacdet,
+    "decoder": k_decoder, "jacdet": k_jacdet, "hyper": k_hyper,
 }
 # the VecInt and warp backwards scatter with atomics, so two runs differ in the last bits: each is within 1e-5 of the fp64
 # adjoint in its own test (test_gpu_fp32_step_kernels.py, test_gpu_fp32_other_paths.py), so two runs within twice that
@@ -314,6 +338,8 @@ def _step(vxm, cuda, family):
     elif family == "template":
         model = vxm.networks.TemplateCreation(STEP_SHAPE)
         model.set_atlas(torch.from_numpy(s))
+    elif family == "hyper":
+        model = vxm.networks.HyperVxmDense(STEP_SHAPE)
     else:
         model = vxm.networks.ConditionalTemplateCreation(STEP_SHAPE, (2,), conv_nb_features=4)
     model = model.to(cuda).train()
@@ -328,6 +354,10 @@ def _step(vxm, cuda, family):
     elif family == "template":
         y_source, y_target, ms, pos = model(T)
         loss = 0.5 * ncc(T, y_source) + 0.5 * ncc(model.atlas, y_target) + mse(zeros, ms) + 0.01 * grad(None, pos)
+    elif family == "hyper":
+        hyp = torch.tensor([[0.3]], device=cuda)
+        y, flow = model(S, T, hyp)
+        loss = vxm.losses.hyper_loss(hyp, ncc(T, y), grad(None, flow))
     else:
         y_source, ms, pos, _ = model(torch.tensor([[0.3, -1.0]], device=cuda), S, T)
         loss = ncc(T, y_source) + mse(zeros, ms) + grad(None, pos) + 0.01 * mse(zeros, pos)
@@ -338,7 +368,7 @@ def _step(vxm, cuda, family):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("family", ["vxm", "probs", "template", "cond_template"])
+@pytest.mark.parametrize("family", ["vxm", "probs", "template", "cond_template", "hyper"])
 def test_training_step_on_poisoned_buffers(vxm, cuda, monkeypatch, poisoned, family):
     """one bf16 step with FusedAdam and the family's own losses: loss and updated flat parameters finite and within the step
     tests' tolerances of the unpoisoned step"""

@@ -2,7 +2,9 @@
 (NCC, (1 - lambda) NCC + lambda Grad('l2', 2) through losses.hyper_loss; FusedAdam over every parameter) against the
 graphed VxmDense step (NCC + 0.01 Grad).  Then the per-launch times of the four hypernetwork kernels — the hypernetwork
 forward and backward, the weight generation and its backward (accumulating into flat gradients, as in the step) — with
-their bytes and share of the HBM bound, and of the FusedAdam step over each model's flat buffer.
+their bytes and share of the HBM bound, the weight generation and its backward again on operands 1 and 2 floats past
+16-byte alignment (the 4- and 8-byte loads the 3-D and 2-D steps take inside FusedAdam's buffer), and the FusedAdam step
+over each model's flat buffer.
 
 The step legs alternate over `--rounds` rounds in one session, on a fresh model per leg; times are CUDA events around
 `--steps` graph replays after `--warmup` replays, with lambda changing between replays.  Launch times are CUDA events
@@ -69,8 +71,9 @@ def _bound(ms, nbytes):
 
 
 def launch_legs(vxm, dev, shape, reps):
-    """us per launch of the four hypernetwork kernels at the default sizes (P = 1, 6 layers of U = 128, N = 326 032) and of
-    FusedAdam over the HyperVxmDense's and the VxmDense's parameters"""
+    """us per launch of the four hypernetwork kernels at the default sizes (P = 1, 6 layers of U = 128, N = 326 032), of
+    the weight generation and its backward at each narrower load width, and of FusedAdam over the HyperVxmDense's and
+    the VxmDense's parameters"""
     import torch
     from voxelmorph_b200 import _lib
     from voxelmorph_b200.layers import _ptr_array
@@ -107,6 +110,21 @@ def launch_legs(vxm, dev, shape, reps):
     ms = timed(lambda: _lib.check(lib.vxm_hyper_weights_bwd(_lib.ptr(h), _lib.ptr(A), _lib.ptr(dW), _lib.ptr(gA), _lib.ptr(ga),
                                                             _lib.ptr(dh), _lib.ptr(work), U, N, 1, s()), "bwd"), reps)
     out["hyper_weights_bwd_accumulate"] = _bound(ms, 4 * (3 * U * N + 3 * N))
+    # the same two launches on A, a, W, gA, ga placed 1 and 2 floats into their buffers: the 4- and 8-byte loads of the
+    # 3-D and 2-D steps, whose FusedAdam buffer puts hyper_kernel after the flow head's 1299 or 290 floats
+    for off, width in ((1, 4), (2, 8)):
+        bufs = [torch.zeros(n + off, device=dev) for n in (U * N, N, N, U * N, N)]
+        Ao, ao, Wo, gAo, gao = [b[off:] for b in bufs]
+        Ao.copy_(A.reshape(-1))
+        ao.copy_(a)
+        ms = timed(lambda: _lib.check(lib.vxm_hyper_weights_fwd(_lib.ptr(h), _lib.ptr(Ao), _lib.ptr(ao), _lib.ptr(Wo), U, N, s()),
+                                      "fwd"), reps)
+        out["hyper_weights_fwd_%dB_loads" % width] = _bound(ms, 4 * (U * N + 2 * N))
+        ms = timed(lambda: _lib.check(lib.vxm_hyper_weights_bwd(_lib.ptr(h), _lib.ptr(Ao), _lib.ptr(dW), _lib.ptr(gAo),
+                                                                _lib.ptr(gao), _lib.ptr(dh), _lib.ptr(work), U, N, 1, s()),
+                                      "bwd"), reps)
+        out["hyper_weights_bwd_accumulate_%dB_loads" % width] = _bound(ms, 4 * (3 * U * N + 3 * N))
+        del bufs, Ao, ao, Wo, gAo, gao
     out["sizes"] = dict(P=P, U=U, layers=L, N=N)
     del gA, model, hw, A
     torch.cuda.empty_cache()
