@@ -427,6 +427,25 @@ int vxm_hyper_weights_fwd(const float* h, const float* A, const float* a, float*
 int vxm_hyper_weights_bwd(const float* h, const float* A, const float* grad_W, float* grad_A, float* grad_a,
                           float* grad_h, void* work, int U, size_t N, int accumulate, void* stream);
 
+/* ---- MutualInformation: reference voxelmorph/tf/losses.py:352-367 (neurite's soft-binned MI, `volumes` form) ----
+ * y_true = x, y_pred = y: (N, V) fp32 each (single-channel volumes).  2 <= nbins = B <= 64.  centers: B device floats
+ * used for both tensors, or NULL for c_b = lo + (hi - lo) b / (B - 1) with lo, hi the min and max of that tensor over
+ * all N V elements.  For each tensor t~ = clip(t, min_clip, max_clip), w_vb = softmax_b(-alpha (t~_v - c_b)^2); per item,
+ * with eps = 1e-7:  P = sum_v wx_v wy_v^T,  pxy = P / (sum P + eps),  px = sx / (sum sx + eps), sx = sum_v wx_v (py
+ * likewise),  MI_n = sum pxy log(pxy / (px py^T + eps) + eps);  loss[0] = -mean_n MI_n.
+ * The backward writes grad_loss[0] * dloss/dy_true and/or dloss/dy_pred (a NULL output is not computed): the exact
+ * derivative, clip gradients passed where min_clip <= t <= max_clip, and with data-driven centres the min/max path
+ * split equally among the voxels tied at the min and at the max.  work: vxm_mi_workspace_bytes(N, V, nbins) bytes (no
+ * initial value needed), written by the forward and read by the backward of the same inputs.  reduce_work
+ * (vxm_reduce_workspace_bytes, zeroed once) is used only with data-driven centres.  Sums run in a fixed order and
+ * there is no host synchronisation: results are bit-reproducible and the calls can be captured in a CUDA graph. */
+size_t vxm_mi_workspace_bytes(int N, size_t V, int nbins);
+int vxm_mi_fwd(const float* y_true, const float* y_pred, const float* centers, float* loss, void* work, void* reduce_work,
+               int N, size_t V, int nbins, float alpha, float min_clip, float max_clip, void* stream);
+int vxm_mi_bwd(const float* y_true, const float* y_pred, const float* centers, const float* grad_loss, float* grad_true,
+               float* grad_pred, void* work, int N, size_t V, int nbins, float alpha, float min_clip, float max_clip,
+               void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -112,6 +112,9 @@ SIGNATURES = {
     "vxm_hyper_mlp_bwd": (c_i, [c_f] * 6 + [c_i, c_i, c_i, c_i, c_f]),
     "vxm_hyper_weights_fwd": (c_i, [c_f] * 4 + [c_i, c_sz, c_f]),
     "vxm_hyper_weights_bwd": (c_i, [c_f] * 7 + [c_i, c_sz, c_i, c_f]),
+    "vxm_mi_workspace_bytes": (c_sz, [c_i, c_sz, c_i]),
+    "vxm_mi_fwd": (c_i, [c_f] * 6 + [c_i, c_sz, c_i, c_fl, c_fl, c_fl, c_f]),
+    "vxm_mi_bwd": (c_i, [c_f] * 7 + [c_i, c_sz, c_i, c_fl, c_fl, c_fl, c_f]),
 }
 
 _lib = None

@@ -1,6 +1,6 @@
 """NCC / MSE / Dice / Grad losses with the reference's surface
 (reference voxelmorph/torch/losses.py), and the KL loss and sigma-weighted MSE of the probabilistic
-model (reference voxelmorph/tf/losses.py): plain classes whose bound `.loss(y_true, y_pred)`
+model and the soft-binned MutualInformation (reference voxelmorph/tf/losses.py): plain classes whose bound `.loss(y_true, y_pred)`
 returns a 0-d tensor supporting `.item()`, `*`, `+`, `.backward()`.
 Each loss is one fused sm_90a kernel (plus a fused backward) from libvxm_b200.so.
 """
@@ -258,6 +258,100 @@ class KL:
             raise _lib.VxmError("KL: flow_vol_shape %s does not match flow_params of spatial shape %s"
                                 % (tuple(self.flow_vol_shape), tuple(y_pred.shape[2:])))
         return _KlFn.apply(y_pred, float(self.prior_lambda))
+
+
+class _MiFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, y_true, y_pred, centers, nb_bins, alpha, min_clip, max_clip):
+        _lib.require_cuda(y_true, y_pred, what="MutualInformation")
+        x, y = _lib.contig(y_true), _lib.contig(y_pred)
+        if x.dim() not in (4, 5) or x.shape[1] != 1 or tuple(x.shape) != tuple(y.shape):
+            # neurite's `volumes` asserts one channel and equal shapes; 2-D and 3-D volumes only here
+            raise _lib.VxmError("MutualInformation: expected two single-channel 2-D or 3-D volumes (N, 1, *vol) of equal "
+                                "shape, got %s and %s" % (tuple(x.shape), tuple(y.shape)))
+        N = x.shape[0]
+        V = x.numel() // N
+        lib = _lib.load()
+        loss = _scalar(x.device)
+        work = torch.empty(int(lib.vxm_mi_workspace_bytes(N, V, nb_bins)), dtype=torch.uint8, device=x.device)
+        rw = _lib.reduce_workspace(x.device) if centers is None else None
+        _lib.check(lib.vxm_mi_fwd(_lib.ptr(x), _lib.ptr(y), _lib.ptr(centers), _lib.ptr(loss), _lib.ptr(work), _lib.ptr(rw),
+                                  N, V, nb_bins, alpha, min_clip, max_clip, _lib.stream_ptr()), "vxm_mi_fwd")
+        # the backward re-reads both volumes and the forward's tables in `work`
+        ctx.save_for_backward(x, y)
+        ctx.work, ctx.centers = work, centers
+        ctx.cfg = (N, V, nb_bins, alpha, min_clip, max_clip)
+        return loss
+
+    @staticmethod
+    def backward(ctx, gl):
+        x, y = ctx.saved_tensors
+        N, V, nb_bins, alpha, min_clip, max_clip = ctx.cfg
+        gl = gl.contiguous().float()
+        # like _NccFn: only the sides autograd asks for are computed
+        gx = torch.empty_like(x) if ctx.needs_input_grad[0] else None
+        gy = torch.empty_like(y) if ctx.needs_input_grad[1] else None
+        if gx is not None or gy is not None:
+            _lib.check(_lib.load().vxm_mi_bwd(_lib.ptr(x), _lib.ptr(y), _lib.ptr(ctx.centers), _lib.ptr(gl), _lib.ptr(gx),
+                                              _lib.ptr(gy), _lib.ptr(ctx.work), N, V, nb_bins, alpha, min_clip, max_clip,
+                                              _lib.stream_ptr()), "vxm_mi_bwd")
+        return gx, gy, None, None, None, None, None
+
+
+class MutualInformation:
+    """Soft-binned mutual information loss (reference voxelmorph/tf/losses.py:352-367 on neurite's MutualInformation;
+    Guo 2019, Hoffmann et al. SynthMorph, TMI 2022), for registration across contrasts (T1 to T2, MR to CT).
+
+    Each image's intensities are soft-assigned to B bins with weights softmax_b(-alpha (clip(t) - c_b)^2); the joint
+    histogram of the two images gives MI per item, and `.loss(y_true, y_pred)` returns -mean_n MI_n as a 0-d tensor.
+    Inputs are (N, 1, *vol) fp32 CUDA tensors of equal shape, 2-D or 3-D.
+
+    - `bin_centers` and `nb_bins` are exclusive; with neither, nb_bins = 16.  Without centres, each image's centres are
+      linspace(min, max, B) over its whole batch (the min/max gradient is split among tied voxels, as torch.amin/amax do).
+    - `soft_bin_alpha` defaults to 1 / (2 sigma^2) with sigma = 0.5 / (B - 1) (centres not given: this assumes
+      intensities in [0, 1], which vxm's loaders produce; rescale other data or pass alpha), or sigma = 0.5 mean(diff(
+      bin_centers)).  So alpha = 450 at B = 16 and 1922 at B = 32.
+    - `min_clip` / `max_clip` default to -inf / +inf; the gradient passes where min_clip <= t <= max_clip.
+    - 2 <= B <= 64.  Loss and gradients are computed by fused kernels (csrc/mi.cu) that never store per-voxel bins."""
+
+    def __init__(self, bin_centers=None, nb_bins=None, soft_bin_alpha=None, min_clip=None, max_clip=None):
+        if bin_centers is not None and nb_bins is not None:
+            raise _lib.VxmError("MutualInformation: give bin_centers or nb_bins, not both")
+        if bin_centers is not None:
+            c = np.asarray(bin_centers, dtype=np.float64).reshape(-1)
+            if not np.all(np.isfinite(c)):
+                raise _lib.VxmError("MutualInformation: bin_centers must be finite")
+            nb_bins = c.size
+        elif nb_bins is None:
+            nb_bins = 16
+        nb_bins = int(nb_bins)
+        if nb_bins < 2 or nb_bins > 64:
+            raise _lib.VxmError("MutualInformation: the number of bins must be in [2, 64], got %d" % nb_bins)
+        if soft_bin_alpha is None:
+            sigma = 0.5 * float(np.mean(np.diff(c))) if bin_centers is not None else 0.5 / (nb_bins - 1)
+            soft_bin_alpha = 1.0 / (2.0 * sigma ** 2) if sigma != 0 else float("inf")
+        soft_bin_alpha = float(soft_bin_alpha)
+        if not (np.isfinite(soft_bin_alpha) and soft_bin_alpha > 0):
+            raise _lib.VxmError("MutualInformation: soft_bin_alpha must be finite and positive, got %r" % soft_bin_alpha)
+        self.nb_bins = nb_bins
+        self.bin_centers = None if bin_centers is None else c.astype(np.float32)
+        self.soft_bin_alpha = soft_bin_alpha
+        self.min_clip = -np.inf if min_clip is None else float(min_clip)
+        self.max_clip = np.inf if max_clip is None else float(max_clip)
+        self._dev_centers = {}
+
+    def _centers(self, device):
+        if self.bin_centers is None:
+            return None
+        t = self._dev_centers.get(device)
+        if t is None:
+            t = torch.from_numpy(self.bin_centers).to(device)
+            self._dev_centers[device] = t
+        return t
+
+    def loss(self, y_true, y_pred):
+        return _MiFn.apply(y_true, y_pred, self._centers(y_true.device), self.nb_bins, self.soft_bin_alpha,
+                           self.min_clip, self.max_clip)
 
 
 def hyper_loss(hyp, image_loss, reg_loss):

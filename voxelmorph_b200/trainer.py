@@ -15,12 +15,17 @@ from . import losses
 
 class GraphedTrainStep:
     """`loss_fn(model, *inputs) -> loss` is the forward + loss of one step; the default is train.py's
-    image loss (NCC or MSE) + lam * Grad('l2') on (source, target).  Any number of input tensors can be declared
+    image loss (NCC, MutualInformation for image_loss="mi", or MSE) + lam * Grad('l2') on (source, target).  Any number of input tensors can be declared
     through `capture(*inputs)` (e.g. the two one-hot segmentations of the semi-supervised step)."""
 
     def __init__(self, model, optimizer, image_loss="ncc", lam=0.01, int_downsize=2, warmup=3, keep_warmup=False, loss_fn=None):
         self.model, self.opt = model, optimizer
-        self.img = losses.NCC().loss if image_loss == "ncc" else losses.MSE().loss
+        if image_loss == "ncc":
+            self.img = losses.NCC().loss
+        elif image_loss == "mi":   # cross-contrast: MutualInformation() with its defaults (16 bins, intensities in [0, 1])
+            self.img = losses.MutualInformation().loss
+        else:
+            self.img = losses.MSE().loss
         self.grad = losses.Grad("l2", loss_mult=int_downsize).loss
         self.lam = lam
         self.warmup = warmup
