@@ -99,9 +99,8 @@ int vxm_resize_bwd(const float* grad_out, float* grad_x, int B, int C, int Di, i
 
 /* ---- NCC: reference voxelmorph/torch/losses.py:15-67 (5 x F.conv3d with a ones filter) ----
  * I = y_true, J = y_pred: (B,1,D,H,W).  win = (wd,wh,ww) odd window (1 along D for 2-D).
- * loss[0] = -mean(cc).  `work`: vxm_ncc_workspace_bytes().  If `saved` is non-NULL the
+ * loss[0] = -mean(cc).  `work`: vxm_reduce_workspace_bytes().  If `saved` is non-NULL the
  * forward stores 4 fields (4 * B*D*H*W floats) that the backward consumes. */
-size_t vxm_ncc_workspace_bytes(int B, int D, int H, int W);
 int vxm_ncc_fwd(const float* I, const float* J, float* loss, float* saved, void* work,
                 int B, int D, int H, int W, int wd, int wh, int ww, void* stream);
 /* grad_J = grad_loss[0] * d(-mean cc)/dJ.  grad_loss is a device scalar. */
@@ -234,11 +233,6 @@ int vxm_conv3d_tcs_pack_multi(const void* descs_dev, int ndesc, int total, void*
 int vxm_conv3d_tcs_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
                        int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
                        float slope, void* out2, int csplit, void* stream);
-/* same as vxm_conv3d_tcs_fwd (kept for callers of the former two-issuer variant; the kernel behind vxm_conv3d_tcs_fwd
- * already runs two MMA warpgroups) */
-int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
-                        int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                        float slope, void* out2, int csplit, void* stream);
 /* Split-precision ("bf16x3") passes of the same kernel — the in-tolerance tensor-core mode (reference layer:
  * voxelmorph/torch/networks.py:290-305 in fp32).  Every operand is a bf16 pair hi + lo (16 mantissa bits); a layer is
  * three launches that accumulate  x_lo*w_hi + x_hi*w_lo + x_hi*w_hi  in fp32:
@@ -329,8 +323,6 @@ int vxm_pool2_split_ndhwc_bf16(const void* x_hi, const void* x_lo, void* y_hi, v
  * e_hi + e_lo (the child vxm_pool2_split_ndhwc_bf16 copied); the LeakyReLU derivative reads e_hi < 0 */
 int vxm_unpool_combine_split_ndhwc_bf16(const void* e_hi, const void* e_lo, const void* g_skip_fine, const void* g_pool_coarse,
                                         void* out_fine, int B, int Dc, int Hc, int Wc, int C, int nd, float slope, void* stream);
-/* out[c] = sum_{b,v} x[b][c][v] for planar fp32 x (B,C,V), C <= 32; work: 128*C floats */
-int vxm_planar_channel_sums(const float* x, float* out, void* work, int B, int C, size_t V, void* stream);
 
 /* ---- MaxPool(2) / nearest Upsample(2) + concat: reference networks.py:83-85,130,137-138 ----
  * pool factor is 2 on H, W and on D when D > 1 (nd == 3).  idx (uint8, same shape as y) stores the

@@ -33,7 +33,6 @@ SIGNATURES = {
     "vxm_debug_gridsync": (c_i, [c_i, c_i, c_f]),
     "vxm_resize_fwd": (c_i, [c_f, c_f] + [c_i] * 8 + [c_fl, c_fl, c_f]),
     "vxm_resize_bwd": (c_i, [c_f, c_f] + [c_i] * 8 + [c_fl, c_fl, c_f]),
-    "vxm_ncc_workspace_bytes": (c_sz, [c_i] * 4),
     "vxm_ncc_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 7 + [c_f]),
     "vxm_ncc_bwd": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 7 + [c_f]),
     "vxm_ncc_fwd2": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 8 + [c_f]),
@@ -70,7 +69,6 @@ SIGNATURES = {
     "vxm_conv3d_tcs_pack_desc_fold": (c_i, [c_f, c_f, c_f] + [c_i] * 5),
     "vxm_conv3d_tcs_pack_multi": (c_i, [c_f, c_i, c_i, c_f]),
     "vxm_conv3d_tcs_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f, c_i, c_f]),
-    "vxm_conv3d_tcs2_fwd": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f, c_i, c_f]),
     "vxm_conv3d_tcs_fwd_acc": (c_i, [c_f, c_f, c_f, c_f, c_f, c_f, c_f] + [c_i] * 11 + [c_fl, c_f]),
     "vxm_conv3d_tcs_fits": (c_i, [c_i] * 3),
     "vxm_conv3d_tcs_fwd_blk": (c_i, [c_f] * 8 + [c_i] * 11 + [c_fl, c_i, c_f]),
@@ -93,7 +91,6 @@ SIGNATURES = {
     "vxm_planar_fold_kd_bf16": (c_i, [c_f, c_f, c_i, c_f, c_i, c_i, c_sz, c_i, c_f]),
     "vxm_pool2_split_ndhwc_bf16": (c_i, [c_f, c_f, c_f, c_f] + [c_i] * 6 + [c_f]),
     "vxm_unpool_combine_split_ndhwc_bf16": (c_i, [c_f, c_f, c_f, c_f, c_f] + [c_i] * 6 + [c_fl, c_f]),
-    "vxm_planar_channel_sums": (c_i, [c_f, c_f, c_f, c_i, c_i, c_sz, c_f]),
     "vxm_maxpool2_fwd": (c_i, [c_f, c_f, c_f] + [c_i] * 6 + [c_f]),
     "vxm_maxpool2_bwd": (c_i, [c_f, c_f, c_f] + [c_i] * 6 + [c_f]),
     "vxm_upcat_fwd": (c_i, [c_f, c_f, c_f] + [c_i] * 7 + [c_f]),

@@ -971,12 +971,6 @@ extern "C" int vxm_conv3d_tcs_fwd_blk(const void* xa, const void* xb, const void
                          acc_in, out_lo, opitch == Cout ? 0 : opitch, 0, stream);
 }
 
-extern "C" int vxm_conv3d_tcs2_fwd(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, const void* mask,
-                                   int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp, int kd, int out_mode,
-                                   float slope, void* out2, int csplit, void* stream) {
-  return vxm_conv3d_tcs_fwd(xa, xb, wpk, bias, out, mask, B, D, H, W, Ca, Cb, up, Cout, coutp, kd, out_mode, slope, out2, csplit, stream);
-}
-
 extern "C" int vxm_conv3d_tcs_fwd_acc(const void* xa, const void* xb, const void* wpk, const float* bias, void* out, void* out_lo,
                                       const float* acc_in, int B, int D, int H, int W, int Ca, int Cb, int up, int Cout, int coutp,
                                       int kd, int out_mode, float slope, void* stream) {
@@ -1021,37 +1015,22 @@ static int conv_tcs_launch(const void* xa, const void* xb, const void* wpk, cons
   {
     const size_t slab8 = (size_t)10 * WT * (g0 + g1) * 2;
     const int ns8 = (int)((227 * 1024 - fixed) / slab8);
-    const char* e = getenv("VXM_B200_TCS_HT");
-    if (g0 <= 32 && coutp <= 32 && ns8 >= (kd == 3 ? 5 : 3) && H > 4 && !(e && e[0] == '4') && !opitch) HTv = 8;
+    if (g0 <= 32 && coutp <= 32 && ns8 >= (kd == 3 ? 5 : 3) && H > 4 && !opitch) HTv = 8;
     if (poly) HTv = poly == 2 ? 8 : 4;               // the polyphase kernels exist at one tile height each
   }
   a.tiles_h = (H + HTv - 1) / HTv; a.tiles_w = (W + WUSE - 1) / WUSE;
   int nsm = conv_ctas();
   // depth chunking: balance the persistent CTAs (waves of nsm items) against the 2 halo slabs every chunk re-loads
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
-  int best_nch = 1;
-  double best_cost = 1e300;
   // (the coarse dgrad: output slices of 2 fine slabs each, so the halo weighs half as much)
   const int Do = poly == 2 ? D / 2 : D;
-  for (int nch = 1; nch <= 40 && nch <= Do; ++nch) {
-    const int dc = (Do + nch - 1) / nch;
-    const long long items = tiles * ((Do + dc - 1) / dc);
-    const long long waves = (items + nsm - 1) / nsm;
-    const double cost = (double)waves * (dc + (poly == 2 ? 1.25 : (kd == 3 ? 2.5 : 0.5)));
-    if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
-  }
-  a.dchunk = (Do + best_nch - 1) / best_nch; a.nchunks = (Do + a.dchunk - 1) / a.dchunk;
+  a.dchunk = depth_chunk(Do, tiles, nsm, poly == 2 ? 1.25 : (kd == 3 ? 2.5 : 0.5), 40);
+  a.nchunks = (Do + a.dchunk - 1) / a.dchunk;
   a.nitems = (int)(tiles * a.nchunks);
   const size_t slab = (size_t)(HTv + 2) * WT * (g0 + g1) * 2;
   int nslot = (int)((227 * 1024 - fixed) / slab);
-  {
-    // ring depth: the slabs of up to 13 steps ahead (16-channel layers) hide the L2 / HBM latency of the tensor copies.
-    // VXM_B200_RING=8: A/B switch.
-    const char* e = getenv("VXM_B200_RING");
-    const int cap = e ? atoi(e) : MAXSLOT;
-    if (nslot > cap) nslot = cap;
-    if (nslot > MAXSLOT) nslot = MAXSLOT;
-  }
+  // ring depth: the slabs of up to 13 steps ahead (16-channel layers) hide the L2 / HBM latency of the tensor copies
+  if (nslot > MAXSLOT) nslot = MAXSLOT;
   VXM_REQUIRE(nslot >= 4, "conv3d_tcs_fwd: not enough shared memory for the slab ring");
   a.nslot = nslot;
   size_t smem = fixed + (size_t)nslot * slab;

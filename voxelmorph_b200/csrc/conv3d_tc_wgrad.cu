@@ -363,10 +363,10 @@ using namespace vxm::tc;
 namespace vxm {
 namespace tcw {   // conv3d_tc_wgrad2.cu: the kw-stacked Toeplitz formulation (channels-last bf16 sources only)
 bool wgrad2_supported(int Ca, int Cb, int Cg);
-struct ReduceDesc;
 int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
-                  int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer = nullptr,
-                  size_t* work_used = nullptr, bool khm = false, int x_pitch = 0, int g_pitch = 0, int co_off = 0);
+                  int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* desc,
+                  size_t* work_used, bool khm, int x_pitch, int g_pitch, int co_off);
+int wgrad2_reduce(const ReduceDesc* d, int n, cudaStream_t st);
 }
 }
 
@@ -406,19 +406,26 @@ extern "C" int vxm_conv3d_tc_wgrad(const void* xa, const void* xb, const float* 
   }
   VXM_REQUIRE(Cout_real > 0 && Cout_real <= Cg, "conv3d_tc_wgrad: Cout_real out of range");
   if (nplanar_x == 0 && nplanar_g == 0 && tcw::wgrad2_supported(Ca, Cb, Cg)) {
-    // one launch per source tensor of the (virtual) concatenation: xa -> weights [0, Ca), xb -> [Ca, Ca + Cb)
+    // one launch per source tensor of the (virtual) concatenation: xa -> weights [0, Ca), xb -> [Ca, Ca + Cb), then one
+    // reduction of both.  Their partials, 2 x (256 x kd x 9 x 32 x 32 + 256 x 32) floats + 2 x 255 bytes of rounding at
+    // most, fit the 256 x kd x 9 x 64 x 32 + 1024 x 32 floats of vxm_conv3d_tc_wgrad_workspace_bytes(kd).
     cudaStream_t st2 = as_stream(stream);
-    int rc = 0;
+    tcw::ReduceDesc d[2];
+    int n = 0;
+    size_t used = 0, used_b = 0;
     if (Ca) {
       const int cnt = Cin_real < Ca ? Cin_real : Ca;
-      rc = tcw::wgrad2_launch(xa, Ca, up, gz, Cg, grad_w, grad_b, work, B, D, H, W, kd, Cout_real, Cin_real, 0, cnt, accumulate, st2);
+      int rc = tcw::wgrad2_launch(xa, Ca, up, gz, Cg, grad_w, grad_b, work, B, D, H, W, kd, Cout_real, Cin_real, 0, cnt, accumulate, st2,
+                                  &d[n++], &used, false, 0, 0, 0);
       if (rc) return rc;
     }
     if (Cb && Cin_real > Ca) {
       const int cnt = Cin_real - Ca < Cb ? Cin_real - Ca : Cb;
-      rc = tcw::wgrad2_launch(xb, Cb, 0, gz, Cg, grad_w, Ca ? nullptr : grad_b, work, B, D, H, W, kd, Cout_real, Cin_real, Ca, cnt, accumulate, st2);
+      int rc = tcw::wgrad2_launch(xb, Cb, 0, gz, Cg, grad_w, Ca ? nullptr : grad_b, (char*)work + used, B, D, H, W, kd, Cout_real, Cin_real, Ca,
+                                  cnt, accumulate, st2, &d[n++], &used_b, false, 0, 0, 0);
+      if (rc) return rc;
     }
-    return rc;
+    return tcw::wgrad2_reduce(d, n, st2);
   }
   a.xa = (const __nv_bfloat16*)xa; a.xb = (const __nv_bfloat16*)xb; a.gz = (const __nv_bfloat16*)gz;
   a.Ca = Ca; a.Cb = Cb; a.up = up; a.upd = (up && kd == 3) ? 1 : 0; a.Cg = Cg;

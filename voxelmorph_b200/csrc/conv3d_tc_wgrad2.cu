@@ -16,7 +16,7 @@
 // products that pair a voxel with a neighbour across the tile-row wrap vanish.
 // All 3 (kh) x [M x 3*GOUT] fp32 accumulators stay in the registers of two MMA warpgroups for the CTA's whole lifetime
 // (M = 128: one m64 half each; M = 64: kh 0-1 / kh 2); each CTA writes ONE partial
-// [27][G][GOUT]; wgrad2_reduce_kernel sums the partials in fixed order (deterministic).  The first MMA warpgroup also
+// [27][G][GOUT]; wgrad2_reduce_multi_kernel sums the partials in fixed order (deterministic).  The first MMA warpgroup also
 // folds the bias gradient (sum of gz) out of the staged gz rows while its wgmma chain runs.
 #include <stdlib.h>
 
@@ -42,7 +42,6 @@ struct Wgrad2Args {
   float* bias_partial;                       // [grid][GOUT] or null
   int B, D, H, W;
   int tiles_h, tiles_w, dchunk, nchunks, nitems, nslot;
-  int dbg;      // profiling only (VXM_B200_WGRAD_DBG): 2 = no slab copies, 4 = no bias sums
   int xpitch, gpitch;   // channels per voxel of the x / gz tensors (> Cx / Cg: a channel slice of a wider tensor)
 };
 
@@ -153,7 +152,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
         for (int k = 0; k < KX; ++k) {
           const bool ok = dok && soff[k] >= 0;
           const __nv_bfloat16* src = ok ? base + soff[k] : a.x;
-          if (a.dbg & 2) continue;
           cp_async16(slab + doff[k], src, ok ? 16u : 0u);
           if (NMIRROR && xslot < (uint32_t)NMIRROR) cp_async16(slab + (size_t)NS * XSLAB + doff[k], src, ok ? 16u : 0u);
         }
@@ -168,7 +166,6 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
 #pragma unroll
           for (int k = 0; k < KG; ++k) {
             const bool ok = goff[k] >= 0;
-            if (a.dbg & 2) continue;
             cp_async16(gt + gdoff[k], ok ? baseG + goff[k] : a.gz, ok ? 16u : 0u);
           }
           cp_async_arrive_noinc(&gfull[gslot]);
@@ -188,7 +185,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) wgrad2_kernel(const Wgrad2Args a)
     if (wg == 0)
 #pragma unroll
       for (int c = 0; c < GOUT; ++c) bsum[c] = 0.f;
-    const bool do_bias = wg == 0 && a.bias_partial && !(a.dbg & 4);
+    const bool do_bias = wg == 0 && a.bias_partial;
     uint32_t roff[GOUT / 8];
 #pragma unroll
     for (int c8 = 0; c8 < GOUT / 8; ++c8) roff[c8] = swz((uint32_t)(GPAD + t) * WG + (uint32_t)c8 * 16u, WG);
@@ -580,44 +577,11 @@ __global__ void __launch_bounds__(PNTHREADS, 1) wgrad2_poly_kernel(const Wgrad2P
   }
 }
 
-// gw[co][ci_off + ci][tap] (+)= sum_cta partial[cta][tap][ci][co]   (fixed order -> deterministic).  Block = 64 elements
-// x 4 quarters of the CTA range: threads follow the partial layout (co fastest) so the reads coalesce, and the four
-// quarter sums (combined in fixed order through shared memory) keep 4x more loads in flight than one serial loop.
-__global__ void __launch_bounds__(256) wgrad2_reduce_kernel(const float* __restrict__ partial, float* __restrict__ gw, int ncta, int T, int G,
-                                                            int GOUT, int Cout, int Cin_total, int ci_off, int ci_cnt,
-                                                            const float* __restrict__ bias_partial, float* __restrict__ gb, int accumulate) {
-  __shared__ float sh[4][64];
-  const int tx = threadIdx.x & 63, ty = threadIdx.x >> 6;
-  if (gb && blockIdx.x == 0 && threadIdx.x < Cout) {
-    float acc = accumulate ? gb[threadIdx.x] : 0.f;
-    for (int c = 0; c < ncta; ++c) acc += bias_partial[(size_t)c * GOUT + threadIdx.x];
-    gb[threadIdx.x] = acc;
-  }
-  const int per_cta = T * G * GOUT;
-  const int j = blockIdx.x * 64 + tx;
-  const int q = (ncta + 3) / 4, c0 = ty * q, c1 = min(c0 + q, ncta);
-  float acc = 0.f;
-  if (j < per_cta)
-    for (int c = c0; c < c1; ++c) acc += partial[(size_t)c * per_cta + j];
-  sh[ty][tx] = acc;
-  __syncthreads();
-  if (ty == 0 && j < per_cta) {
-    const int co = j % GOUT, ci = (j / GOUT) % G, tap = j / (GOUT * G);
-    if (co < Cout && ci < ci_cnt) {
-      const float tot = ((sh[0][tx] + sh[1][tx]) + sh[2][tx]) + sh[3][tx];
-      float* dst = gw + ((size_t)co * Cin_total + ci_off + ci) * T + tap;
-      *dst = (accumulate ? *dst : 0.f) + tot;
-    }
-  }
-}
-
-// All reductions of a backward pass in ONE launch (16 reduce launches per training step otherwise).  The descriptors
-// travel by value in the kernel parameters (no device table to keep alive or re-upload inside a captured graph).
-struct ReduceDesc {
-  const float* partial; float* gw; const float* bias_partial; float* gb;
-  int ncta, T, G, GOUT, Cout, Cin_total, ci_off, ci_cnt, accumulate, blk_begin;
-  int co_off;            // first output channel of a gz slice (gw rows co_off .. co_off + Cout - 1; gb already offset)
-};
+// gw[co_off + co][ci_off + ci][tap] (+)= sum_cta partial[cta][tap][ci][co] for every pending reduction of a backward pass,
+// in ONE launch (16 reduce launches per training step otherwise); fixed order -> deterministic.  Block = 64 elements x 4
+// quarters of the CTA range: threads follow the partial layout (co fastest) so the reads coalesce, and the four quarter
+// sums (combined in fixed order through shared memory) keep 4x more loads in flight than one serial loop.  The
+// descriptors travel by value in the kernel parameters (no device table to keep alive or re-upload inside a captured graph).
 constexpr int MAXRED = 40;
 struct ReduceBatch {
   ReduceDesc d[MAXRED];
@@ -666,40 +630,17 @@ namespace tcw {
 static bool chan_ok(int c) { return c == 8 || c == 16 || c == 32; }
 
 bool wgrad2_supported(int Ca, int Cb, int Cg) {
-  const char* e = getenv("VXM_B200_WGRAD");
-  if (e && e[0] == 'o') return false;   // "old": conv3d_tc_wgrad.cu
   return (Ca == 0 || chan_ok(Ca)) && (Cb == 0 || chan_ok(Cb)) && Ca + Cb > 0 && chan_ok(Cg);
 }
 
-// depth chunking: balance the persistent CTAs (waves of nsm items) against the `halo` slabs every chunk re-loads
-static int wgrad2_dchunk(int D, long long tiles, int nsm, double halo) {
-  int best_nch = 1;
-  double best_cost = 1e300;
-  for (int nch = 1; nch <= 32 && nch <= D; ++nch) {
-    const int dc = (D + nch - 1) / nch;
-    const long long items = tiles * ((D + dc - 1) / dc);
-    const long long waves = (items + nsm - 1) / nsm;
-    const double cost = (double)waves * (dc + halo);
-    if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
-  }
-  return (D + best_nch - 1) / best_nch;
-}
-
-// Partials of `grid` CTAs of T x G x GOUT floats at `partial` (bias partials at `bias_partial`): record the deferred
-// reduction, or reduce now.
-static int wgrad2_finish(float* partial, float* bias_partial, int grid, int T, int G, int GOUT, float* grad_w, float* grad_b, int Cout_real,
-                         int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer, int co_off) {
+// Partials of `grid` CTAs of T x G x GOUT floats at `partial` (bias partials at `bias_partial`): record their reduction.
+static void wgrad2_record(float* partial, float* bias_partial, int grid, int T, int G, int GOUT, float* grad_w, float* grad_b, int Cout_real,
+                          int Cin_total, int ci_off, int ci_cnt, int accumulate, ReduceDesc* desc, int co_off) {
   const int per_cta = T * G * GOUT;
-  if (defer) {
-    defer->partial = partial; defer->gw = grad_w; defer->bias_partial = bias_partial; defer->gb = grad_b;
-    defer->ncta = grid; defer->T = T; defer->G = G; defer->GOUT = GOUT; defer->Cout = Cout_real; defer->Cin_total = Cin_total;
-    defer->ci_off = ci_off; defer->ci_cnt = ci_cnt; defer->accumulate = accumulate; defer->blk_begin = (per_cta + 63) / 64;   // block count, turned into an offset by the flush
-    defer->co_off = co_off;
-    return VXM_OK;
-  }
-  wgrad2_reduce_kernel<<<(per_cta + 63) / 64, 256, 0, st>>>(partial, grad_w, grid, T, G, GOUT, Cout_real, Cin_total, ci_off, ci_cnt,
-                                                              bias_partial, grad_b, accumulate);
-  return check_launch("conv3d_tc_wgrad2_reduce");
+  desc->partial = partial; desc->gw = grad_w; desc->bias_partial = bias_partial; desc->gb = grad_b;
+  desc->ncta = grid; desc->T = T; desc->G = G; desc->GOUT = GOUT; desc->Cout = Cout_real; desc->Cin_total = Cin_total;
+  desc->ci_off = ci_off; desc->ci_cnt = ci_cnt; desc->accumulate = accumulate; desc->blk_begin = (per_cta + 63) / 64;   // block count, turned into an offset by wgrad2_reduce
+  desc->co_off = co_off;
 }
 
 // The coarse form (wgrad2_poly_kernel) serves every 3-D launch whose source is a 32-channel nearest-x2 upsampled slice
@@ -712,7 +653,7 @@ static bool wgrad2_poly_ok(int Cx, int up, int Cg, int kd, int D, int H, int W) 
 
 static int wgrad2_poly_launch(const void* x, int x_pitch, const void* gz, int Cg, int g_pitch, float* grad_w, float* grad_b, void* work, int B,
                               int D, int H, int W, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st,
-                              ReduceDesc* defer, size_t* work_used, int co_off) {
+                              ReduceDesc* desc, size_t* work_used, int co_off) {
   Wgrad2PolyArgs a{};
   a.x = (const __nv_bfloat16*)x; a.xpitch = x_pitch;
   a.gz = (const __nv_bfloat16*)gz; a.Cg = Cg; a.gpitch = g_pitch;
@@ -721,67 +662,55 @@ static int wgrad2_poly_launch(const void* x, int x_pitch, const void* gz, int Cg
   a.tiles_h = (a.Hc + PTH) / PTH; a.tiles_w = (a.Wc + PTU) / PTU;
   const int nsm = conv_ctas();
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
-  a.dchunk = wgrad2_dchunk(a.Dc + 1, tiles, nsm, 0.5);
+  a.dchunk = depth_chunk(a.Dc + 1, tiles, nsm, 0.5, 32);
   a.nchunks = (a.Dc + a.dchunk) / a.dchunk;
   a.nitems = (int)(tiles * a.nchunks);
   int grid = a.nitems < nsm ? a.nitems : nsm;
   if (grid > 256) grid = 256;
+  // this launch owns exactly [work, work + *work_used): partials, then bias partials
   a.partial = (float*)work;
-  if (defer) {
-    const size_t npart = (size_t)grid * 27 * 32 * 32;
-    a.bias_partial = grad_b ? (float*)work + npart : nullptr;
-    *work_used = (npart + (grad_b ? (size_t)grid * 32 : 0)) * sizeof(float);
-    *work_used = (*work_used + 255) & ~(size_t)255;
-  } else {
-    a.bias_partial = grad_b ? (float*)work + (size_t)256 * 27 * 64 * 32 : nullptr;
-  }
+  const size_t npart = (size_t)grid * 27 * 32 * 32;
+  a.bias_partial = grad_b ? (float*)work + npart : nullptr;
+  *work_used = (npart + (grad_b ? (size_t)grid * 32 : 0)) * sizeof(float);
+  *work_used = (*work_used + 255) & ~(size_t)255;
   a.nslot = PNSLOT;
   const size_t smem = PSMEM;
   VXM_CUDA(cudaFuncSetAttribute(wgrad2_poly_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   wgrad2_poly_kernel<<<grid, PNTHREADS, smem, st>>>(a);
   int rc = check_launch("conv3d_tc_wgrad2_poly");
   if (rc) return rc;
-  return wgrad2_finish(a.partial, a.bias_partial, grid, 27, 32, 32, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, st, defer,
-                       co_off);
+  wgrad2_record(a.partial, a.bias_partial, grid, 27, 32, 32, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, desc, co_off);
+  return VXM_OK;
 }
 
 // one source tensor (C channels, optionally nearest-x2 upsampled) against gz; weights [ci_off, ci_off + ci_cnt) of Cin_total
 int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* grad_w, float* grad_b, void* work, int B, int D, int H, int W,
-                  int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* defer,
+                  int kd, int Cout_real, int Cin_total, int ci_off, int ci_cnt, int accumulate, cudaStream_t st, ReduceDesc* desc,
                   size_t* work_used, bool khm, int x_pitch, int g_pitch, int co_off) {
-  VXM_REQUIRE(defer || co_off == 0, "conv3d_tc_wgrad2: gz slices need the deferred reduction");
   if (!khm && wgrad2_poly_ok(Cx, up, Cg, kd, D, H, W))
     return wgrad2_poly_launch(x, x_pitch ? x_pitch : Cx, gz, Cg, g_pitch ? g_pitch : Cg, grad_w, grad_b, work, B, D, H, W, Cout_real, Cin_total,
-                              ci_off, ci_cnt, accumulate, st, defer, work_used, co_off);
+                              ci_off, ci_cnt, accumulate, st, desc, work_used, co_off);
   Wgrad2Args a{};
   a.x = (const __nv_bfloat16*)x; a.Cx = Cx; a.up = up; a.upd = (up && kd == 3) ? 1 : 0;
   a.gz = (const __nv_bfloat16*)gz; a.Cg = Cg;
   a.xpitch = x_pitch ? x_pitch : Cx; a.gpitch = g_pitch ? g_pitch : Cg;
   a.B = B; a.D = D; a.H = H; a.W = W;
   a.tiles_h = (H + TH - 1) / TH; a.tiles_w = (W + TUSE - 1) / TUSE;
-  {
-    const char* de = getenv("VXM_B200_WGRAD_DBG");
-    a.dbg = de ? atoi(de) : 0;
-  }
   const int G = Cx <= 16 ? 16 : 32, GOUT = Cg <= 16 ? 16 : 32;
   const int nsm = conv_ctas();
   // depth chunking: balance the persistent CTAs (waves of nsm items) against the 2 halo slabs every chunk re-loads
   const long long tiles = (long long)B * a.tiles_h * a.tiles_w;
-  a.dchunk = wgrad2_dchunk(D, tiles, nsm, kd == 3 ? 2.5 : 0.5);
+  a.dchunk = depth_chunk(D, tiles, nsm, kd == 3 ? 2.5 : 0.5, 32);
   a.nchunks = (D + a.dchunk - 1) / a.dchunk;
   a.nitems = (int)(tiles * a.nchunks);
   int grid = a.nitems < nsm ? a.nitems : nsm;
   if (grid > 256) grid = 256;
+  // this launch owns exactly [work, work + *work_used): partials, then bias partials
   a.partial = (float*)work;
-  if (defer) {
-    // deferred reduction: this launch owns exactly [work, work + *work_used): partials, then bias partials
-    const size_t npart = (size_t)grid * kd * 9 * G * GOUT;
-    a.bias_partial = grad_b ? (float*)work + npart : nullptr;
-    *work_used = (npart + (grad_b ? (size_t)grid * GOUT : 0)) * sizeof(float);
-    *work_used = (*work_used + 255) & ~(size_t)255;
-  } else {
-    a.bias_partial = grad_b ? (float*)work + (size_t)256 * kd * 9 * 64 * 32 : nullptr;
-  }
+  const size_t npart = (size_t)grid * kd * 9 * G * GOUT;
+  a.bias_partial = grad_b ? (float*)work + npart : nullptr;
+  *work_used = (npart + (grad_b ? (size_t)grid * GOUT : 0)) * sizeof(float);
+  *work_used = (*work_used + 255) & ~(size_t)255;
   const size_t xslab = (size_t)XROWS * 2 * G, gslab = (size_t)GSROWS * 2 * GOUT;
   const int extra = kd == 3 ? 3 : 0;
   int nslot = (int)((200 * 1024 - NGS * gslab - 512) / xslab) - extra;
@@ -806,8 +735,24 @@ int wgrad2_launch(const void* x, int Cx, int up, const void* gz, int Cg, float* 
   } else if (kd == 3) VXM_W2_G(3); else VXM_W2_G(1);
   int rc = check_launch("conv3d_tc_wgrad2");
   if (rc) return rc;
-  return wgrad2_finish(a.partial, a.bias_partial, grid, kd * 9, G, GOUT, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, st,
-                       defer, co_off);
+  wgrad2_record(a.partial, a.bias_partial, grid, kd * 9, G, GOUT, grad_w, grad_b, Cout_real, Cin_total, ci_off, ci_cnt, accumulate, desc,
+                co_off);
+  return VXM_OK;
+}
+
+// Every recorded reduction d[0 .. n), 0 < n <= MAXRED, in one launch on `st`
+int wgrad2_reduce(const ReduceDesc* d, int n, cudaStream_t st) {
+  ReduceBatch rb;
+  int blocks = 0;
+  for (int i = 0; i < n; ++i) {
+    rb.d[i] = d[i];
+    const int nb = d[i].blk_begin;      // wgrad2_record stored the block count here
+    rb.d[i].blk_begin = blocks;
+    blocks += nb;
+  }
+  rb.n = n; rb.total_blocks = blocks;
+  wgrad2_reduce_multi_kernel<<<blocks, 256, 0, st>>>(rb);
+  return check_launch("conv3d_tc_wgrad2_reduce_multi");
 }
 
 }  // namespace tcw
@@ -834,8 +779,7 @@ extern "C" int vxm_conv3d_tc_wgrad2_partial(const void* xa, const void* xb, cons
                                             int Ca, int Cb, int up, int Cin_real, int Cg, int Cout_real, int kd, int accumulate, void* stream) {
   VXM_REQUIRE(B > 0 && D > 0 && H > 0 && W > 0 && grad_w && work && work_used && descs_host && ndesc && gz, "conv3d_tc_wgrad2_partial: bad argument");
   VXM_REQUIRE(kd == 1 || kd == 3, "conv3d_tc_wgrad2_partial: kd must be 1 or 3");
-  const char* e = getenv("VXM_B200_WGRAD");
-  VXM_REQUIRE(!(e && e[0] == 'o') && (Ca == 0 || chan_ok64(Ca)) && (Cb == 0 || chan_ok64(Cb)) && Ca + Cb > 0 && chan_ok64(Cg),
+  VXM_REQUIRE((Ca == 0 || chan_ok64(Ca)) && (Cb == 0 || chan_ok64(Cb)) && Ca + Cb > 0 && chan_ok64(Cg),
               "conv3d_tc_wgrad2_partial: channel counts (%d,%d | %d) unsupported", Ca, Cb, Cg);
   VXM_REQUIRE((Ca == 0 || xa) && (Cb == 0 || xb), "conv3d_tc_wgrad2_partial: missing source tensor");
   const int nsub = ((Ca + 31) / 32 + (Cb + 31) / 32) * ((Cg + 31) / 32);
@@ -891,16 +835,5 @@ extern "C" int vxm_conv3d_tc_wgrad2_partial_khm(const void* x, const void* gz, f
 
 extern "C" int vxm_conv3d_tc_wgrad2_flush(const void* descs_host, int ndesc, void* stream) {
   VXM_REQUIRE(descs_host && ndesc > 0 && ndesc <= MAXRED, "conv3d_tc_wgrad2_flush: bad argument");
-  ReduceBatch rb;
-  const ReduceDesc* d = (const ReduceDesc*)descs_host;
-  int blocks = 0;
-  for (int i = 0; i < ndesc; ++i) {
-    rb.d[i] = d[i];
-    const int nb = d[i].blk_begin;      // wgrad2_launch stored the block count here
-    rb.d[i].blk_begin = blocks;
-    blocks += nb;
-  }
-  rb.n = ndesc; rb.total_blocks = blocks;
-  wgrad2_reduce_multi_kernel<<<blocks, 256, 0, as_stream(stream)>>>(rb);
-  return check_launch("conv3d_tc_wgrad2_reduce_multi");
+  return wgrad2_reduce((const ReduceDesc*)descs_host, ndesc, as_stream(stream));
 }

@@ -584,7 +584,6 @@ static int ncc_check(int B, int D, int H, int W, int wd, int wh, int ww, dim3* g
 using namespace vxm;
 
 extern "C" size_t vxm_reduce_workspace_bytes(void) { return sizeof(double) * kMaxReduceBlocks + 256; }
-extern "C" size_t vxm_ncc_workspace_bytes(int, int, int, int) { return vxm_reduce_workspace_bytes(); }
 
 namespace vxm {
 ReduceWork as_reduce_work(void* work) {

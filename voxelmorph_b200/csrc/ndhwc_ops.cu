@@ -168,26 +168,6 @@ __global__ void __launch_bounds__(256) unpool_combine_kernel(const __nv_bfloat16
   }
 }
 
-// out[c] = sum over b, v of x[b][c][v]   (planar fp32; two-stage deterministic)
-__global__ void __launch_bounds__(256) planar_sum_partial_kernel(const float* __restrict__ x, float* __restrict__ part, int B, int C, size_t V) {
-  __shared__ double s_red[32];
-  const int c = blockIdx.y;
-  double acc = 0.0;
-  for (int b = 0; b < B; ++b) {
-    const float* p = x + ((size_t)b * C + c) * V;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < V; i += (size_t)gridDim.x * blockDim.x) acc += (double)__ldg(p + i);
-  }
-  double t = block_sum<double>(acc, s_red);
-  if (threadIdx.x == 0) part[(size_t)c * gridDim.x + blockIdx.x] = (float)t;
-}
-__global__ void planar_sum_final_kernel(const float* __restrict__ part, float* __restrict__ out, int C, int nblk) {
-  int c = threadIdx.x;
-  if (c >= C) return;
-  double acc = 0.0;
-  for (int i = 0; i < nblk; ++i) acc += (double)part[(size_t)c * nblk + i];
-  out[c] = (float)acc;
-}
-
 struct PlanarSrc {
   const float* p[8];
   long long bstride[8];
@@ -345,16 +325,6 @@ extern "C" int vxm_unpool_combine_split_ndhwc_bf16(const void* e_hi, const void*
                                                                            (const __nv_bfloat16*)g_pool, (__nv_bfloat16*)out, g, slope,
                                                                            (const __nv_bfloat16*)e_lo);
   return check_launch("unpool_combine_split");
-}
-
-extern "C" int vxm_planar_channel_sums(const float* x, float* out, void* work, int B, int C, size_t V, void* stream) {
-  VXM_REQUIRE(x && out && work && B > 0 && C > 0 && C <= 32 && V > 0, "planar_channel_sums: bad argument");
-  const int nblk = 128;
-  planar_sum_partial_kernel<<<dim3(nblk, C), 256, 0, as_stream(stream)>>>(x, (float*)work, B, C, V);
-  int rc = check_launch("planar_sum_partial");
-  if (rc) return rc;
-  planar_sum_final_kernel<<<1, 32, 0, as_stream(stream)>>>((const float*)work, out, C, nblk);
-  return check_launch("planar_sum_final");
 }
 
 extern "C" int vxm_planar_to_ndhwc8_bf16(const float* const* planes, const long long* bstrides, int nplanes, void* out, int B, size_t V,

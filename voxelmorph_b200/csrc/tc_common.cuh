@@ -209,5 +209,30 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&v);
 }
 
+// Depth chunking of a persistent launch over `tiles` (b, h, w) tiles and D slices: balance the CTAs' waves of nsm items
+// against the `halo` slabs every chunk re-loads, over 1 .. max_chunks chunks.  Returns the chunk depth.
+inline int depth_chunk(int D, long long tiles, int nsm, double halo, int max_chunks) {
+  int best_nch = 1;
+  double best_cost = 1e300;
+  for (int nch = 1; nch <= max_chunks && nch <= D; ++nch) {
+    const int dc = (D + nch - 1) / nch;
+    const long long items = tiles * ((D + dc - 1) / dc);
+    const long long waves = (items + nsm - 1) / nsm;
+    const double cost = (double)waves * (dc + halo);
+    if (cost < best_cost - 1e-9) { best_cost = cost; best_nch = nch; }
+  }
+  return (D + best_nch - 1) / best_nch;
+}
+
 }  // namespace tc
+
+namespace tcw {
+// One pending reduction of the Toeplitz weight gradient (conv3d_tc_wgrad2.cu): `ncta` per-CTA partials of T x G x GOUT
+// floats at `partial` (and GOUT bias partials each at `bias_partial`), summed in fixed order into gw / gb.
+struct ReduceDesc {
+  const float* partial; float* gw; const float* bias_partial; float* gb;
+  int ncta, T, G, GOUT, Cout, Cin_total, ci_off, ci_cnt, accumulate, blk_begin;
+  int co_off;            // first output channel of a gz slice (gw rows co_off .. co_off + Cout - 1; gb already offset)
+};
+}  // namespace tcw
 }  // namespace vxm
