@@ -438,6 +438,31 @@ int vxm_mi_bwd(const float* y_true, const float* y_pred, const float* centers, c
                float* grad_pred, void* work, int N, size_t V, int nbins, float alpha, float min_clip, float max_clip,
                void* stream);
 
+/* ---- Surface points: reference voxelmorph/tf/utils/utils.py:465-499 (point_spatial_transformer) and 71-88
+ * (value_at_location), as VxmDenseSemiSupervisedPointCloud uses them (voxelmorph/tf/networks.py:391-486) ----
+ * Sampling is neurite's interpn(..., 'linear', fill_value=None): per axis of size n at x, c = clip(x, 0, n-1),
+ * i0 = clip(floor x, 0, n-1), i1 = clip(i0+1, 0, n-1), weight i1 - c on i0 and 1 - (i1 - c) on i1, weights multiplied
+ * across axes; outside the volume the border value, and d/dx = 0 there (the clip passes its gradient for 0 <= x <= n-1).
+ * points: (B, N, nd+1), the spatial coordinates in the flow's axis order (3-D: D, H, W; 2-D: H, W), the last column a
+ * label index.  flow: (B, nd, D, H, W).  Point warp: out (B, N, nd+1), out = p + r * interp(flow, p), label column
+ * copied.  Its backward ADDS to grad_flow (B, nd, D, H, W) the flow gradient of grad_out (B, N, nd+1; label column
+ * ignored): pairs sorted by voxel (CUB radix sort) and summed per voxel in point order in fp64, no float atomics and no
+ * host synchronisation, so it is bit-reproducible and graph-capturable.  work: vxm_point_warp_workspace_bytes(...)
+ * bytes, O(B N 2^nd), no initial value (the size query asks CUB for its scratch size, which reads the current
+ * device; 0 for sizes the kernels refuse: B * D * H * W must stay below 2^32, B * N * 2^nd below 2^31).
+ * Distance lookup: sdt (B, L, D, H, W), points (B, N, nd+1) with the label index interpolated (and clamped) as an
+ * (nd+1)-th axis; out (B, N) = |interp(sdt, q)|.  Backward: grad_points (B, N, nd+1) = grad_out * sign(v) * d interp/dq
+ * over the spatial columns (sign(0) = 0), 0 in the label column (overwritten). */
+size_t vxm_point_warp_workspace_bytes(int B, int N, int D, int H, int W, int nd);
+int vxm_point_warp_fwd(const float* points, const float* flow, float* out, int B, int N, int D, int H, int W, int nd,
+                       float r, void* stream);
+int vxm_point_warp_bwd(const float* points, const float* grad_out, float* grad_flow, void* work, size_t work_bytes,
+                       int B, int N, int D, int H, int W, int nd, float r, void* stream);
+int vxm_value_at_fwd(const float* sdt, const float* points, float* out, int B, int N, int L, int D, int H, int W,
+                     int nd, void* stream);
+int vxm_value_at_bwd(const float* sdt, const float* points, const float* grad_out, float* grad_points, int B, int N,
+                     int L, int D, int H, int W, int nd, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

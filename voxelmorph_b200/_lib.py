@@ -112,6 +112,11 @@ SIGNATURES = {
     "vxm_mi_workspace_bytes": (c_sz, [c_i, c_sz, c_i]),
     "vxm_mi_fwd": (c_i, [c_f] * 6 + [c_i, c_sz, c_i, c_fl, c_fl, c_fl, c_f]),
     "vxm_mi_bwd": (c_i, [c_f] * 7 + [c_i, c_sz, c_i, c_fl, c_fl, c_fl, c_f]),
+    "vxm_point_warp_workspace_bytes": (c_sz, [c_i] * 6),
+    "vxm_point_warp_fwd": (c_i, [c_f] * 3 + [c_i] * 6 + [c_fl, c_f]),
+    "vxm_point_warp_bwd": (c_i, [c_f] * 4 + [c_sz] + [c_i] * 6 + [c_fl, c_f]),
+    "vxm_value_at_fwd": (c_i, [c_f] * 3 + [c_i] * 7 + [c_f]),
+    "vxm_value_at_bwd": (c_i, [c_f] * 4 + [c_i] * 7 + [c_f]),
 }
 
 _lib = None

@@ -274,4 +274,82 @@ __device__ __forceinline__ FastCell<IS3D> fast_cell(float cz, float cy, float cx
   return c;
 }
 
+// ------------------------------------------------------------------------------------------------------------
+// Clamped mode: neurite's ne.utils.interpn(vol, loc, 'linear', fill_value=None), which the reference's surface
+// utilities sample with (voxelmorph/tf/utils/utils.py:71-88, 465-499).  Per axis of size n at coordinate x:
+//   c = clip(x, 0, n-1),  i0 = clip(floor(x), 0, n-1),  i1 = clip(i0 + 1, 0, n-1),
+//   weight (i1 - c) on i0 and 1 - (i1 - c) on i1; the axis weights multiply.
+// Outside the volume the value is the border value.  d/dx is the cell's difference along the axis where
+// 0 <= x <= n-1 (both ends included: the clip passes its gradient there) and 0 elsewhere; at an integer k < n-1 that
+// is the forward difference v[k+1] - v[k], at n-1 it is 0 (i0 == i1).
+// ------------------------------------------------------------------------------------------------------------
+
+struct ClampTap {
+  int i0, i1;      // the two taps (equal on the last voxel)
+  float w0, w1;    // their weights
+  float pass;      // 1 where the clip passes the gradient, else 0
+};
+
+__device__ __forceinline__ ClampTap clamp_tap(float x, int n) {
+  ClampTap t;
+  const float hi = (float)(n - 1);
+  const float c = fminf(fmaxf(x, 0.f), hi);
+  t.i0 = (int)fminf(fmaxf(floorf(x), 0.f), hi);   // clip before the cast: wild coordinates stay in range
+  t.i1 = min(t.i0 + 1, n - 1);
+  t.w0 = (float)t.i1 - c;
+  t.w1 = 1.f - t.w0;
+  t.pass = (x >= 0.f && x <= hi) ? 1.f : 0.f;
+  return t;
+}
+
+// The clamped cell of one point over an (D, H, W) plane (2-D: D == 1, only the y and x taps are read).  Corners are
+// numbered as in the other cells: bit0 = x+1, bit1 = y+1, bit2 = z+1; every corner is inside the volume.
+template <bool IS3D>
+struct ClampCell {
+  ClampTap tz, ty, tx;
+  int W, HW;
+
+  __device__ __forceinline__ int off(int k) const {
+    const int z = IS3D ? ((k & 4) ? tz.i1 : tz.i0) : 0, y = (k & 2) ? ty.i1 : ty.i0, x = (k & 1) ? tx.i1 : tx.i0;
+    return z * HW + y * W + x;
+  }
+  // (z-weight * y-weight) * x-weight: interpn's product in axis order
+  __device__ __forceinline__ float weight(int k) const {
+    const float wy = (k & 2) ? ty.w1 : ty.w0, wx = (k & 1) ? tx.w1 : tx.w0;
+    return IS3D ? (((k & 4) ? tz.w1 : tz.w0) * wy) * wx : wy * wx;
+  }
+  __device__ __forceinline__ float value(const float* __restrict__ plane) const {
+    float v = 0.f;
+#pragma unroll
+    for (int k = 0; k < (IS3D ? 8 : 4); ++k) v = fmaf(weight(k), __ldg(plane + off(k)), v);
+    return v;
+  }
+  // d(value)/d(coordinate), scaled by s, added to (gz, gy, gx)
+  __device__ __forceinline__ void grad(const float* __restrict__ plane, float s, float& gz, float& gy, float& gx) const {
+    float dz = 0.f, dy = 0.f, dx = 0.f;
+#pragma unroll
+    for (int k = 0; k < (IS3D ? 8 : 4); ++k) {
+      const float v = __ldg(plane + off(k));
+      const float wz = IS3D ? ((k & 4) ? tz.w1 : tz.w0) : 1.f, wy = (k & 2) ? ty.w1 : ty.w0, wx = (k & 1) ? tx.w1 : tx.w0;
+      dx = fmaf((k & 1) ? v : -v, wz * wy, dx);
+      dy = fmaf((k & 2) ? v : -v, wz * wx, dy);
+      if (IS3D) dz = fmaf((k & 4) ? v : -v, wy * wx, dz);
+    }
+    gx = fmaf(s * tx.pass, dx, gx);
+    gy = fmaf(s * ty.pass, dy, gy);
+    if (IS3D) gz = fmaf(s * tz.pass, dz, gz);
+  }
+};
+
+template <bool IS3D>
+__device__ __forceinline__ ClampCell<IS3D> clamp_cell(float cz, float cy, float cx, int D, int H, int W) {
+  ClampCell<IS3D> c;
+  c.tz = IS3D ? clamp_tap(cz, D) : ClampTap{0, 0, 1.f, 0.f, 0.f};
+  c.ty = clamp_tap(cy, H);
+  c.tx = clamp_tap(cx, W);
+  c.W = W;
+  c.HW = H * W;
+  return c;
+}
+
 }  // namespace vxm

@@ -26,7 +26,7 @@ from collections import OrderedDict
 import numpy as np
 
 __all__ = ["VolumeCache", "load_volfile", "volgen", "scan_to_scan", "scan_to_atlas", "semisupervised", "template_creation",
-           "conditional_template_creation", "hypermorph", "Prefetcher"]
+           "conditional_template_creation", "hypermorph", "surf_semisupervised", "Prefetcher"]
 
 
 def _cuda_ready():
@@ -353,6 +353,109 @@ def semisupervised(vol_names, seg_names, labels, atlas_file=None, downsize=2, pr
         if zeros is None:
             zeros = _zero_flow(1, src_vol.shape[1:-1], zeros_dtype)
         yield ([src_vol, trg_vol, src_seg], [trg_vol, zeros, trg_seg])
+
+
+def surf_semisupervised(vol_names, atlas_vol, atlas_seg, nb_surface_pts, labels=None, batch_size=1, surf_bidir=True,
+                        surface_pts_upsample_factor=2, smooth_seg_std=1, nb_labels_sample=None, sdt_vol_resize=1,
+                        align_segs=False, add_feat_axis=True, sdt_dtype=np.float32, pts_dtype=np.float32,
+                        zeros_dtype=np.float32, cache=None):
+    """Scan-to-atlas batches with surface targets for VxmDenseSemiSupervisedPointCloud (reference
+    generators.py:256-418): arguments, yield contract and np.random draws as the reference's.  Yields
+
+        ([subj, atlas, subj_sdt, atlas_sdt, subj_surf, atlas_surf], [atlas, subj, zero_flow, zeros, zeros])
+
+    or, without `surf_bidir`, ([subj, atlas, subj_sdt, atlas_surf], [atlas, subj, zero_flow, zeros]); arrays are
+    channel-last: SDTs (B, *sdt_shape, nb_labels_sample), surfaces (B, nb_surface_pts, nd + 1) with the label slot in
+    the last column, zeros (B, nb_surface_pts, 1).  Per label the segmentation is cleaned (pyutils.clean_seg), its
+    signed distance transform taken and points drawn on its surface; with nb_labels_sample below the label count a
+    random subset of labels is drawn per batch.  Batch size 1 only, like the reference.
+
+    The reference yields float64; `sdt_dtype`, `pts_dtype` and `zeros_dtype` (float32 by default) choose the output
+    types, the computation stays float64 (38 labels at 160x192x224 are 2.1 GB of SDTs per batch in float32).  The
+    reference's quirk is kept: the atlas SDT stacked for a sampled label is that of its position in the sample, not of
+    the label itself (generators.py:384)."""
+    from . import pyutils
+    assert nb_surface_pts > 0, 'number of surface point should be greater than 0'
+    vol_shape = atlas_seg.shape
+    nd = len(vol_shape)
+    sdt_shape = [int(f * sdt_vol_resize) for f in vol_shape]
+    if labels is not None:
+        atlas_seg = pyutils.filter_labels(atlas_seg, labels)
+    else:
+        labels = np.sort(np.unique(atlas_seg))[1:]
+    nb_labels = len(labels)
+    if nb_labels_sample is None:
+        nb_labels_sample = nb_labels
+    sample = nb_labels_sample != nb_labels
+
+    atlas_vol_bs = np.repeat(atlas_vol[np.newaxis, ..., np.newaxis], batch_size, axis=0)
+    atlas_seg_bs = np.repeat(atlas_seg[np.newaxis, ..., np.newaxis], batch_size, axis=0)
+
+    def surf_pts(sdt, n):
+        return pyutils.sdt_to_surface_pts(sdt, n, surface_pts_upsample_factor=surface_pts_upsample_factor,
+                                          thr=(1 / surface_pts_upsample_factor + 1e-5))
+
+    zero_flow = np.zeros((batch_size, *vol_shape, nd), dtype=zeros_dtype)
+    zero_values = np.zeros((batch_size, nb_surface_pts, 1), dtype=zeros_dtype)
+
+    atlas_sdt = []
+    nb_edges = np.zeros(nb_labels)
+    for li, label in enumerate(labels):
+        atlas_sdt.append(pyutils.vol_to_sdt(pyutils.clean_seg(atlas_seg == label, smooth_seg_std), sdt=True,
+                                            sdt_vol_resize=sdt_vol_resize))
+        nb_edges[li] = np.sum(np.abs(atlas_sdt[li]) < 1.01)
+    edge_ratios = nb_edges / np.sum(nb_edges)
+
+    def slot(counts, li):
+        return slice(int(np.sum(counts[:li])), int(np.sum(counts[:li + 1])))
+
+    atlas_surf = np.zeros((batch_size, nb_surface_pts, nd + 1), dtype=pts_dtype)
+    if not sample:
+        counts = pyutils.get_surface_pts_per_label(nb_surface_pts, edge_ratios)
+        for li in range(nb_labels):
+            s = slot(counts, li)
+            atlas_surf[:, s, :-1] = surf_pts(atlas_sdt[li], counts[li])[np.newaxis]
+            atlas_surf[:, s, -1] = li
+
+    gen = volgen(vol_names, segs=True, batch_size=batch_size, add_feat_axis=add_feat_axis, cache=cache)
+    assert batch_size == 1, 'only batch size 1 supported for now'
+
+    while True:
+        X_img, X_lab = next(gen)
+        X_seg = pyutils.filter_labels(X_lab, labels)
+        sel = range(nb_labels)
+        if sample:
+            sel = np.sort(np.random.choice(range(nb_labels), size=nb_labels_sample, replace=False))
+            counts = pyutils.get_surface_pts_per_label(nb_surface_pts, [edge_ratios[li] for li in sel])
+            atlas_surf = np.zeros((batch_size, nb_surface_pts, nd + 1), dtype=pts_dtype)
+        subj_sdt = np.zeros((batch_size, *sdt_shape, nb_labels_sample), dtype=sdt_dtype)
+        atl_sdt = np.zeros((batch_size, *sdt_shape, nb_labels_sample), dtype=sdt_dtype)
+        subj_surf = np.zeros((batch_size, nb_surface_pts, nd + 1), dtype=pts_dtype)
+
+        for li, sli in enumerate(sel):
+            s = slot(counts, li)
+            if sample:
+                atlas_surf[:, s, :-1] = surf_pts(atlas_sdt[sli], counts[li])[np.newaxis]
+                atlas_surf[:, s, -1] = sli
+            label_bw = pyutils.clean_seg_batch(X_seg == labels[sli], smooth_seg_std)
+            sdt = pyutils.vol_to_sdt_batch(label_bw, sdt=True, sdt_vol_resize=sdt_vol_resize)[..., 0]
+            subj_sdt[..., li] = sdt
+            if surf_bidir:
+                atl_sdt[..., li] = atlas_sdt[li][np.newaxis]
+                subj_surf[:, s, :-1] = np.stack([surf_pts(f, counts[li]) for f in sdt], 0)
+                subj_surf[:, s, -1] = li
+
+        X_ret, atlas_ret = X_img, atlas_vol_bs
+        if align_segs:
+            assert nb_labels == 1, 'align_seg generator is only implemented for single label'
+            X_ret = X_seg == labels[0]
+            atlas_ret = atlas_seg_bs == labels[0]
+
+        if surf_bidir:
+            yield ([X_ret, atlas_ret, subj_sdt, atl_sdt, subj_surf, atlas_surf],
+                   [atlas_ret, X_ret, zero_flow, zero_values, zero_values])
+        else:
+            yield ([X_ret, atlas_ret, subj_sdt, atlas_surf], [atlas_ret, X_ret, zero_flow, zero_values])
 
 
 class Prefetcher:

@@ -552,3 +552,97 @@ class HyperWeights(nn.Module):
     def views(self, wflat):
         """[(weight, bias)] views of a flat layout, in the order of `shapes`."""
         return [(wflat[ow:ob].view(s), wflat[ob:ob + s[0]]) for s, (ow, ob) in zip(self.shapes, self.offsets)]
+
+
+def _surface_dims(points, vol, what, vol_name):
+    """(B, N, nd, C, D, H, W) of points (B, N, nd+1) and a (B, C, [D,] H, W) volume, or VxmError."""
+    _lib.require_cuda(points, vol, what=what)
+    if vol.dim() not in (4, 5):
+        raise _lib.VxmError("%s: %s must be (B, C, H, W) or (B, C, D, H, W), got shape %s"
+                            % (what, vol_name, tuple(vol.shape)))
+    B, C, D, H, W, nd = _dims(vol)
+    if points.dim() != 3 or points.shape[0] != B or points.shape[2] != nd + 1 or points.shape[1] < 1:
+        raise _lib.VxmError("%s: points must be (B, N, nd + 1) = (%d, N, %d) for %s %s, got shape %s"
+                            % (what, B, nd + 1, vol_name, tuple(vol.shape), tuple(points.shape)))
+    return B, points.shape[1], nd, C, D, H, W
+
+
+class _PointWarpFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, points, flow, r):
+        B, N, nd, C, D, H, W = _surface_dims(points, flow, "point_spatial_transformer", "flow")
+        if C != nd:
+            raise _lib.VxmError("point_spatial_transformer: flow must have %d channels, got %d" % (nd, C))
+        points, flow = _lib.contig(points), _lib.contig(flow)
+        out = torch.empty_like(points)
+        _lib.check(_lib.load().vxm_point_warp_fwd(_lib.ptr(points), _lib.ptr(flow), _lib.ptr(out), B, N, D, H, W, nd,
+                                                  r, _lib.stream_ptr()), "vxm_point_warp_fwd")
+        ctx.save_for_backward(points)
+        ctx.cfg = (B, N, D, H, W, nd, r, flow.shape)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        if not ctx.needs_input_grad[1]:
+            return None, None, None
+        (points,) = ctx.saved_tensors
+        B, N, D, H, W, nd, r, fshape = ctx.cfg
+        lib = _lib.load()
+        nbytes = int(lib.vxm_point_warp_workspace_bytes(B, N, D, H, W, nd))
+        if nbytes == 0:
+            raise _lib.VxmError("point_spatial_transformer: no workspace for B=%d, N=%d, volume %s: %s"
+                                % (B, N, tuple(fshape[2:]), _lib.last_error()))
+        work = torch.empty(nbytes, dtype=torch.uint8, device=points.device)
+        gflow = torch.zeros(fshape, dtype=torch.float32, device=points.device)
+        _lib.check(lib.vxm_point_warp_bwd(_lib.ptr(points), _lib.ptr(_lib.contig(gout)), _lib.ptr(gflow),
+                                          _lib.ptr(work), nbytes, B, N, D, H, W, nd, r, _lib.stream_ptr()),
+                   "vxm_point_warp_bwd")
+        return None, gflow, None
+
+
+class _ValueAtFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, sdt, points):
+        B, N, nd, L, D, H, W = _surface_dims(points, sdt, "value_at_location", "sdt")
+        sdt, points = _lib.contig(sdt), _lib.contig(points)
+        out = torch.empty((B, N, 1), dtype=torch.float32, device=sdt.device)
+        _lib.check(_lib.load().vxm_value_at_fwd(_lib.ptr(sdt), _lib.ptr(points), _lib.ptr(out), B, N, L, D, H, W, nd,
+                                                _lib.stream_ptr()), "vxm_value_at_fwd")
+        ctx.save_for_backward(sdt, points)
+        ctx.cfg = (B, N, L, D, H, W, nd)
+        return out
+
+    @staticmethod
+    def backward(ctx, gout):
+        if not ctx.needs_input_grad[1]:
+            return None, None
+        sdt, points = ctx.saved_tensors
+        B, N, L, D, H, W, nd = ctx.cfg
+        gpts = torch.empty_like(points)
+        _lib.check(_lib.load().vxm_value_at_bwd(_lib.ptr(sdt), _lib.ptr(points), _lib.ptr(_lib.contig(gout)),
+                                                _lib.ptr(gpts), B, N, L, D, H, W, nd, _lib.stream_ptr()),
+                   "vxm_value_at_bwd")
+        return None, gpts
+
+
+def point_spatial_transformer(points, flow, sdt_vol_resize=1):
+    """Move surface points with a displacement field (reference voxelmorph/tf/utils/utils.py:465-499).
+
+    points (B, N, nd+1): spatial coordinates in the flow's axis order, the last column a label index (passed through);
+    flow (B, nd, *S).  Returns p + r * interp(flow, p) with r = sdt_vol_resize and neurite's clamped linear interpn
+    (a point outside the volume reads the border).  A field that moves image A onto B is defined on B's grid, so it
+    moves points of B onto A.  Only `flow` is differentiated (deterministically, see include/vxm_b200.h); `points`
+    must not require a gradient."""
+    if points.requires_grad:
+        raise _lib.VxmError("point_spatial_transformer: points must not require a gradient")
+    return _PointWarpFn.apply(points, flow, float(sdt_vol_resize))
+
+
+def value_at_location(sdt, points):
+    """|sdt| at the points (reference voxelmorph/tf/utils/utils.py:71-88 with force_post_absolute_val): sdt
+    (B, L, *S), points (B, N, nd+1) whose last column is the label channel, interpolated as an (nd+1)-th axis like the
+    others.  Returns (B, N, 1).  Only `points` is differentiated (sign(v) times the spatial gradient, 0 for the label
+    column); `sdt` must not require a gradient."""
+    if sdt.requires_grad:
+        raise _lib.VxmError("value_at_location: sdt must not require a gradient")
+    return _ValueAtFn.apply(sdt, points)

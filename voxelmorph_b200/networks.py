@@ -396,6 +396,99 @@ class VxmDenseSemiSupervisedSeg(LoadableModel):
         return layers.SpatialTransformer(tuple(img.shape[2:]), mode=mode)(img, flow)
 
 
+class VxmDenseSemiSupervisedPointCloud(LoadableModel):
+    """VoxelMorph network for registration aided by surface points (Dalca et al., "Unsupervised learning of
+    probabilistic diffeomorphic registration for images and surfaces", MedIA 2019).
+
+    The torch backend of the reference has no such class; the semantics are those of its TensorFlow model
+    (voxelmorph/tf/networks.py:391-486).  A bidirectional VxmDense (`self.vxm_model`; a VxmDenseProbabilistic with
+    `use_probs`) registers source to target.  `pos_flow` moves the atlas surface points into subject space and
+    `neg_flow` the subject's into atlas space (layers.point_spatial_transformer); each side's signed distance
+    transform (SDT) is read at the other side's moved points (layers.value_at_location), and a loss drives those
+    distances to zero:
+
+        y_source, y_target, flow, subj_dt_value, atl_dt_value = model(source, target, subj_dt, atl_dt,
+                                                                       subj_surf, atl_surf)
+
+    `flow` is preint_flow (or flow_params with use_probs).  SDTs are (B, nb_labels_sample, *sdt_shape) with
+    sdt_shape = int(inshape * sdt_vol_resize); surfaces are (B, nb_surface_points, nd + 1), the last column the SDT
+    channel.  Without `surf_bidir` the call is model(source, target, subj_dt, atl_surf) and atl_dt_value is dropped.
+
+    As in the reference (voxelmorph/tf/utils/utils.py:480-493), with sdt_vol_resize != 1 the full-resolution flow,
+    scaled by sdt_vol_resize, is sampled at the points' SDT-space coordinates, not at the matching full-resolution
+    ones.  Checkpoint keys are `vxm_model.*`; `kwargs` are forwarded to the inner model."""
+
+    @store_config_args
+    def __init__(self, inshape, nb_surface_points, nb_labels_sample, nb_unet_features=None, sdt_vol_resize=1,
+                 surf_bidir=True, use_probs=False, **kwargs):
+        super().__init__()
+        self.nb_surface_points = int(nb_surface_points)
+        self.nb_labels_sample = int(nb_labels_sample)
+        self.sdt_vol_resize = sdt_vol_resize
+        self.surf_bidir = bool(surf_bidir)
+        self.use_probs = bool(use_probs)
+        self.sdt_shape = tuple(int(f * sdt_vol_resize) for f in inshape)
+        cls = VxmDenseProbabilistic if use_probs else VxmDense
+        self.vxm_model = cls(inshape, nb_unet_features=nb_unet_features, bidir=True, **kwargs)
+
+    def _check_surface(self, sdt, surf, sdt_name, surf_name):
+        B = sdt.shape[0]
+        want_sdt = (B, self.nb_labels_sample) + self.sdt_shape
+        want_surf = (B, self.nb_surface_points, len(self.sdt_shape) + 1)
+        if tuple(sdt.shape) != want_sdt:
+            raise _lib.VxmError("VxmDenseSemiSupervisedPointCloud: %s must be %s, got %s"
+                                % (sdt_name, want_sdt, tuple(sdt.shape)))
+        if tuple(surf.shape) != want_surf:
+            raise _lib.VxmError("VxmDenseSemiSupervisedPointCloud: %s must be %s, got %s"
+                                % (surf_name, want_surf, tuple(surf.shape)))
+
+    def forward(self, source, target, *surface, registration=False):
+        vm = self.vxm_model
+        if registration:
+            return vm(source, target, registration=True)
+        if len(surface) != (4 if self.surf_bidir else 2):
+            raise TypeError("VxmDenseSemiSupervisedPointCloud.forward takes (source, target, %s)"
+                            % ("subj_dt, atl_dt, subj_surf, atl_surf" if self.surf_bidir else "subj_dt, atl_surf"))
+        if self.surf_bidir:
+            subj_dt, atl_dt, subj_surf, atl_surf = surface
+            self._check_surface(atl_dt, subj_surf, "atl_dt", "subj_surf")
+        else:
+            subj_dt, atl_surf = surface
+        self._check_surface(subj_dt, atl_surf, "subj_dt", "atl_surf")
+        vm._maybe_attach_dp()
+        if self.use_probs:
+            flow_out = vm._head(source, target)
+            pos_flow, neg_flow, _ = vm._integrate(layers.sample_normal_logvar(flow_out, vm.noise_state))
+        else:
+            pos_flow, neg_flow, flow_out = vm.flows(source, target)
+        y_source = vm.transformer(source, pos_flow)
+        y_target = vm.transformer(target, neg_flow)
+        r = self.sdt_vol_resize
+        subj_dt_value = layers.value_at_location(subj_dt, layers.point_spatial_transformer(atl_surf, pos_flow, r))
+        outs = (y_source, y_target, flow_out, subj_dt_value)
+        if self.surf_bidir:
+            atl_dt_value = layers.value_at_location(atl_dt, layers.point_spatial_transformer(subj_surf, neg_flow, r))
+            outs += (atl_dt_value,)
+        return outs
+
+    def save(self, path):
+        dp = self.vxm_model._dp
+        if dp is not None and not dp.is_writer():
+            return
+        super().save(path)
+
+    def register(self, source, target):
+        """The transform from source to target (full resolution; the mean's with use_probs), like tf register."""
+        with torch.no_grad():
+            return self.vxm_model(source, target, registration=True)[1]
+
+    def apply_transform(self, source, target, img, interp_method='linear'):
+        """Predict the transform from source to target and apply it to `img` ('linear' or 'nearest')."""
+        mode = 'bilinear' if interp_method == 'linear' else interp_method
+        flow = self.register(source, target)
+        return layers.SpatialTransformer(tuple(img.shape[2:]), mode=mode)(img, flow)
+
+
 class TemplateCreation(LoadableModel):
     """VoxelMorph network to learn an unconditional template (atlas) image.
 

@@ -14,7 +14,9 @@ from .utils import count_folds, dice, jacobian_determinant  # noqa: F401  (re-ex
 
 __all__ = ["default_unet_features", "get_backend", "read_file_list", "read_pair_list", "load_volfile", "save_volfile",
            "load_labels", "load_pheno_csv", "pad", "resize", "dice", "filter_labels", "affine_shift_to_matrix",
-           "jacobian_determinant", "count_folds"]
+           "jacobian_determinant", "count_folds", "extract_largest_vol", "clean_seg", "clean_seg_batch", "dist_trf",
+           "signed_dist_trf", "vol_to_sdt", "vol_to_sdt_batch", "get_surface_pts_per_label", "edge_to_surface_pts",
+           "sdt_to_surface_pts"]
 
 
 def default_unet_features():
@@ -205,3 +207,103 @@ def affine_shift_to_matrix(trf, resize=None, unshift_shape=None):
         to_centre[:3, 3] = (np.asarray(unshift_shape, dtype=float) - 1) / 2
         m = to_centre @ m @ np.linalg.inv(to_centre)
     return m
+
+
+# ---- surface targets of VxmDenseSemiSupervisedPointCloud (py/utils.py:308-470), on scipy.ndimage alone ----
+
+def extract_largest_vol(bw, connectivity=1):
+    """The largest connected component of a binary image (py/utils.py:308-318).  Components are labelled in raster
+    order with `connectivity` (1: faces), as skimage's measure.label numbers them; ties in size go to the component
+    np.argsort(areas)[::-1] puts first."""
+    from scipy import ndimage
+    bw = np.asarray(bw).astype(int)
+    lab, n = ndimage.label(bw, structure=ndimage.generate_binary_structure(bw.ndim, connectivity))
+    areas = np.bincount(lab.ravel(), minlength=n + 1)[1:]
+    return lab == np.argsort(areas)[::-1][0] + 1
+
+
+def clean_seg(x, std=1):
+    """Clean a binary segmentation (py/utils.py:321-337): keep the largest island, fill the holes, blur with a
+    Gaussian of sigma `std` and threshold the blur so that the volume is kept.  Returns float64 0 / 1."""
+    from scipy import ndimage
+    bw = extract_largest_vol(x)
+    bw = 1 - extract_largest_vol(1 - bw)
+    blur = ndimage.gaussian_filter(bw.astype(float), std)
+    k = int(np.ceil(bw.sum()))
+    flat = blur.ravel()
+    thr = np.partition(flat, flat.size - 1 - k)[flat.size - 1 - k]     # the (k+1)-th largest value
+    clean = blur > thr
+    assert np.isclose(bw.sum(), clean.sum(), atol=5), 'cleaning segmentation failed'
+    return clean.astype(float)
+
+
+def clean_seg_batch(X_label, std=1):
+    """clean_seg of every (*vol, 1) item of a batch (py/utils.py:340-351); float64 (B, *vol, 1)."""
+    X_label = np.asarray(X_label)
+    out = np.zeros(X_label.shape)
+    for i, x in enumerate(X_label):
+        out[i, ..., 0] = clean_seg(x[..., 0], std)
+    return out
+
+
+def dist_trf(bwvol):
+    """Euclidean distance of every voxel to the nearest True voxel (py/utils.py:364-369)."""
+    from scipy import ndimage
+    return ndimage.distance_transform_edt(np.logical_not(bwvol))
+
+
+def signed_dist_trf(bwvol):
+    """Signed distance to the surface of a binary image, positive outside and negative inside; no voxel is 0
+    (py/utils.py:372-391)."""
+    outside = np.logical_not(bwvol)
+    return dist_trf(bwvol) * outside - dist_trf(outside) * bwvol
+
+
+def vol_to_sdt(X_label, sdt=True, sdt_vol_resize=1):
+    """Signed distance transform of a binary volume, zoomed by `sdt_vol_resize` (linear, 'reflect'); its absolute
+    value unless `sdt` (py/utils.py:394-410)."""
+    from scipy import ndimage
+    X_dt = signed_dist_trf(X_label)
+    if sdt_vol_resize != 1:
+        factors = list(sdt_vol_resize) if isinstance(sdt_vol_resize, (list, tuple)) else [sdt_vol_resize] * X_dt.ndim
+        if any(f != 1 for f in factors):
+            X_dt = ndimage.zoom(X_dt, factors, order=1, mode='reflect')
+    return X_dt if sdt else np.abs(X_dt)
+
+
+def vol_to_sdt_batch(X_label, sdt=True, sdt_vol_resize=1):
+    """vol_to_sdt of every item of a (B, *vol, 1) batch (py/utils.py:413-424)."""
+    assert X_label.shape[-1] == 1, 'implemented assuming size is [batch_size, *vol_shape, 1]'
+    return np.stack([vol_to_sdt(x[..., 0], sdt=sdt, sdt_vol_resize=sdt_vol_resize) for x in X_label], 0)[..., np.newaxis]
+
+
+def get_surface_pts_per_label(total_nb_surface_pts, layer_edge_ratios):
+    """Split a point budget over labels in proportion to their edge counts, the last label taking the remainder
+    (py/utils.py:427-434)."""
+    n = np.round(np.array(layer_edge_ratios) * total_nb_surface_pts).astype('int')
+    n[-1] = total_nb_surface_pts - int(np.sum(n[:-1]))
+    return n
+
+
+def edge_to_surface_pts(X_edges, nb_surface_pts=None):
+    """Coordinates (P, nd) of the True voxels, or `nb_surface_pts` of them drawn with replacement
+    (np.random.choice, py/utils.py:437-449)."""
+    pts = np.stack(np.where(X_edges), 0).transpose()
+    if nb_surface_pts is not None:
+        pts = pts[np.random.choice(pts.shape[0], size=nb_surface_pts), :]
+    return pts
+
+
+def sdt_to_surface_pts(X_sdt, nb_surface_pts, surface_pts_upsample_factor=2, thr=0.50001, resize_fn=None):
+    """Surface points of a signed distance transform (py/utils.py:452-470): the SDT is upsampled (linear zoom,
+    'reflect', or `resize_fn`), voxels with |sdt| < thr are the surface, `nb_surface_pts` of them are drawn and
+    mapped back to the SDT's grid, coordinates scaled by (S - 1) / (S_up - 1) per axis."""
+    from scipy import ndimage
+    if resize_fn is None:
+        up = ndimage.zoom(X_sdt, [surface_pts_upsample_factor] * X_sdt.ndim, order=1, mode='reflect')
+    else:
+        up = resize_fn(X_sdt)
+        assert np.array_equal(np.array(X_sdt.shape) * surface_pts_upsample_factor, up.shape), 'resizing failed'
+    edges = np.abs(up) < thr
+    pts = edge_to_surface_pts(edges, nb_surface_pts=nb_surface_pts)
+    return np.stack([pts[..., d] * (X_sdt.shape[d] - 1) / (edges.shape[d] - 1) for d in range(X_sdt.ndim)], -1)
